@@ -4,22 +4,27 @@
 // Reference: CorrBlock.__init__ / CorrBlock.corr (src/modules/corr.py:25-41,67-76) —
 // torch.matmul (cuBLAS) writes level 0, then three F.avg_pool2d passes re-read the volume.
 //
-// Design (one CTA per SM, persistent, warp-specialised, 544 threads):
-//   warp 16     TMA producer: A tile = 128 source pixels x 128 channels (2 boxes of 64 ch,
-//               128B-swizzled, K-major) once per work item (edge, source tile, 8-row target band);
-//               B tile = an 8x16 patch of TARGET pixels x 128 channels (4-D tensor map
-//               (ch, x, y, slot) -> rows ordered y*16+x), 2-stage ring.  Out-of-image rows/cols are
-//               zero-filled by TMA.  Feature maps are indexed per edge on the device
-//               (slot1 = rig*ii, slot2 = rig*jj + (ii==jj)), so no gathered copies exist.
-//   warps 0-15  two consumer groups of two warpgroups; group g takes the x-tiles of parity g (B stage g),
-//               so one group's MMAs overlap the other's epilogue.  Each warpgroup issues 16 wgmma
-//               m64n64k16 (fp16 in, fp32 accumulate in registers) for its 64 rows of the 128x128 tile,
-//               rounds to fp16 and transposes the fragment through a small per-warp buffer so that a
-//               thread owns 4 rows x 16 columns of its source pixel's patch: level 0 as full-sector
-//               32-byte stores, levels 1-2 pooled in registers FROM THE ROUNDED finer level (the
-//               avg_pool2d numerics) and staged in shared memory per band; when the band's x-tiles are
-//               done the pooled rows (and level 3, pooled from the staged level 2) leave as long
-//               contiguous runs.  The volume is never re-read.
+// Design (one CTA per SM, persistent, warp-specialised, 384 threads = 3 warpgroups):
+//   warpgroup 2 TMA producer (one thread; the warpgroup drops to 40 registers with setmaxnreg):
+//               A tile = 128 source pixels x 128 channels (2 boxes of 64 ch, 128B-swizzled, K-major) once
+//               per work item (edge, source tile, 8-row target band); B tile = an 8x16 patch of TARGET
+//               pixels x 128 channels (4-D tensor map (ch, x, y, slot) -> rows ordered y*16+x), 2-stage
+//               ring.  Out-of-image rows/cols are zero-filled by TMA.  Feature maps are indexed per edge on
+//               the device (slot1 = rig*ii, slot2 = rig*jj + (ii==jj)), so no gathered copies exist.
+//               A is released as soon as the item's last MMAs retire, so the next item's A and B tiles
+//               load under the current epilogue and band write-out.
+//   warpgroups 0-1  consumers (232 registers each: the 128 fp32 accumulators and the epilogue stay in
+//               registers, no local memory); warpgroup g takes the x-tiles of parity g (B stage g), so
+//               one warpgroup's MMAs overlap the other's epilogue.  A warpgroup issues 32 wgmma m64n64k16
+//               (fp16 in, fp32 accumulate) for the whole 128x128 tile, then per m64 half rounds to fp16
+//               and transposes the fragment through a small per-warp buffer, 8 rows per pass.  Tiled
+//               level 0 leaves straight from that buffer as whole 128-byte lines (8 lanes per line, 4
+//               lines per warp store); each thread then owns 4 rows x 16 columns of its source pixel's
+//               patch (row-major level 0 as full-sector 32-byte stores), levels 1-2 are pooled in
+//               registers FROM THE ROUNDED finer level (the avg_pool2d numerics) and staged in shared
+//               memory per band; when the band's x-tiles are done the pooled rows (and level 3, pooled
+//               from the staged level 2) leave as contiguous runs (tiled: TMA bulk stores, asynchronous).
+//               The volume is never re-read.
 // Why the band staging: partial 32-byte-sector writes cost an ECC read-modify-write in L2.
 // The 1/4 feature scaling of the reference (`fmap / 4.0` in half) is applied by the K-major
 // re-layout prepass, exactly as the reference does it, so the accumulator needs no scaling.
@@ -42,10 +47,12 @@ constexpr int kPY = 8, kPX = 16;        // target patch
 constexpr int kKBox = 64;               // channels per TMA box (128 B)
 constexpr int kTileBytes = kBM * kD * 2;          // 32 KB (A or B tile)
 constexpr int kBoxBytes = kBM * kKBox * 2;        // 16 KB
-constexpr int kBStages = 2;                       // = the two consumer groups: group g owns B stage g
-constexpr int kGroupWarps = 8;                    // per consumer group: two warpgroups of 64 tile rows each
-constexpr int kEpiThreads = 2 * kGroupWarps * 32; // 512
-constexpr int kThreadsTC = kEpiThreads + 32;      // + the TMA producer warp
+constexpr int kBStages = 2;                       // = the two consumer warpgroups: warpgroup g owns B stage g
+constexpr int kGroupWarps = 4;                    // per consumer warpgroup: all 128 tile rows, as two m64 halves
+constexpr int kEpiThreads = 2 * kGroupWarps * 32; // 256
+constexpr int kThreadsTC = kEpiThreads + 128;     // + the TMA producer warpgroup
+// register reallocation: 128 x 40 + 256 x 232 <= 65,536 (the producer needs few, the accumulators many)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kMaxXB = 8;                                // x-tiles per band (w <= 128)
 constexpr int kPoolMax = kBM * ((4 * kMaxXB * 16 + 16) + (2 * kMaxXB * 8 + 48));  // 90,112 B (level 1 | level 2 + 3 pieces)
 // per-warp transpose of the accumulator fragment: 8 tile rows x 128 fp16 columns, rows padded to 68 words
@@ -71,8 +78,6 @@ struct TcParams {
   int pitch2, pitch3;         // tiled: bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
   int aligned;                // w % 16 == 0 && h % 8 == 0: every store is a whole aligned sector run
   int experiment;             // profiling only: 1 = no output writes
-  int bulk;                   // tiled: pooled levels leave through bulk (TMA) stores, asynchronously
-  int pingpong;               // tiled: the two epilogue groups take turns in their level-0 store sections
 };
 
 // ---- packed fp16 rows live in registers as uint32 pairs (lo = even column) ----
@@ -148,15 +153,17 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    mbar_init(full_a, 1); mbar_init(empty_a, 1);
+    // A is released by every consumer warp once its last MMA of the item has retired
+    mbar_init(full_a, 1); mbar_init(empty_a, kEpiThreads / 32);
     for (int i = 0; i < kBStages; ++i) { mbar_init(&full_b[i], 1); mbar_init(&empty_b[i], kGroupWarps); }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == kEpiThreads / 32) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp >= kEpiThreads / 32) {
+    // ===================== TMA producer (one thread of the producer warpgroup) =====================
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kEpiThreads / 32 && lane == 0) {
       int aph = 0, bs = 0, bph = 0;
       for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
         const int yb = item % p.n_yb;
@@ -184,64 +191,71 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
       }
     }
   } else {
-    // ===================== consumers (warps 0..15): wgmma + epilogue, two groups of 8 =====================
-    const int group = warp >> 3;                  // takes the tiles of parity `group`, held in B stage `group`
-    const int wg_row = ((warp >> 2) & 1) * 64;    // first tile row of this warpgroup's m64 MMAs
-    const int wrow = wg_row + (warp & 3) * 16;    // first of the warp's 16 fragment rows
-    const int row = wrow + (lane & 15);           // row of the 128-row tile = source pixel (after the transpose)
+    // ===================== consumers (warps 0..7): wgmma + epilogue, two warpgroups =====================
+    setmaxnreg_inc<kConsumerRegs>();
+    const int group = warp >> 2;                  // takes the tiles of parity `group`, held in B stage `group`
     const int half = lane >> 4;                   // patch rows 4*half .. 4*half+3 (columns 64*half..)
-    const int etid = threadIdx.x;                 // 0..511
+    const int etid = threadIdx.x;                 // 0..255
     const int ts = group;
     uint32_t* xp = reinterpret_cast<uint32_t*>(smXp + warp * kXpWarpBytes);
     // band staging strides (bytes); the +16 / +8 pads make the per-source-pixel stride conflict-free
     const int p1row = p.n_xb * 16, p1src = 4 * p1row + 16;
-    const int p2row = p.n_xb * 8;   // (bulk mode keeps the level-3 piece behind the level-2 piece)
-    const int p2src = p.tiled ? p.pitch2 + (p.bulk ? 48 : 8) : 2 * p2row + 8;
+    const int p2row = p.n_xb * 8;   // (tiled: the level-3 piece is staged behind the level-2 piece)
+    const int p2src = p.tiled ? p.pitch2 + 48 : 2 * p2row + 8;
     unsigned char* pool1 = smPool;
     unsigned char* pool2 = smPool + kBM * p1src;
     const int h1 = p.h >> 1, w1 = p.w >> 1, h2 = p.h >> 2, w2 = p.w >> 2, h3 = p.h >> 3, w3 = p.w >> 3;
     const bool wr = p.experiment != 1;
     int aph = 0, bph = 0, tile = 0;
-    // ordered store sections (ping-pong): named barrier 4+g = "group g may store"; 256 waiters + 256 arrivers
-    if (p.pingpong && group == 1) asm volatile("bar.arrive 4, 512;" ::: "memory");
     for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
       const int yb = item % p.n_yb;
       const int mt = (item / p.n_yb) % p.n_mt;
       const int n = item / (p.n_yb * p.n_mt);
-      const int src = mt * kBM + row;
-      const bool src_ok = src < p.hw && wr;
       const int n_out = p.out_slot ? __ldg(p.out_slot + n) : n;
-      const long long plane_id = (long long)n_out * p.hw + src;
       const int y0 = yb * kPY;
       mbar_wait(full_a, aph);
       aph ^= 1;
+      bool a_held = true;
       for (int xb = 0; xb < p.n_xb; ++xb, ++tile) {
         if ((tile & (kBStages - 1)) != ts) continue;
         const int x0 = xb * kPX;
         mbar_wait(&full_b[ts], bph);
         bph ^= 1;
-        // 128 x 128 x 128 tile: this warpgroup's 64 rows, N = 128 as two m64n64 halves (columns 0-63 | 64-127)
-        float acc[2][32];
+        // 128 x 128 x 128 tile: two m64 row halves, N = 128 as two m64n64 halves (columns 0-63 | 64-127)
+        float acc[2][2][32];
         {
-          const uint32_t a_addr = smem_u32(smA) + wg_row * 128;
+          const uint32_t a_addr = smem_u32(smA);
           const uint32_t b_addr = smem_u32(smB + ts * kTileBytes);
           wgmma_fence();
 #pragma unroll
           for (int kb = 0; kb < kD / kKBox; ++kb) {
 #pragma unroll
             for (int k = 0; k < kKBox / 16; ++k) {
-              const uint64_t da = make_desc_sw128(a_addr + kb * kBoxBytes + k * 32);
               const uint64_t db = make_desc_sw128(b_addr + kb * kBoxBytes + k * 32);
               const uint32_t on = (kb | k) != 0 ? 1u : 0u;
-              wgmma_m64n64(acc[0], da, db, on);
-              wgmma_m64n64(acc[1], da, db + ((64 * 128) >> 4), on);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh) {
+                const uint64_t da = make_desc_sw128(a_addr + mh * 64 * 128 + kb * kBoxBytes + k * 32);
+                wgmma_m64n64(acc[mh][0], da, db, on);
+                wgmma_m64n64(acc[mh][1], da, db + ((64 * 128) >> 4), on);
+              }
             }
           }
           wgmma_commit();
           wgmma_wait<0>();
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_b[ts]);  // this warp's MMAs are done reading the B stage
+        if (lane == 0) {
+          mbar_arrive(&empty_b[ts]);                // this warp's MMAs are done reading the B stage
+          if (xb + kBStages >= p.n_xb) mbar_arrive(empty_a);  // ... and its last MMA of the item has retired
+        }
+        if (xb + kBStages >= p.n_xb) a_held = false;
+#pragma unroll
+        for (int mh = 0; mh < 2; ++mh) {
+        const int row = mh * 64 + (warp & 3) * 16 + (lane & 15);  // tile row = source pixel (after the transpose)
+        const int src = mt * kBM + row;
+        const bool src_ok = src < p.hw && wr;
+        const long long plane_id = (long long)n_out * p.hw + src;
         // fp16 rounding, then fragment -> (row, half) through the warp's transpose buffer, 8 rows per pass:
         // hr[R][x] = columns 64*half + 16R + 2x, 2x+1 of the thread's row (patch row 4*half + R)
         uint32_t hr[4][8];
@@ -252,8 +266,30 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
 #pragma unroll
             for (int j = 0; j < 8; ++j)
               xp[(lane >> 2) * kXpRowWords + sub * 32 + 4 * j + (lane & 3)] =
-                  pack2(acc[sub][4 * j + 2 * pass], acc[sub][4 * j + 2 * pass + 1]);
+                  pack2(acc[mh][sub][4 * j + 2 * pass], acc[mh][sub][4 * j + 2 * pass + 1]);
           __syncwarp();
+          if (p.tiled && wr) {
+            // level 0, tiled: the 16 rows x 2 halves staged in this pass are 16 whole 128-byte lines (four
+            // 4x4 tiles each); 8 lanes write one line, so every STG.128 of the warp fills 4 complete lines
+            const int c = lane & 7, t = c >> 1, r0 = 2 * (c & 1);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int li = 4 * i + (lane >> 3);
+              const int r = li & 7, hf = li >> 3;
+              const int lsrc = mt * kBM + mh * 64 + (warp & 3) * 16 + pass * 8 + r;
+              const int lty = 2 * yb + hf;
+              if (lsrc < p.hw && lty < p.h4_0 && xb * 4 + t < p.w4_0) {
+                const uint32_t* s = xp + r * kXpRowWords + hf * 32 + 2 * t;
+                const uint2 u = *reinterpret_cast<const uint2*>(s + 8 * r0);
+                const uint2 v = *reinterpret_cast<const uint2*>(s + 8 * (r0 + 1));
+                unsigned char* dst = reinterpret_cast<unsigned char*>(p.lvl[0]) +
+                                     ((((long long)n_out * p.hw + lsrc) * p.h4_0 + lty) * p.w4_0 + xb * 4 + t) * 32LL +
+                                     (c & 1) * 16;
+                asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(dst), "r"(u.x), "r"(u.y), "r"(v.x), "r"(v.y)
+                             : "memory");
+              }
+            }
+          }
           if (((lane >> 3) & 1) == pass) {
             const uint4* sp = reinterpret_cast<const uint4*>(xp + (lane & 7) * kXpRowWords + half * 32);
 #pragma unroll
@@ -267,28 +303,8 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
         }
         uint32_t l1[2][4];     // the two level-1 rows this thread produces (8 halves each)
         if (p.tiled) {
-          // ---- tiled layout: this thread's 4 patch rows x 16 columns are exactly four 4x4 tiles,
-          // adjacent in memory: one 128-byte run per thread (8 x STG.128) ----
-          const int ty = 2 * yb + half;
-          if (p.pingpong) {
-            if (group == 0) asm volatile("bar.sync 4, 512;" ::: "memory");
-            else asm volatile("bar.sync 5, 512;" ::: "memory");
-          }
-          if (src_ok && ty < p.h4_0) {
-            unsigned char* dst = reinterpret_cast<unsigned char*>(p.lvl[0]) +
-                                 ((plane_id * p.h4_0 + ty) * p.w4_0 + xb * 4) * 32LL;
-#pragma unroll
-            for (int t = 0; t < 4; ++t)
-              if (xb * 4 + t < p.w4_0)
-                asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(dst + t * 32),
-                             "r"(hr[0][2 * t]), "r"(hr[0][2 * t + 1]), "r"(hr[1][2 * t]), "r"(hr[1][2 * t + 1]),
-                             "r"(hr[2][2 * t]), "r"(hr[2][2 * t + 1]), "r"(hr[3][2 * t]), "r"(hr[3][2 * t + 1])
-                             : "memory");
-          }
-          if (p.pingpong) {                          // the other group's turn
-            if (group == 0) asm volatile("bar.arrive 5, 512;" ::: "memory");
-            else asm volatile("bar.arrive 4, 512;" ::: "memory");
-          }
+          // ---- tiled layout (level 0 left from the transpose buffer above): level 1 pooled from the
+          // thread's 4 patch rows x 16 columns ----
 #pragma unroll
           for (int cc = 0; cc < 2; ++cc) {
 #pragma unroll
@@ -325,19 +341,22 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           const uint32_t a1 = pack2(pool_pair(l1[0][2], l1[1][2]), pool_pair(l1[0][3], l1[1][3]));
           *reinterpret_cast<uint2*>(pool2 + row * p2src + half * p2row + xb * 8) = make_uint2(a0, a1);
         }
+        }
       }
-      // ---- band write-out: all 16 consumer warps have staged every x-tile of this 8-row band ----
-      if (p.bulk) fence_async_smem();            // staged rows become visible to the async (TMA) proxy
-      asm volatile("bar.sync 3, 512;" ::: "memory");
-      if (etid == 0) mbar_arrive(empty_a);       // every MMA of this item has retired: A may be reloaded
-      if (wr && p.num_levels > 1) {
-        const int s_loc = etid >> 2, part = etid & 3;          // four threads per source pixel
+      // a warp that had no tile in this item releases A here
+      if (a_held && lane == 0) mbar_arrive(empty_a);
+      // ---- band write-out: both consumer warpgroups have staged every x-tile of this 8-row band ----
+      if (p.tiled) fence_async_smem();           // staged rows become visible to the async (TMA) proxy
+      asm volatile("bar.sync 3, 256;" ::: "memory");
+      if (wr && p.num_levels > 1)
+      for (int s_loc = etid >> 2; s_loc < kBM; s_loc += kEpiThreads / 4) {
+        const int part = etid & 3;                             // four threads per source pixel
         const int s_glb = mt * kBM + s_loc;
         if (s_glb < p.hw) {
           const long long pl = (long long)n_out * p.hw + s_glb;
           const unsigned char* sp1 = pool1 + s_loc * p1src;
           const unsigned char* sp2 = pool2 + s_loc * p2src;
-          if (p.tiled && p.bulk) {
+          if (p.tiled) {
             // The staged pieces are byte-for-byte what goes to memory: hand them to the TMA engine
             // (one bulk copy per source pixel and level) and go back to draining accumulators; the
             // copies stream out while the next band's level-0 stores are being issued.
@@ -366,50 +385,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
             }
             bulk_commit();
             bulk_wait_read();                      // the staging rows may be overwritten after the next barrier
-          } else if (p.tiled) {
-            // level 1: one tile-row of 4x4 tiles = w4_1 contiguous sectors, already in tile order
-            if (yb < p.h4_1) {
-              unsigned char* g1 = reinterpret_cast<unsigned char*>(p.lvl[1]) +
-                                  ((pl * p.h4_1 + yb) * p.w4_1) * 32LL;
-              for (int off = part * 32; off < p.w4_1 * 32; off += 128) {
-                uint32_t rr[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) rr[k] = *reinterpret_cast<const uint32_t*>(sp1 + off + 4 * k);
-                asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(g1 + off), "r"(rr[0]),
-                             "r"(rr[1]), "r"(rr[2]), "r"(rr[3]), "r"(rr[4]), "r"(rr[5]), "r"(rr[6]), "r"(rr[7])
-                             : "memory");
-              }
-            }
-            // levels 2 / 3: one padded, sector-aligned piece per (source pixel, band): whole sectors only
-            if (part == 1 && p.num_levels > 2 && 2 * yb < h2) {
-              unsigned char* g2 = reinterpret_cast<unsigned char*>(p.lvl[2]) + (pl * p.n_yb + yb) * (long long)p.pitch2;
-              for (int off = 0; off < p.pitch2; off += 32) {
-                uint32_t rr[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) rr[k] = *reinterpret_cast<const uint32_t*>(sp2 + off + 4 * k);
-                asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(g2 + off), "r"(rr[0]),
-                             "r"(rr[1]), "r"(rr[2]), "r"(rr[3]), "r"(rr[4]), "r"(rr[5]), "r"(rr[6]), "r"(rr[7])
-                             : "memory");
-              }
-            }
-            if (part == 2 && p.num_levels > 3 && yb < h3) {
-              uint32_t rr[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {                    // level-3 columns 2k, 2k+1 of this band's row
-                rr[k] = 0u;
-                if (k < p.n_xb) {
-                  const uint32_t t = *reinterpret_cast<const uint32_t*>(sp2 + 8 * k);
-                  const uint32_t t2 = *reinterpret_cast<const uint32_t*>(sp2 + 8 * k + 4);
-                  const uint32_t b = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 8 * k);
-                  const uint32_t b2 = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 8 * k + 4);
-                  rr[k] = pack2(pool_pair(t, b), pool_pair(t2, b2));
-                }
-              }
-              unsigned char* g3 = reinterpret_cast<unsigned char*>(p.lvl[3]) + (pl * p.n_yb + yb) * 32LL;
-              asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(g3), "r"(rr[0]),
-                           "r"(rr[1]), "r"(rr[2]), "r"(rr[3]), "r"(rr[4]), "r"(rr[5]), "r"(rr[6]), "r"(rr[7])
-                           : "memory");
-            }
           } else
           if (p.aligned) {
             if (!p.tiled) {
@@ -474,9 +449,9 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           }
         }
       }
-      asm volatile("bar.sync 3, 512;" ::: "memory");
+      asm volatile("bar.sync 3, 256;" ::: "memory");
     }
-    if (p.bulk) bulk_wait_all();
+    if (p.tiled) bulk_wait_all();
   }
 }
 
@@ -539,12 +514,6 @@ EncodeTiledFn get_encode_fn() {
 
 #ifndef GOSLAM_TC_EXPERIMENT
 #define GOSLAM_TC_EXPERIMENT 0
-#endif
-#ifndef GOSLAM_TC_BULK
-#define GOSLAM_TC_BULK 0
-#endif
-#ifndef GOSLAM_TC_PINGPONG
-#define GOSLAM_TC_PINGPONG 0
 #endif
 // Tensor maps depend only on (base pointer, frame count, h, w): a factor graph builds from the same
 // video-level K-major buffer for its whole life, so the two cuTensorMapEncodeTiled driver calls per launch
@@ -619,12 +588,8 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
   p.pitch2 = (p.n_xb * 16 + 31) / 32 * 32; p.pitch3 = 32;
   p.aligned = (w % 16 == 0 && h % 8 == 0) ? 1 : 0;
-  // Build-time A/B switches (-DGOSLAM_TC_EXPERIMENT=1 ..., tools/ only): the shipped library has them all 0.
+  // Build-time switch (-DGOSLAM_TC_EXPERIMENT=1, profiling builds only): the shipped library has it at 0.
   p.experiment = GOSLAM_TC_EXPERIMENT;
-  // bulk (TMA) stores of the pooled levels are off by default: on the B200 version they were no
-  // faster than plain stores; not re-measured on the H100
-  p.bulk = (p.tiled && GOSLAM_TC_BULK) ? 1 : 0;
-  p.pingpong = (p.tiled && GOSLAM_TC_PINGPONG) ? 1 : 0;
   // per-device: opt-in shared memory + SM count, looked up once per device
   static int sm_count[64];
   static std::mutex dev_mu;
