@@ -16,15 +16,16 @@
 //   warpgroups 0-1  consumers (232 registers each: the 128 fp32 accumulators and the epilogue stay in
 //               registers, no local memory); warpgroup g takes the x-tiles of parity g (B stage g), so
 //               one warpgroup's MMAs overlap the other's epilogue.  A warpgroup issues 32 wgmma m64n64k16
-//               (fp16 in, fp32 accumulate) for the whole 128x128 tile, then per m64 half rounds to fp16
-//               and transposes the fragment through a small per-warp buffer, 8 rows per pass.  Tiled
-//               level 0 leaves straight from that buffer as whole 128-byte lines (8 lanes per line, 4
-//               lines per warp store); each thread then owns 4 rows x 16 columns of its source pixel's
-//               patch (row-major level 0 as full-sector 32-byte stores), levels 1-2 are pooled in
-//               registers FROM THE ROUNDED finer level (the avg_pool2d numerics) and staged in shared
-//               memory per band; when the band's x-tiles are done the pooled rows (and level 3, pooled
-//               from the staged level 2) leave as contiguous runs (tiled: TMA bulk stores, asynchronous).
-//               The volume is never re-read.
+//               (fp16 in, fp32 accumulate) for the whole 128x128 tile, then per m64 half rounds to fp16.
+//               Tiled layout: level 0 goes into swizzled staging with stmatrix, level 1 is pooled in
+//               registers from the rounded fragment and staged beside it, and one thread per warpgroup
+//               writes both with TMA tensor stores (tiled_half_epilogue); the consumers issue no global
+//               stores.  Row-major layout: the fragment is transposed through a small per-warp buffer,
+//               each thread then owns 4 rows x 16 columns of its source pixel's patch (level 0 as
+//               full-sector 32-byte stores) and pools level 1 in registers.  Both pool FROM THE ROUNDED
+//               finer level (the avg_pool2d numerics) and stage level 2 (row-major: also level 1) per band;
+//               when the band's x-tiles are done those rows (and level 3, pooled from the staged level 2)
+//               leave as contiguous runs (tiled: TMA bulk stores).  The volume is never re-read.
 // Why the band staging: partial 32-byte-sector writes cost an ECC read-modify-write in L2.
 // The 1/4 feature scaling of the reference (`fmap / 4.0` in half) is applied by the K-major
 // re-layout prepass, exactly as the reference does it, so the accumulator needs no scaling.
@@ -54,12 +55,35 @@ constexpr int kThreadsTC = kEpiThreads + 128;     // + the TMA producer warpgrou
 // register reallocation: 128 x 40 + 256 x 232 <= 65,536 (the producer needs few, the accumulators many)
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kMaxXB = 8;                                // x-tiles per band (w <= 128)
-constexpr int kPoolMax = kBM * ((4 * kMaxXB * 16 + 16) + (2 * kMaxXB * 8 + 48));  // 90,112 B (level 1 | level 2 + 3 pieces)
+// Shared memory, sized per launch from n_xb (the x-tiles of a band); offsets from a 1024-byte aligned base:
+//   item                                        tiled                    row-major
+//   mbarriers                                   1 KB                     1 KB
+//   A tile (128 source px x 128 ch)             32 KB                    32 KB
+//   B stages (2 x 128 target px x 128 ch)       64 KB                    64 KB
+//   level-0 staging (2 per warpgroup, m64)      4 x 16 KB                -
+//   level-1 staging (2 per warpgroup, m64)      4 x 4 KB                 128 x (64 n_xb + 16) B   (band pool)
+//   level-2/3 band pool                         128 x (pitch2 + 48) B    128 x (16 n_xb + 8) B
+//   per-warp transpose buffers                  -                        8 x 2,176 B
+//   + 1 KB of alignment slack.  At w = 128 (n_xb = 8): tiled 200 KB, row-major 198 KB (<= 227 KB).
+constexpr int kBarBytes = 1024;
+constexpr int kL0HalfBytes = 64 * 2 * 128;        // m64 half of a tile's level 0: 64 source px x 2 tile rows x 128 B
+constexpr int kL1HalfBytes = 64 * 64;             // ... of its level 1: 64 source px x one tile row of 2 tiles (64 B)
 // per-warp transpose of the accumulator fragment: 8 tile rows x 128 fp16 columns, rows padded to 68 words
 constexpr int kXpRowWords = 68;
 constexpr int kXpWarpBytes = 8 * kXpRowWords * 4;                                 // 2,176 B
-constexpr int kSmemTC = 1024 + (1 + kBStages) * kTileBytes + kPoolMax + kEpiThreads / 32 * kXpWarpBytes + 256;
-static_assert(kSmemTC <= 227 * 1024, "corr_build_tc_kernel exceeds the 227 KB of shared memory of a block");
+constexpr int kFixedBytes = 1024 + kBarBytes + (1 + kBStages) * kTileBytes;
+__host__ __device__ constexpr int pitch2_of(int n_xb) { return (n_xb * 16 + 31) / 32 * 32; }
+__host__ __device__ constexpr int pool2_src_bytes(bool tiled, int n_xb) {
+  return tiled ? pitch2_of(n_xb) + 48 : 2 * n_xb * 8 + 8;
+}
+__host__ __device__ constexpr int pool1_src_bytes(int n_xb) { return 4 * n_xb * 16 + 16; }
+__host__ __device__ constexpr int smem_bytes(bool tiled, int n_xb) {
+  return tiled ? kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + kBM * pool2_src_bytes(true, n_xb)
+               : kFixedBytes + kBM * (pool1_src_bytes(n_xb) + pool2_src_bytes(false, n_xb)) +
+                     kEpiThreads / 32 * kXpWarpBytes;
+}
+static_assert(smem_bytes(true, kMaxXB) <= 227 * 1024 && smem_bytes(false, kMaxXB) <= 227 * 1024,
+              "corr_build_tc_kernel exceeds the 227 KB of shared memory of a block");
 
 using namespace gs_tc;
 
@@ -72,11 +96,11 @@ struct TcParams {
   // slot1 = rig*ii[e], slot2 = rig*jj[e] + (ii[e]==jj[e])   (src/factor_graph.py:108-113,290)
   const int64_t* ii; const int64_t* jj; int rig;
   const int* out_slot;        // optional edge -> output slot of the level buffers (CorrPool)
-  // tiled = 1: levels 0 and 1 are stored as 4x4-element (32-byte) tiles, tile-row-major inside each
+  // tiled: levels 0 and 1 are stored as 4x4-element (32-byte) tiles, tile-row-major inside each
   // source pixel's plane (plane = H4*W4 tiles, padded with zeros); levels 2, 3 stay row-major.
-  int tiled, w4_0, h4_0, w4_1, h4_1;
+  int w4_0, h4_0, w4_1, h4_1;
   int pitch2, pitch3;         // tiled: bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
-  int aligned;                // w % 16 == 0 && h % 8 == 0: every store is a whole aligned sector run
+  int aligned;                // row-major: w % 16 == 0 && h % 8 == 0: every store is a whole aligned sector run
   int experiment;             // profiling only: 1 = no output writes
 };
 
@@ -133,18 +157,107 @@ __device__ __forceinline__ void store_row(__half* dst, const uint32_t (&r)[NW], 
   }
 }
 
+// Tiled epilogue of one m64 half of a 128x128 tile (this warp: 16 source rows x 128 target pixels, the
+// wgmma fragment acc[ty][.], ty = tile row of level 0 = columns 64ty..64ty+63 = patch rows 4ty..4ty+3).
+// Fragment: acc[ty][4j + 2rh + e] = source row 8rh + lane/4, patch row 4ty + j/2, x = 8(j%2) + 2(lane%4) + e.
+//   level 0 -> st0, the box (64 halves, 2 tile rows, 64 source px) of the level-0 tensor map, 128B-swizzled:
+//             smem row R = 2 src + ty holds tiles 0..3 of that tile row, 16-byte chunk 2t + r4/2 = rows
+//             r4, r4+1 of tile t.  A lane owns x pair (2q, 2q+1), q = 4(j%2) + lane%4, i.e. half of a chunk
+//             row; one shfl.xor(2) per two words completes the chunks, then stmatrix writes 8 rows x 16 B.
+//   level 1 -> st1, the box (32 halves, 1 tile row, 64 source px) of the level-1 tensor map, 64B-swizzled:
+//             the 2x2 pools of a lane's own x pair, rows 2k, 2k+1 (y1 = 2ty + k, x1 = q); one shfl.xor(1)
+//             pairs x1 columns into words.
+//   level 2 -> the band pool, from those level-1 words (y2 = lane parity).
+__device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], unsigned char* st0, unsigned char* st1,
+                                                    unsigned char* pool2_row0, int p2src, int p2row, int xb,
+                                                    int wrow, int lane) {
+  // packed rounded fp16 pairs: W[rh][ty][r4][jx] = x pair (8jx + 2(lane%4), +1) of patch row 4ty + r4
+  uint32_t W[2][2][4][2];
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+    for (int ty = 0; ty < 2; ++ty)
+#pragma unroll
+      for (int r4 = 0; r4 < 4; ++r4)
+#pragma unroll
+        for (int jx = 0; jx < 2; ++jx) {
+          const int j = 2 * r4 + jx;
+          W[rh][ty][r4][jx] = pack2(acc[ty][4 * j + 2 * rh], acc[ty][4 * j + 2 * rh + 1]);
+        }
+  // ---- level 0: 8 x stmatrix.x4 ----
+  // Matrix row s (source row 8rh + s) takes tile row ty = a ^ (s >> 2): the 8 rows of a matrix then land on
+  // 8 different swizzle phases (R & 7 = (2s + ty) & 7), so each matrix is one conflict-free wavefront.
+  {
+    const bool lo = (lane & 3) < 2;                // lanes holding tile 2jx (the others: tile 2jx + 1)
+    const bool dflip = (lane >> 4) & 1;            // data rows s = lane/4 >= 4
+    const int s8 = lane & 7;                       // address: row s8 of matrix lane/8 = (rh, tile parity)
+    const uint32_t st0_u = smem_u32(st0);
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+      for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int jx = 0; jx < 2; ++jx) {
+          uint32_t m[4];
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            const uint32_t ra = dflip ? W[rh][a ^ 1][2 * k][jx] : W[rh][a][2 * k][jx];
+            const uint32_t rb = dflip ? W[rh][a ^ 1][2 * k + 1][jx] : W[rh][a][2 * k + 1][jx];
+            const uint32_t recv = __shfl_xor_sync(0xffffffffu, lo ? rb : ra, 2);
+            m[2 * rh] = lo ? ra : recv;            // tile 2jx:     (r4 = 2k | 2k+1) x (x 0-1 | 2-3)
+            m[2 * rh + 1] = lo ? recv : rb;        // tile 2jx + 1
+          }
+          const int tya = a ^ (s8 >> 2);
+          const int R = 2 * (wrow + 8 * (lane >> 4) + s8) + tya;
+          const int chunk = 2 * (2 * jx + ((lane >> 3) & 1)) + k;
+          stmatrix_x4(st0_u + R * 128 + ((chunk ^ (R & 7)) << 4), m);
+        }
+  }
+  // ---- levels 1 and 2 ----
+  const bool ev = (lane & 1) == 0;                 // even lanes: level-1 rows 0, 1 and level-2 row 0
+  const uint32_t st1_u = smem_u32(st1);
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    const int s = wrow + 8 * rh + (lane >> 2);     // source row within the m64 half
+#pragma unroll
+    for (int jx = 0; jx < 2; ++jx) {
+      float v[4];                                  // level-1 rows y1 = 2ty + k at x1 = 4jx + lane%4
+#pragma unroll
+      for (int ty = 0; ty < 2; ++ty)
+#pragma unroll
+        for (int k = 0; k < 2; ++k) v[2 * ty + k] = pool_pair(W[rh][ty][2 * k][jx], W[rh][ty][2 * k + 1][jx]);
+      const uint32_t own01 = pack2(v[0], v[1]), own23 = pack2(v[2], v[3]);
+      const uint32_t recv = __shfl_xor_sync(0xffffffffu, ev ? own23 : own01, 1);
+      const uint32_t mine = ev ? own01 : own23;
+      const uint32_t lo_w = ev ? mine : recv, hi_w = ev ? recv : mine;   // even x1 column | odd x1 column
+      const uint32_t w0 = __byte_perm(lo_w, hi_w, 0x5410);              // row 2 * (lane & 1)
+      const uint32_t w1 = __byte_perm(lo_w, hi_w, 0x7632);              // row 2 * (lane & 1) + 1
+      // tile jx, rows y1 (8 B each), column pair (lane & 3) / 2; 16-byte chunk 2jx + y1/2, 64B swizzle
+      const int chunk = (2 * jx + (lane & 1)) ^ ((s >> 1) & 3);
+      const uint32_t a1 = st1_u + s * 64 + (chunk << 4) + ((lane & 3) >> 1) * 4;
+      // even lanes write row 0 first, odd lanes row 3 first: the two stores are conflict-free
+      st_shared_u32(a1 + (ev ? 0 : 8), ev ? w0 : w1);
+      st_shared_u32(a1 + (ev ? 8 : 0), ev ? w1 : w0);
+      // level 2: row (lane & 1) of the band, column 4xb + 2jx + (lane & 3) / 2
+      const uint32_t l2 = pack2(pool_pair(w0, w1), 0.f);
+      st_shared_u16(smem_u32(pool2_row0 + s * p2src + (lane & 1) * p2row + xb * 8 + (2 * jx + ((lane & 3) >> 1)) * 2),
+                    (uint16_t)(l2 & 0xffffu));
+    }
+  }
+}
+
+template <bool kTiled>
 __global__ void __launch_bounds__(kThreadsTC, 1)
-corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
-                     const __grid_constant__ CUtensorMap mapB, const TcParams p) {
+corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                     const __grid_constant__ CUtensorMap mapL0, const __grid_constant__ CUtensorMap mapL1,
+                     const TcParams p) {
   extern __shared__ unsigned char smem_raw[];
-  // 1024-byte alignment for the 128B swizzle atoms
-  unsigned char* base =
-      reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* smA = base;                                   // ONE A stage, reloaded once per band item
-  unsigned char* smB = base + kTileBytes;                      // [kBStages]
-  unsigned char* smPool = base + (1 + kBStages) * kTileBytes;
-  unsigned char* smXp = smPool + kPoolMax;                     // [16 consumer warps][kXpWarpBytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smXp + kEpiThreads / 32 * kXpWarpBytes);
+  // 1024-byte alignment for the 128B swizzle atoms (pointer arithmetic on smem_raw: stays in the shared window)
+  unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base);
+  unsigned char* smA = base + kBarBytes;                       // ONE A stage, reloaded once per band item
+  unsigned char* smB = smA + kTileBytes;                       // [kBStages]
+  unsigned char* smEpi = smB + kBStages * kTileBytes;
   uint64_t* full_a = bars;
   uint64_t* empty_a = bars + 1;
   uint64_t* full_b = bars + 2;                   // [kBStages]
@@ -194,18 +307,29 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
     // ===================== consumers (warps 0..7): wgmma + epilogue, two warpgroups =====================
     setmaxnreg_inc<kConsumerRegs>();
     const int group = warp >> 2;                  // takes the tiles of parity `group`, held in B stage `group`
-    const int half = lane >> 4;                   // patch rows 4*half .. 4*half+3 (columns 64*half..)
+    const int half = lane >> 4;                   // row-major: patch rows 4*half .. 4*half+3 (columns 64*half..)
     const int etid = threadIdx.x;                 // 0..255
     const int ts = group;
-    uint32_t* xp = reinterpret_cast<uint32_t*>(smXp + warp * kXpWarpBytes);
+    // tiled: level-0 / level-1 staging, two m64 halves per warpgroup, then the band pool (levels 2, 3)
+    unsigned char* smL0 = smEpi;
+    unsigned char* smL1 = smL0 + 2 * kBStages * kL0HalfBytes;
     // band staging strides (bytes); the +16 / +8 pads make the per-source-pixel stride conflict-free
-    const int p1row = p.n_xb * 16, p1src = 4 * p1row + 16;
+    const int p1row = p.n_xb * 16, p1src = pool1_src_bytes(p.n_xb);
     const int p2row = p.n_xb * 8;   // (tiled: the level-3 piece is staged behind the level-2 piece)
-    const int p2src = p.tiled ? p.pitch2 + 48 : 2 * p2row + 8;
-    unsigned char* pool1 = smPool;
-    unsigned char* pool2 = smPool + kBM * p1src;
+    const int p2src = pool2_src_bytes(kTiled, p.n_xb);
+    unsigned char* pool1 = smEpi;                 // row-major only
+    unsigned char* pool2 = kTiled ? smL1 + 2 * kBStages * kL1HalfBytes : pool1 + kBM * p1src;
+    unsigned char* smXp = pool2 + kBM * p2src;    // row-major only: [8 consumer warps][kXpWarpBytes]
+    uint32_t* xp = reinterpret_cast<uint32_t*>(smXp + warp * kXpWarpBytes);
     const int h1 = p.h >> 1, w1 = p.w >> 1, h2 = p.h >> 2, w2 = p.w >> 2, h3 = p.h >> 3, w3 = p.w >> 3;
     const bool wr = p.experiment != 1;
+    // tiled: one thread per warpgroup issues that warpgroup's level-0/1 tensor stores (one bulk group per m64 half)
+    const bool tma_thread = (etid & 127) == 0;
+    if (kTiled && etid < kBM) {
+      // the level-2 piece's padding to pitch2 is written out with it: zeros, once
+      for (int b = 2 * p2row; b < p.pitch2; b += 4)
+        *reinterpret_cast<uint32_t*>(pool2 + etid * p2src + b) = 0u;
+    }
     int aph = 0, bph = 0, tile = 0;
     for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
       const int yb = item % p.n_yb;
@@ -252,6 +376,25 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
         if (xb + kBStages >= p.n_xb) a_held = false;
 #pragma unroll
         for (int mh = 0; mh < 2; ++mh) {
+        if constexpr (kTiled) {
+          unsigned char* st0 = smL0 + (group * 2 + mh) * kL0HalfBytes;
+          unsigned char* st1 = smL1 + (group * 2 + mh) * kL1HalfBytes;
+          tiled_half_epilogue(acc[mh], st0, st1, pool2 + mh * 64 * p2src, p2src, p2row, xb, (warp & 3) * 16, lane);
+          fence_async_smem();                        // the staged boxes become visible to the TMA engine
+          // The other half's buffers are written next: their last stores (the only bulk group of this thread
+          // still pending, issued one half-epilogue ago) must have been read out before this barrier.
+          if (tma_thread) bulk_wait_read<0>();
+          named_bar_sync(1 + group, 128);
+          if (tma_thread) {
+            const int s0 = mt * kBM + mh * 64;
+            if (wr && s0 < p.hw) {
+              // source pixels >= hw of the ragged last m-tile are clipped by the map's per-slot bound
+              tma_store_4d(&mapL0, st0, xb * 64, 2 * yb, s0, n_out);
+              if (p.num_levels > 1 && yb < p.h4_1) tma_store_4d(&mapL1, st1, xb * 32, yb, s0, n_out);
+            }
+            bulk_commit();
+          }
+        } else {
         const int row = mh * 64 + (warp & 3) * 16 + (lane & 15);  // tile row = source pixel (after the transpose)
         const int src = mt * kBM + row;
         const bool src_ok = src < p.hw && wr;
@@ -268,28 +411,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
               xp[(lane >> 2) * kXpRowWords + sub * 32 + 4 * j + (lane & 3)] =
                   pack2(acc[mh][sub][4 * j + 2 * pass], acc[mh][sub][4 * j + 2 * pass + 1]);
           __syncwarp();
-          if (p.tiled && wr) {
-            // level 0, tiled: the 16 rows x 2 halves staged in this pass are 16 whole 128-byte lines (four
-            // 4x4 tiles each); 8 lanes write one line, so every STG.128 of the warp fills 4 complete lines
-            const int c = lane & 7, t = c >> 1, r0 = 2 * (c & 1);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int li = 4 * i + (lane >> 3);
-              const int r = li & 7, hf = li >> 3;
-              const int lsrc = mt * kBM + mh * 64 + (warp & 3) * 16 + pass * 8 + r;
-              const int lty = 2 * yb + hf;
-              if (lsrc < p.hw && lty < p.h4_0 && xb * 4 + t < p.w4_0) {
-                const uint32_t* s = xp + r * kXpRowWords + hf * 32 + 2 * t;
-                const uint2 u = *reinterpret_cast<const uint2*>(s + 8 * r0);
-                const uint2 v = *reinterpret_cast<const uint2*>(s + 8 * (r0 + 1));
-                unsigned char* dst = reinterpret_cast<unsigned char*>(p.lvl[0]) +
-                                     ((((long long)n_out * p.hw + lsrc) * p.h4_0 + lty) * p.w4_0 + xb * 4 + t) * 32LL +
-                                     (c & 1) * 16;
-                asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(dst), "r"(u.x), "r"(u.y), "r"(v.x), "r"(v.y)
-                             : "memory");
-              }
-            }
-          }
           if (((lane >> 3) & 1) == pass) {
             const uint4* sp = reinterpret_cast<const uint4*>(xp + (lane & 7) * kXpRowWords + half * 32);
 #pragma unroll
@@ -302,21 +423,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           __syncwarp();
         }
         uint32_t l1[2][4];     // the two level-1 rows this thread produces (8 halves each)
-        if (p.tiled) {
-          // ---- tiled layout (level 0 left from the transpose buffer above): level 1 pooled from the
-          // thread's 4 patch rows x 16 columns ----
-#pragma unroll
-          for (int cc = 0; cc < 2; ++cc) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              l1[cc][j] = pack2(pool_pair(hr[2 * cc][2 * j], hr[2 * cc + 1][2 * j]),
-                                pool_pair(hr[2 * cc][2 * j + 1], hr[2 * cc + 1][2 * j + 1]));
-            // level-1 row (2*half+cc) of the band, columns 8*xb .. 8*xb+7 = sub-row of two 4x4 tiles
-            unsigned char* st = pool1 + row * p1src + (2 * half + cc) * 8;
-            *reinterpret_cast<uint2*>(st + (xb * 2) * 32) = make_uint2(l1[cc][0], l1[cc][1]);
-            *reinterpret_cast<uint2*>(st + (xb * 2 + 1) * 32) = make_uint2(l1[cc][2], l1[cc][3]);
-          }
-        } else {
 #pragma unroll
         for (int cc = 0; cc < 2; ++cc) {
           const int c = 2 * half + cc;           // 32-column chunk = patch rows 2c, 2c+1
@@ -334,7 +440,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           *reinterpret_cast<uint4*>(pool1 + row * p1src + c * p1row + xb * 16) =
               make_uint4(l1[cc][0], l1[cc][1], l1[cc][2], l1[cc][3]);
         }
-        }
         // level-2 row `half` of the band, from the two level-1 rows
         {
           const uint32_t a0 = pack2(pool_pair(l1[0][0], l1[1][0]), pool_pair(l1[0][1], l1[1][1]));
@@ -342,12 +447,13 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           *reinterpret_cast<uint2*>(pool2 + row * p2src + half * p2row + xb * 8) = make_uint2(a0, a1);
         }
         }
+        }
       }
       // a warp that had no tile in this item releases A here
       if (a_held && lane == 0) mbar_arrive(empty_a);
       // ---- band write-out: both consumer warpgroups have staged every x-tile of this 8-row band ----
-      if (p.tiled) fence_async_smem();           // staged rows become visible to the async (TMA) proxy
-      asm volatile("bar.sync 3, 256;" ::: "memory");
+      if (kTiled) fence_async_smem();            // staged rows become visible to the async (TMA) proxy
+      named_bar_sync(3, kEpiThreads);
       if (wr && p.num_levels > 1)
       for (int s_loc = etid >> 2; s_loc < kBM; s_loc += kEpiThreads / 4) {
         const int part = etid & 3;                             // four threads per source pixel
@@ -356,18 +462,18 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           const long long pl = (long long)n_out * p.hw + s_glb;
           const unsigned char* sp1 = pool1 + s_loc * p1src;
           const unsigned char* sp2 = pool2 + s_loc * p2src;
-          if (p.tiled) {
-            // The staged pieces are byte-for-byte what goes to memory: hand them to the TMA engine
-            // (one bulk copy per source pixel and level) and go back to draining accumulators; the
-            // copies stream out while the next band's level-0 stores are being issued.
-            if (part == 0 && yb < p.h4_1)
-              bulk_store(reinterpret_cast<unsigned char*>(p.lvl[1]) + ((pl * p.h4_1 + yb) * p.w4_1) * 32LL, sp1,
-                         (uint32_t)p.w4_1 * 32u);
-            if (part == 1 && p.num_levels > 2 && 2 * yb < h2)
+          if constexpr (kTiled) {
+            // Levels 2 and 3 (levels 0 and 1 left per tile): the staged pieces are byte-for-byte what goes
+            // to memory, one bulk copy per source pixel and level.  Parts 0 and 3 (among them the level-0/1
+            // store threads) issue none, so their bulk groups hold only the per-tile stores.
+            if (part == 1 && p.num_levels > 2 && 2 * yb < h2) {
               bulk_store(reinterpret_cast<unsigned char*>(p.lvl[2]) + (pl * p.n_yb + yb) * (long long)p.pitch2, sp2,
                          (uint32_t)p.pitch2);
+              bulk_commit();
+              bulk_wait_read();                    // the staging rows may be overwritten after the next barrier
+            }
             if (part == 2 && p.num_levels > 3 && yb < h3) {
-              uint32_t* s3 = reinterpret_cast<uint32_t*>(const_cast<unsigned char*>(sp2) + p.pitch2);
+              unsigned char* s3 = const_cast<unsigned char*>(sp2) + p.pitch2;
 #pragma unroll
               for (int k = 0; k < 8; ++k) {
                 uint32_t v = 0u;
@@ -378,16 +484,14 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
                   const uint32_t b2 = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 8 * k + 4);
                   v = pack2(pool_pair(t, b), pool_pair(t2, b2));
                 }
-                s3[k] = v;
+                reinterpret_cast<uint32_t*>(s3)[k] = v;
               }
               fence_async_smem();
               bulk_store(reinterpret_cast<unsigned char*>(p.lvl[3]) + (pl * p.n_yb + yb) * 32LL, s3, 32u);
+              bulk_commit();
+              bulk_wait_read();
             }
-            bulk_commit();
-            bulk_wait_read();                      // the staging rows may be overwritten after the next barrier
-          } else
-          if (p.aligned) {
-            if (!p.tiled) {
+          } else if (p.aligned) {
             // level 1: 4 full rows, contiguous in memory, 32-byte aligned: whole sectors
             unsigned char* g1 = reinterpret_cast<unsigned char*>(p.lvl[1]) +
                                 (pl * h1 + (y0 >> 1)) * (long long)p1row;
@@ -398,7 +502,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
               asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(g1 + off), "r"(rr[0]),
                            "r"(rr[1]), "r"(rr[2]), "r"(rr[3]), "r"(rr[4]), "r"(rr[5]), "r"(rr[6]), "r"(rr[7])
                            : "memory");
-            }
             }
             if (part == 1 && p.num_levels > 2) {                // level 2: 2 rows, 16-byte chunks
               unsigned char* g2 = reinterpret_cast<unsigned char*>(p.lvl[2]) +
@@ -422,13 +525,12 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
             // ragged shapes: element-wise with bounds (staging rows are n_xb*8 / n_xb*4 halves wide)
             const __half* s1 = reinterpret_cast<const __half*>(sp1);
             const __half* s2 = reinterpret_cast<const __half*>(sp2);
-            if (!p.tiled)
-              for (int r = 0; r < 4; ++r) {
-                const int y = (y0 >> 1) + r;
-                if (y >= h1) break;
-                __half* g = p.lvl[1] + (pl * h1 + y) * w1;
-                for (int x = part; x < w1; x += 4) g[x] = s1[r * (p1row / 2) + x];
-              }
+            for (int r = 0; r < 4; ++r) {
+              const int y = (y0 >> 1) + r;
+              if (y >= h1) break;
+              __half* g = p.lvl[1] + (pl * h1 + y) * w1;
+              for (int x = part; x < w1; x += 4) g[x] = s1[r * (p1row / 2) + x];
+            }
             if (p.num_levels > 2)
               for (int r = 0; r < 2; ++r) {
                 const int y = (y0 >> 2) + r;
@@ -449,9 +551,9 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA,
           }
         }
       }
-      asm volatile("bar.sync 3, 256;" ::: "memory");
+      named_bar_sync(3, kEpiThreads);
     }
-    if (p.tiled) bulk_wait_all();
+    if (kTiled) bulk_wait_all();
   }
 }
 
@@ -515,9 +617,10 @@ EncodeTiledFn get_encode_fn() {
 #ifndef GOSLAM_TC_EXPERIMENT
 #define GOSLAM_TC_EXPERIMENT 0
 #endif
-// Tensor maps depend only on (base pointer, frame count, h, w): a factor graph builds from the same
-// video-level K-major buffer for its whole life, so the two cuTensorMapEncodeTiled driver calls per launch
-// (~2 us of host time each) are paid once.  Small most-recently-used table, shared by all threads.
+// Tensor maps depend only on (base pointer, frame count, h, w, kind): a factor graph builds from the same
+// video-level K-major buffer into the same slot pool for its whole life, so the cuTensorMapEncodeTiled driver
+// calls of a launch (~2 us of host time each) are paid once.  Small most-recently-used table, shared by all
+// threads.  kind: 0 = A operand, 1 = B operand, 2 / 3 = tiled level 0 / 1 output (F unused).
 struct MapKey { const void* base; int F, h, w, kind; };
 struct MapSlot { MapKey key; CUtensorMap map; unsigned long long stamp; bool used; };
 constexpr int kMapSlots = 16;
@@ -532,6 +635,27 @@ bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
     return enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(k.base), dims, strides, box, es,
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  }
+  if (k.kind >= 2) {
+    // tiled level 0 / 1 output, one plane of H4 x W4 tiles (32 B) per (slot, source pixel), as the 4-D tensor
+    // (halves within a tile row, tile row, source pixel, slot).  Box = one m64 half of a 128x128 tile:
+    //   level 0: 64 halves (4 tiles) x 2 tile rows x 64 source px, 128B-swizzled;
+    //   level 1: 32 halves (2 tiles) x 1 tile row x 64 source px, 64B-swizzled.
+    // The source-pixel bound is per slot, so the ragged last m-tile of a slot is clipped, and so are tile
+    // rows / columns past H4 / W4.  The slot count is left open (CorrPool slot ids come from the device):
+    // as many slots as 2^40 bytes hold.
+    const int lv = k.kind - 2;
+    const cuuint64_t w4 = (cuuint64_t)gs_cdiv(k.w >> lv, 4), h4 = (cuuint64_t)gs_cdiv(k.h >> lv, 4);
+    const cuuint64_t slot_bytes = hw * h4 * w4 * 32;
+    cuuint64_t slots = ((cuuint64_t)1 << 40) / slot_bytes;
+    if (slots > 0x7fffffffull) slots = 0x7fffffffull;
+    cuuint64_t dims[4] = {w4 * 16, h4, hw, slots};
+    cuuint64_t strides[3] = {w4 * 32, h4 * w4 * 32, slot_bytes};
+    cuuint32_t box[4] = {lv == 0 ? 64u : 32u, lv == 0 ? 2u : 1u, 64u, 1u};
+    cuuint32_t es[4] = {1, 1, 1, 1};
+    return enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(k.base), dims, strides, box, es,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, lv == 0 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+               CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
   }
   // B: (ch, x, y, frame), box 64 ch x 16 x 8: an image patch; rows / columns outside the image read as zero
   cuuint64_t dims[4] = {(cuuint64_t)kD, (cuuint64_t)k.w, (cuuint64_t)k.h, (cuuint64_t)k.F};
@@ -574,19 +698,28 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   const int hw = h * w;
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return GOSLAM_ELAUNCH;
-  CUtensorMap mapA, mapB;
+  CUtensorMap mapA, mapB, mapL0, mapL1;
   if (!cached_map(enc, MapKey{f1t, F1, h, w, 0}, &mapA) || !cached_map(enc, MapKey{f2t, F2, h, w, 1}, &mapB))
     return GOSLAM_ELAUNCH;
+  mapL0 = mapL1 = mapA;                      // row-major: unused
+  if (tiled) {
+    // the tensor stores need 16-byte aligned level 0 / 1 buffers
+    if ((reinterpret_cast<uintptr_t>(levels[0]) & 15) ||
+        (num_levels > 1 && (reinterpret_cast<uintptr_t>(levels[1]) & 15)))
+      return GOSLAM_EINVAL;
+    if (!cached_map(enc, MapKey{levels[0], 0, h, w, 2}, &mapL0) ||
+        (num_levels > 1 && !cached_map(enc, MapKey{levels[1], 0, h, w, 3}, &mapL1)))
+      return GOSLAM_ELAUNCH;
+  }
   TcParams p{};
   for (int i = 0; i < 4; ++i) p.lvl[i] = i < num_levels ? levels[i] : nullptr;
   p.num_levels = num_levels; p.N = N; p.h = h; p.w = w; p.hw = hw;
   p.n_mt = gs_cdiv(hw, kBM); p.n_yb = gs_cdiv(h, kPY); p.n_xb = gs_cdiv(w, kPX);
   p.n_items = N * p.n_mt * p.n_yb;
   p.ii = ii; p.jj = jj; p.rig = rig; p.out_slot = out_slot;
-  p.tiled = tiled ? 1 : 0;
   p.w4_0 = gs_cdiv(w, 4); p.h4_0 = gs_cdiv(h, 4);
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
-  p.pitch2 = (p.n_xb * 16 + 31) / 32 * 32; p.pitch3 = 32;
+  p.pitch2 = pitch2_of(p.n_xb); p.pitch3 = 32;
   p.aligned = (w % 16 == 0 && h % 8 == 0) ? 1 : 0;
   // Build-time switch (-DGOSLAM_TC_EXPERIMENT=1, profiling builds only): the shipped library has it at 0.
   p.experiment = GOSLAM_TC_EXPERIMENT;
@@ -600,8 +733,10 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   {
     std::lock_guard<std::mutex> lock(dev_mu);
     if (sm_count[dev] == 0) {
-      if (cudaFuncSetAttribute(corr_build_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               kSmemTC) != cudaSuccess)
+      if (cudaFuncSetAttribute(corr_build_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               smem_bytes(true, kMaxXB)) != cudaSuccess ||
+          cudaFuncSetAttribute(corr_build_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               smem_bytes(false, kMaxXB)) != cudaSuccess)
         return GOSLAM_ELAUNCH;
       int n = kNumSms;
       cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
@@ -610,7 +745,11 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
     sms = sm_count[dev];
   }
   const int grid = p.n_items < sms ? p.n_items : sms;
-  corr_build_tc_kernel<<<grid, kThreadsTC, kSmemTC, st>>>(mapA, mapB, p);
+  const int smem = smem_bytes(tiled != 0, p.n_xb);
+  if (tiled)
+    corr_build_tc_kernel<true><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, p);
+  else
+    corr_build_tc_kernel<false><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, p);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

@@ -55,10 +55,34 @@ __device__ __forceinline__ void bulk_store(void* gdst, const void* ssrc, uint32_
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
                "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
 }
+// tensor (TMA) store shared -> global of one box; the tensor map clips rows / columns outside its bounds
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* ssrc, int c0, int c1, int c2,
+                                             int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   (uint64_t)map), "r"(smem_u32(ssrc)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the source shared memory of all but the newest N committed bulk groups may be overwritten
+template <int N = 0>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// four 8x8 b16 matrices to shared memory: register i of lane l holds row l/4, columns 2(l%4), 2(l%4)+1 of
+// matrix i; lane 8i + r gives the (16-byte aligned) address of row r of matrix i
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_u16(uint32_t saddr, uint16_t v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(saddr), "h"(v) : "memory");
+}
+// barrier over `count` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // Hopper wgmma shared-memory matrix descriptor for a K-major, SWIZZLE_128B operand (the layout a TMA box of
 // 64 fp16 channels x rows writes): start>>4 | LBO(unused for SW128, =1)<<16 | SBO(=1024B, one 8-row atom)>>4 <<32 |
