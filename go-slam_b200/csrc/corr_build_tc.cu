@@ -13,19 +13,25 @@
 //               the device (slot1 = rig*ii, slot2 = rig*jj + (ii==jj)), so no gathered copies exist.
 //               A is released as soon as the item's last MMAs retire, so the next item's A and B tiles
 //               load under the current epilogue and band write-out.
+//               Tiled layout: warps 9-11 of this warpgroup are the store warps.  Per band they pool level 3
+//               from the staged level 2 and write both with one TMA tensor store each, out of a double-
+//               buffered band pool handed over by mbarriers ("staged": the 8 consumer warps, "freed": the
+//               store thread after cp.async.bulk.wait_group.read).  The consumer warpgroups never join.
 //   warpgroups 0-1  consumers (232 registers each: the 128 fp32 accumulators and the epilogue stay in
 //               registers, no local memory); warpgroup g takes the x-tiles of parity g (B stage g), so
 //               one warpgroup's MMAs overlap the other's epilogue.  A warpgroup issues 32 wgmma m64n64k16
 //               (fp16 in, fp32 accumulate) for the whole 128x128 tile, then per m64 half rounds to fp16.
 //               Tiled layout: level 0 goes into swizzled staging with stmatrix, level 1 is pooled in
-//               registers from the rounded fragment and staged beside it, and one thread per warpgroup
-//               writes both with TMA tensor stores (tiled_half_epilogue); the consumers issue no global
-//               stores.  Row-major layout: the fragment is transposed through a small per-warp buffer,
+//               registers from the rounded fragment and staged beside it; lane 0 of each warp writes its own
+//               16 source pixels of both with TMA tensor stores, level 0 as soon as it is staged
+//               (tiled_half_epilogue), so the warps of a warpgroup never wait for each other; the
+//               consumers issue no global stores.  Row-major layout: the fragment is transposed through a small per-warp buffer,
 //               each thread then owns 4 rows x 16 columns of its source pixel's patch (level 0 as
 //               full-sector 32-byte stores) and pools level 1 in registers.  Both pool FROM THE ROUNDED
 //               finer level (the avg_pool2d numerics) and stage level 2 (row-major: also level 1) per band;
 //               when the band's x-tiles are done those rows (and level 3, pooled from the staged level 2)
-//               leave as contiguous runs (tiled: TMA bulk stores).  The volume is never re-read.
+//               leave as contiguous runs (tiled: through the store warps; row-major: both consumer
+//               warpgroups join and write them out).  The volume is never re-read.
 // Why the band staging: partial 32-byte-sector writes cost an ECC read-modify-write in L2.
 // The 1/4 feature scaling of the reference (`fmap / 4.0` in half) is applied by the K-major
 // re-layout prepass, exactly as the reference does it, so the accumulator needs no scaling.
@@ -55,30 +61,37 @@ constexpr int kThreadsTC = kEpiThreads + 128;     // + the TMA producer warpgrou
 // register reallocation: 128 x 40 + 256 x 232 <= 65,536 (the producer needs few, the accumulators many)
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kMaxXB = 8;                                // x-tiles per band (w <= 128)
+constexpr int kStoreWarps = 3;                           // tiled: producer-warpgroup warps 9-11 write levels 2, 3
 // Shared memory, sized per launch from n_xb (the x-tiles of a band); offsets from a 1024-byte aligned base:
-//   item                                        tiled                    row-major
-//   mbarriers                                   1 KB                     1 KB
-//   A tile (128 source px x 128 ch)             32 KB                    32 KB
-//   B stages (2 x 128 target px x 128 ch)       64 KB                    64 KB
-//   level-0 staging (2 per warpgroup, m64)      4 x 16 KB                -
-//   level-1 staging (2 per warpgroup, m64)      4 x 4 KB                 128 x (64 n_xb + 16) B   (band pool)
-//   level-2/3 band pool                         128 x (pitch2 + 48) B    128 x (16 n_xb + 8) B
-//   per-warp transpose buffers                  -                        8 x 2,176 B
-//   + 1 KB of alignment slack.  At w = 128 (n_xb = 8): tiled 200 KB, row-major 198 KB (<= 227 KB).
+//   item                                        tiled                           row-major
+//   mbarriers                                   1 KB                            1 KB
+//   A tile (128 source px x 128 ch)             32 KB                           32 KB
+//   B stages (2 x 128 target px x 128 ch)       64 KB                           64 KB
+//   level-0 staging (2 per warpgroup, m64)      4 x 16 KB                       -
+//   level-1 staging (2 per warpgroup, m64)      4 x 4 KB                        128 x (64 n_xb + 16) B   (band pool)
+//   level-2/3 band pool                         2 x 128 x (pitch2 + 32) B       128 x (16 n_xb + 8) B
+//   per-warp transpose buffers                  -                               8 x 2,176 B
+//   + 1 KB of alignment slack.  w = 80 (n_xb = 5): tiled 210 KB, row-major 168 KB; w = 128 (n_xb = 8): tiled
+//   218 KB, row-major 198 KB (<= 227 KB).
 constexpr int kBarBytes = 1024;
 constexpr int kL0HalfBytes = 64 * 2 * 128;        // m64 half of a tile's level 0: 64 source px x 2 tile rows x 128 B
 constexpr int kL1HalfBytes = 64 * 64;             // ... of its level 1: 64 source px x one tile row of 2 tiles (64 B)
+constexpr int kL0WarpBytes = kL0HalfBytes / kGroupWarps, kL1WarpBytes = kL1HalfBytes / kGroupWarps;  // 16 source px
+constexpr int kL3BandBytes = kBM * 32;            // tiled: a band's level-3 pieces, 32 B per source pixel
 // per-warp transpose of the accumulator fragment: 8 tile rows x 128 fp16 columns, rows padded to 68 words
 constexpr int kXpRowWords = 68;
 constexpr int kXpWarpBytes = 8 * kXpRowWords * 4;                                 // 2,176 B
 constexpr int kFixedBytes = 1024 + kBarBytes + (1 + kBStages) * kTileBytes;
 __host__ __device__ constexpr int pitch2_of(int n_xb) { return (n_xb * 16 + 31) / 32 * 32; }
+// tiled: the level-2 staging is dense (the box of the level-2 tensor map); row-major: padded against bank conflicts
 __host__ __device__ constexpr int pool2_src_bytes(bool tiled, int n_xb) {
-  return tiled ? pitch2_of(n_xb) + 48 : 2 * n_xb * 8 + 8;
+  return tiled ? pitch2_of(n_xb) : 2 * n_xb * 8 + 8;
 }
+// tiled: one of the two band buffers, level 2 then level 3
+__host__ __device__ constexpr int band_bytes(int n_xb) { return kBM * pool2_src_bytes(true, n_xb) + kL3BandBytes; }
 __host__ __device__ constexpr int pool1_src_bytes(int n_xb) { return 4 * n_xb * 16 + 16; }
 __host__ __device__ constexpr int smem_bytes(bool tiled, int n_xb) {
-  return tiled ? kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + kBM * pool2_src_bytes(true, n_xb)
+  return tiled ? kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + 2 * band_bytes(n_xb)
                : kFixedBytes + kBM * (pool1_src_bytes(n_xb) + pool2_src_bytes(false, n_xb)) +
                      kEpiThreads / 32 * kXpWarpBytes;
 }
@@ -101,8 +114,15 @@ struct TcParams {
   int w4_0, h4_0, w4_1, h4_1;
   int pitch2, pitch3;         // tiled: bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
   int aligned;                // row-major: w % 16 == 0 && h % 8 == 0: every store is a whole aligned sector run
-  int experiment;             // profiling only: 1 = no output writes
 };
+
+// Build-time switch for profiling builds only (tools/build_variant.py -DGOSLAM_TC_EXPERIMENT=N); the shipped
+// library has it at 0.  1 = no output writes.  2 = stores only: no operand loads and no MMAs (the accumulators
+// are zero), but the whole epilogue and every store, i.e. the floor of the kernel's write pattern.
+#ifndef GOSLAM_TC_EXPERIMENT
+#define GOSLAM_TC_EXPERIMENT 0
+#endif
+constexpr int kExperiment = GOSLAM_TC_EXPERIMENT;
 
 // ---- packed fp16 rows live in registers as uint32 pairs (lo = even column) ----
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -168,9 +188,12 @@ __device__ __forceinline__ void store_row(__half* dst, const uint32_t (&r)[NW], 
 //             the 2x2 pools of a lane's own x pair, rows 2k, 2k+1 (y1 = 2ty + k, x1 = q); one shfl.xor(1)
 //             pairs x1 columns into words.
 //   level 2 -> the band pool, from those level-1 words (y2 = lane parity).
+// Every smem row a warp writes belongs to its own 16 source pixels.  between_levels() runs after the level-0
+// stmatrix and before the first level-1 store (the warp issues its level-0 store there).
+template <typename F>
 __device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], unsigned char* st0, unsigned char* st1,
                                                     unsigned char* pool2_row0, int p2src, int p2row, int xb,
-                                                    int wrow, int lane) {
+                                                    int wrow, int lane, F between_levels) {
   // packed rounded fp16 pairs: W[rh][ty][r4][jx] = x pair (8jx + 2(lane%4), +1) of patch row 4ty + r4
   uint32_t W[2][2][4][2];
 #pragma unroll
@@ -213,6 +236,7 @@ __device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], u
           stmatrix_x4(st0_u + R * 128 + ((chunk ^ (R & 7)) << 4), m);
         }
   }
+  between_levels();
   // ---- levels 1 and 2 ----
   const bool ev = (lane & 1) == 0;                 // even lanes: level-1 rows 0, 1 and level-2 row 0
   const uint32_t st1_u = smem_u32(st1);
@@ -250,6 +274,7 @@ template <bool kTiled>
 __global__ void __launch_bounds__(kThreadsTC, 1)
 corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                      const __grid_constant__ CUtensorMap mapL0, const __grid_constant__ CUtensorMap mapL1,
+                     const __grid_constant__ CUtensorMap mapL2, const __grid_constant__ CUtensorMap mapL3,
                      const TcParams p) {
   extern __shared__ unsigned char smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms (pointer arithmetic on smem_raw: stays in the shared window)
@@ -262,6 +287,12 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
   uint64_t* empty_a = bars + 1;
   uint64_t* full_b = bars + 2;                   // [kBStages]
   uint64_t* empty_b = full_b + kBStages;
+  uint64_t* staged = empty_b + kBStages;         // tiled: [2] band buffers, written by all consumer warps
+  uint64_t* freed = staged + 2;                  // tiled: [2] ... and read out by the store warps' TMA stores
+  // tiled: level-0 / level-1 staging, two m64 halves per warpgroup, then the two band buffers (levels 2, 3)
+  unsigned char* smL0 = smEpi;
+  unsigned char* smL1 = smL0 + 2 * kBStages * kL0HalfBytes;
+  constexpr bool wr = kExperiment != 1;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -269,6 +300,7 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     // A is released by every consumer warp once its last MMA of the item has retired
     mbar_init(full_a, 1); mbar_init(empty_a, kEpiThreads / 32);
     for (int i = 0; i < kBStages; ++i) { mbar_init(&full_b[i], 1); mbar_init(&empty_b[i], kGroupWarps); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&staged[i], kEpiThreads / 32); mbar_init(&freed[i], 1); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -277,6 +309,8 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     // ===================== TMA producer (one thread of the producer warpgroup) =====================
     setmaxnreg_dec<kProducerRegs>();
     if (warp == kEpiThreads / 32 && lane == 0) {
+      // the feature maps are re-read by every band and edge; the 0.98 GB pyramid streams past them in L2
+      const uint64_t keep = l2_evict_last();
       int aph = 0, bs = 0, bph = 0;
       for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
         const int yb = item % p.n_yb;
@@ -289,19 +323,68 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           n2 = p.rig * fj + ((fi == fj && p.rig > 1) ? 1 : 0);
         }
         mbar_wait(empty_a, aph ^ 1);
-        mbar_expect_tx(full_a, kTileBytes);
-        tma_load_3d(&mapA, full_a, smA, 0, mt * kBM, n1);
-        tma_load_3d(&mapA, full_a, smA + kBoxBytes, kKBox, mt * kBM, n1);
+        if constexpr (kExperiment == 2) {
+          mbar_arrive(full_a);
+        } else {
+          mbar_expect_tx(full_a, kTileBytes);
+          tma_load_3d_hint(&mapA, full_a, smA, 0, mt * kBM, n1, keep);
+          tma_load_3d_hint(&mapA, full_a, smA + kBoxBytes, kKBox, mt * kBM, n1, keep);
+        }
         aph ^= 1;
         for (int xb = 0; xb < p.n_xb; ++xb) {
           mbar_wait(&empty_b[bs], bph ^ 1);
-          mbar_expect_tx(&full_b[bs], kTileBytes);
-          tma_load_4d(&mapB, &full_b[bs], smB + bs * kTileBytes, 0, xb * kPX, yb * kPY, n2);
-          tma_load_4d(&mapB, &full_b[bs], smB + bs * kTileBytes + kBoxBytes, kKBox, xb * kPX,
-                      yb * kPY, n2);
+          if constexpr (kExperiment == 2) {
+            mbar_arrive(&full_b[bs]);
+          } else {
+            mbar_expect_tx(&full_b[bs], kTileBytes);
+            tma_load_4d_hint(&mapB, &full_b[bs], smB + bs * kTileBytes, 0, xb * kPX, yb * kPY, n2, keep);
+            tma_load_4d_hint(&mapB, &full_b[bs], smB + bs * kTileBytes + kBoxBytes, kKBox, xb * kPX,
+                             yb * kPY, n2, keep);
+          }
           if (++bs == kBStages) { bs = 0; bph ^= 1; }
         }
       }
+    } else if (kTiled && warp > kEpiThreads / 32) {
+      // ===================== store warps (tiled): levels 2 and 3 of each band =====================
+      const int sid = threadIdx.x - (kEpiThreads + 32);          // 0 .. 95
+      const int p2src = p.pitch2, p2row = p.n_xb * 8;
+      unsigned char* pool2 = smL1 + 2 * kBStages * kL1HalfBytes;
+      const int h2 = p.h >> 2, h3 = p.h >> 3;
+      int it = 0;                                                // items of this CTA so far
+      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it) {
+        const int yb = item % p.n_yb;
+        const int mt = (item / p.n_yb) % p.n_mt;
+        const int n = item / (p.n_yb * p.n_mt);
+        const bool out2 = wr && p.num_levels > 2 && 2 * yb < h2, out3 = wr && p.num_levels > 3 && yb < h3;
+        unsigned char* s2 = pool2 + (it & 1) * band_bytes(p.n_xb);
+        const uint32_t s2_u = smem_u32(s2), s3_u = s2_u + kBM * p2src;
+        mbar_wait(&staged[it & 1], (it >> 1) & 1);
+        if (out3) {
+          // word k of a source pixel's level-3 piece = columns 2k, 2k + 1, pooled from x-tile k of level 2
+          for (int i = sid; i < kBM * 8; i += kStoreWarps * 32) {
+            const int k = i & 7;
+            uint32_t v = 0u;
+            if (k < p.n_xb) {
+              const uint32_t a = s2_u + (i >> 3) * p2src + 8 * k;
+              v = pack2(pool_pair(ld_shared_u32(a), ld_shared_u32(a + p2row)),
+                        pool_pair(ld_shared_u32(a + 4), ld_shared_u32(a + p2row + 4)));
+            }
+            st_shared_u32(s3_u + 4 * i, v);
+          }
+          fence_async_smem();
+        }
+        named_bar_sync(4, kStoreWarps * 32);
+        if (sid == 0) {
+          // source pixels >= hw of the ragged last m-tile are clipped by the maps' per-slot bound
+          const int n_out = p.out_slot ? __ldg(p.out_slot + n) : n;
+          if (out2) tma_store_4d_hint(&mapL2, s2, 0, yb, mt * kBM, n_out, l2_evict_first());
+          if (out3) tma_store_4d_hint(&mapL3, s2 + kBM * p2src, 0, yb, mt * kBM, n_out, l2_evict_first());
+          bulk_commit();
+          bulk_wait_read<0>();
+          mbar_arrive(&freed[it & 1]);
+        }
+      }
+      if (sid == 0) bulk_wait_all();
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma + epilogue, two warpgroups =====================
@@ -310,28 +393,23 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     const int half = lane >> 4;                   // row-major: patch rows 4*half .. 4*half+3 (columns 64*half..)
     const int etid = threadIdx.x;                 // 0..255
     const int ts = group;
-    // tiled: level-0 / level-1 staging, two m64 halves per warpgroup, then the band pool (levels 2, 3)
-    unsigned char* smL0 = smEpi;
-    unsigned char* smL1 = smL0 + 2 * kBStages * kL0HalfBytes;
-    // band staging strides (bytes); the +16 / +8 pads make the per-source-pixel stride conflict-free
+    // band staging strides (bytes); row-major: the +16 / +8 pads make the per-source-pixel stride conflict-free
     const int p1row = p.n_xb * 16, p1src = pool1_src_bytes(p.n_xb);
-    const int p2row = p.n_xb * 8;   // (tiled: the level-3 piece is staged behind the level-2 piece)
+    const int p2row = p.n_xb * 8;
     const int p2src = pool2_src_bytes(kTiled, p.n_xb);
     unsigned char* pool1 = smEpi;                 // row-major only
     unsigned char* pool2 = kTiled ? smL1 + 2 * kBStages * kL1HalfBytes : pool1 + kBM * p1src;
     unsigned char* smXp = pool2 + kBM * p2src;    // row-major only: [8 consumer warps][kXpWarpBytes]
     uint32_t* xp = reinterpret_cast<uint32_t*>(smXp + warp * kXpWarpBytes);
     const int h1 = p.h >> 1, w1 = p.w >> 1, h2 = p.h >> 2, w2 = p.w >> 2, h3 = p.h >> 3, w3 = p.w >> 3;
-    const bool wr = p.experiment != 1;
-    // tiled: one thread per warpgroup issues that warpgroup's level-0/1 tensor stores (one bulk group per m64 half)
-    const bool tma_thread = (etid & 127) == 0;
-    if (kTiled && etid < kBM) {
-      // the level-2 piece's padding to pitch2 is written out with it: zeros, once
-      for (int b = 2 * p2row; b < p.pitch2; b += 4)
-        *reinterpret_cast<uint32_t*>(pool2 + etid * p2src + b) = 0u;
+    if (kTiled && etid < 2 * kBM) {
+      // the level-2 piece's padding to pitch2 is written out with it: zeros, once per band buffer
+      unsigned char* piece = pool2 + (etid >> 7) * band_bytes(p.n_xb) + (etid & (kBM - 1)) * p2src;
+      for (int b = 2 * p2row; b < p2src; b += 4) st_shared_u32(smem_u32(piece + b), 0u);
     }
-    int aph = 0, bph = 0, tile = 0;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+    const uint64_t stream = l2_evict_first();     // the pyramid is written once and not read back here
+    int aph = 0, bph = 0, tile = 0, it = 0;
+    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it) {
       const int yb = item % p.n_yb;
       const int mt = (item / p.n_yb) % p.n_mt;
       const int n = item / (p.n_yb * p.n_mt);
@@ -340,6 +418,12 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
       mbar_wait(full_a, aph);
       aph ^= 1;
       bool a_held = true;
+      unsigned char* band = pool2;
+      if constexpr (kTiled) {
+        // tiled: band buffer it % 2, free once the store warps' TMA has read out the band staged there before
+        band += (it & 1) * band_bytes(p.n_xb);
+        mbar_wait(&freed[it & 1], ((it >> 1) & 1) ^ 1);
+      }
       for (int xb = 0; xb < p.n_xb; ++xb, ++tile) {
         if ((tile & (kBStages - 1)) != ts) continue;
         const int x0 = xb * kPX;
@@ -347,7 +431,15 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
         bph ^= 1;
         // 128 x 128 x 128 tile: two m64 row halves, N = 128 as two m64n64 halves (columns 0-63 | 64-127)
         float acc[2][2][32];
-        {
+        if constexpr (kExperiment == 2) {
+          // one opaque zero per accumulator, so the compiler keeps the whole epilogue
+#pragma unroll
+          for (int i = 0; i < 128; ++i) {
+            uint32_t z;
+            asm volatile("mov.b32 %0, 0;" : "=r"(z));
+            acc[i >> 6][(i >> 5) & 1][i & 31] = __uint_as_float(z);
+          }
+        } else {
           const uint32_t a_addr = smem_u32(smA);
           const uint32_t b_addr = smem_u32(smB + ts * kTileBytes);
           wgmma_fence();
@@ -379,19 +471,29 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
         if constexpr (kTiled) {
           unsigned char* st0 = smL0 + (group * 2 + mh) * kL0HalfBytes;
           unsigned char* st1 = smL1 + (group * 2 + mh) * kL1HalfBytes;
-          tiled_half_epilogue(acc[mh], st0, st1, pool2 + mh * 64 * p2src, p2src, p2row, xb, (warp & 3) * 16, lane);
-          fence_async_smem();                        // the staged boxes become visible to the TMA engine
-          // The other half's buffers are written next: their last stores (the only bulk group of this thread
-          // still pending, issued one half-epilogue ago) must have been read out before this barrier.
-          if (tma_thread) bulk_wait_read<0>();
-          named_bar_sync(1 + group, 128);
-          if (tma_thread) {
-            const int s0 = mt * kBM + mh * 64;
-            if (wr && s0 < p.hw) {
-              // source pixels >= hw of the ragged last m-tile are clipped by the map's per-slot bound
-              tma_store_4d(&mapL0, st0, xb * 64, 2 * yb, s0, n_out);
-              if (p.num_levels > 1 && yb < p.h4_1) tma_store_4d(&mapL1, st1, xb * 32, yb, s0, n_out);
+          // Each warp writes its own 16 source pixels: one bulk group for level 0, issued as soon as its stmatrix
+          // is done, and one for level 1.  A buffer is written again two halves later, once wait_group.read has
+          // retired its group there; the three newer groups may still be in flight.
+          const int wq = warp & 3;
+          const int s0 = mt * kBM + mh * 64 + wq * 16;
+          const bool out0 = wr && s0 < p.hw;         // rows >= hw of the ragged last m-tile: clipped by the maps
+          if (lane == 0) bulk_wait_read<3>();
+          __syncwarp();
+          tiled_half_epilogue(acc[mh], st0, st1, band + mh * 64 * p2src, p2src, p2row, xb, wq * 16, lane, [&] {
+            fence_async_smem();                      // the staged box becomes visible to the TMA engine
+            __syncwarp();
+            if (lane == 0) {
+              if (out0) tma_store_4d_hint(&mapL0, st0 + wq * kL0WarpBytes, xb * 64, 2 * yb, s0, n_out, stream);
+              bulk_commit();
+              bulk_wait_read<3>();
             }
+            __syncwarp();
+          });
+          fence_async_smem();
+          __syncwarp();
+          if (lane == 0) {
+            if (out0 && p.num_levels > 1 && yb < p.h4_1)
+              tma_store_4d_hint(&mapL1, st1 + wq * kL1WarpBytes, xb * 32, yb, s0, n_out, stream);
             bulk_commit();
           }
         } else {
@@ -451,8 +553,14 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
       }
       // a warp that had no tile in this item releases A here
       if (a_held && lane == 0) mbar_arrive(empty_a);
-      // ---- band write-out: both consumer warpgroups have staged every x-tile of this 8-row band ----
-      if (kTiled) fence_async_smem();            // staged rows become visible to the async (TMA) proxy
+      if constexpr (kTiled) {
+        // hand the band to the store warps; the two consumer warpgroups go on without joining
+        fence_async_smem();                      // staged rows become visible to the async (TMA) proxy
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&staged[it & 1]);
+        continue;
+      }
+      // ---- row-major band write-out: both consumer warpgroups have staged every x-tile of this 8-row band ----
       named_bar_sync(3, kEpiThreads);
       if (wr && p.num_levels > 1)
       for (int s_loc = etid >> 2; s_loc < kBM; s_loc += kEpiThreads / 4) {
@@ -462,36 +570,7 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           const long long pl = (long long)n_out * p.hw + s_glb;
           const unsigned char* sp1 = pool1 + s_loc * p1src;
           const unsigned char* sp2 = pool2 + s_loc * p2src;
-          if constexpr (kTiled) {
-            // Levels 2 and 3 (levels 0 and 1 left per tile): the staged pieces are byte-for-byte what goes
-            // to memory, one bulk copy per source pixel and level.  Parts 0 and 3 (among them the level-0/1
-            // store threads) issue none, so their bulk groups hold only the per-tile stores.
-            if (part == 1 && p.num_levels > 2 && 2 * yb < h2) {
-              bulk_store(reinterpret_cast<unsigned char*>(p.lvl[2]) + (pl * p.n_yb + yb) * (long long)p.pitch2, sp2,
-                         (uint32_t)p.pitch2);
-              bulk_commit();
-              bulk_wait_read();                    // the staging rows may be overwritten after the next barrier
-            }
-            if (part == 2 && p.num_levels > 3 && yb < h3) {
-              unsigned char* s3 = const_cast<unsigned char*>(sp2) + p.pitch2;
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                uint32_t v = 0u;
-                if (k < p.n_xb) {
-                  const uint32_t t = *reinterpret_cast<const uint32_t*>(sp2 + 8 * k);
-                  const uint32_t t2 = *reinterpret_cast<const uint32_t*>(sp2 + 8 * k + 4);
-                  const uint32_t b = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 8 * k);
-                  const uint32_t b2 = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 8 * k + 4);
-                  v = pack2(pool_pair(t, b), pool_pair(t2, b2));
-                }
-                reinterpret_cast<uint32_t*>(s3)[k] = v;
-              }
-              fence_async_smem();
-              bulk_store(reinterpret_cast<unsigned char*>(p.lvl[3]) + (pl * p.n_yb + yb) * 32LL, s3, 32u);
-              bulk_commit();
-              bulk_wait_read();
-            }
-          } else if (p.aligned) {
+          if (p.aligned) {
             // level 1: 4 full rows, contiguous in memory, 32-byte aligned: whole sectors
             unsigned char* g1 = reinterpret_cast<unsigned char*>(p.lvl[1]) +
                                 (pl * h1 + (y0 >> 1)) * (long long)p1row;
@@ -614,16 +693,14 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-#ifndef GOSLAM_TC_EXPERIMENT
-#define GOSLAM_TC_EXPERIMENT 0
-#endif
 // Tensor maps depend only on (base pointer, frame count, h, w, kind): a factor graph builds from the same
 // video-level K-major buffer into the same slot pool for its whole life, so the cuTensorMapEncodeTiled driver
 // calls of a launch (~2 us of host time each) are paid once.  Small most-recently-used table, shared by all
-// threads.  kind: 0 = A operand, 1 = B operand, 2 / 3 = tiled level 0 / 1 output (F unused).
+// threads.  kind: 0 = A operand, 1 = B operand, 2 .. 5 = tiled level 0 .. 3 output (F unused).  A tiled launch
+// needs six maps, so the table holds those of a few pools at once.
 struct MapKey { const void* base; int F, h, w, kind; };
 struct MapSlot { MapKey key; CUtensorMap map; unsigned long long stamp; bool used; };
-constexpr int kMapSlots = 16;
+constexpr int kMapSlots = 32;
 
 bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
   const cuuint64_t hw = (cuuint64_t)k.h * k.w;
@@ -636,11 +713,30 @@ bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
   }
+  if (k.kind >= 4) {
+    // tiled level 2 / 3 output: per (slot, source pixel) one piece of pitch2 / 32 bytes per band, as the 4-D tensor
+    // (halves within a piece, band, source pixel, slot).  Box = one band of a 128-source-pixel tile, the dense
+    // staging of the store warps.  The source pixel is bounded per slot as for levels 0 / 1.
+    const int n_yb = gs_cdiv(k.h, kPY);
+    const cuuint64_t piece = k.kind == 4 ? (cuuint64_t)pitch2_of(gs_cdiv(k.w, kPX)) : 32;
+    const cuuint64_t slot_bytes = hw * n_yb * piece;
+    cuuint64_t slots = ((cuuint64_t)1 << 40) / slot_bytes;
+    if (slots > 0x7fffffffull) slots = 0x7fffffffull;
+    cuuint64_t dims[4] = {piece / 2, (cuuint64_t)n_yb, hw, slots};
+    cuuint64_t strides[3] = {piece, n_yb * piece, slot_bytes};
+    cuuint32_t box[4] = {(cuuint32_t)(piece / 2), 1u, (cuuint32_t)kBM, 1u};
+    cuuint32_t es[4] = {1, 1, 1, 1};
+    return enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(k.base), dims, strides, box, es,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  }
   if (k.kind >= 2) {
     // tiled level 0 / 1 output, one plane of H4 x W4 tiles (32 B) per (slot, source pixel), as the 4-D tensor
-    // (halves within a tile row, tile row, source pixel, slot).  Box = one m64 half of a 128x128 tile:
-    //   level 0: 64 halves (4 tiles) x 2 tile rows x 64 source px, 128B-swizzled;
-    //   level 1: 32 halves (2 tiles) x 1 tile row x 64 source px, 64B-swizzled.
+    // (halves within a tile row, tile row, source pixel, slot).  Box = one warp's 16 source px of a 128x128 tile:
+    //   level 0: 64 halves (4 tiles) x 2 tile rows x 16 source px, 128B-swizzled;
+    //   level 1: 32 halves (2 tiles) x 1 tile row x 16 source px, 64B-swizzled.
+    // A warp's rows are a 1024-byte aligned quarter of its m64 half's staging, so the swizzle phases are those
+    // of the whole half.
     // The source-pixel bound is per slot, so the ragged last m-tile of a slot is clipped, and so are tile
     // rows / columns past H4 / W4.  The slot count is left open (CorrPool slot ids come from the device):
     // as many slots as 2^40 bytes hold.
@@ -651,7 +747,7 @@ bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
     if (slots > 0x7fffffffull) slots = 0x7fffffffull;
     cuuint64_t dims[4] = {w4 * 16, h4, hw, slots};
     cuuint64_t strides[3] = {w4 * 32, h4 * w4 * 32, slot_bytes};
-    cuuint32_t box[4] = {lv == 0 ? 64u : 32u, lv == 0 ? 2u : 1u, 64u, 1u};
+    cuuint32_t box[4] = {lv == 0 ? 64u : 32u, lv == 0 ? 2u : 1u, 16u, 1u};
     cuuint32_t es[4] = {1, 1, 1, 1};
     return enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(k.base), dims, strides, box, es,
                CU_TENSOR_MAP_INTERLEAVE_NONE, lv == 0 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
@@ -698,18 +794,17 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   const int hw = h * w;
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return GOSLAM_ELAUNCH;
-  CUtensorMap mapA, mapB, mapL0, mapL1;
+  CUtensorMap mapA, mapB, mapL0, mapL1, mapL2, mapL3;
   if (!cached_map(enc, MapKey{f1t, F1, h, w, 0}, &mapA) || !cached_map(enc, MapKey{f2t, F2, h, w, 1}, &mapB))
     return GOSLAM_ELAUNCH;
-  mapL0 = mapL1 = mapA;                      // row-major: unused
+  mapL0 = mapL1 = mapL2 = mapL3 = mapA;      // row-major: unused
   if (tiled) {
-    // the tensor stores need 16-byte aligned level 0 / 1 buffers
-    if ((reinterpret_cast<uintptr_t>(levels[0]) & 15) ||
-        (num_levels > 1 && (reinterpret_cast<uintptr_t>(levels[1]) & 15)))
-      return GOSLAM_EINVAL;
-    if (!cached_map(enc, MapKey{levels[0], 0, h, w, 2}, &mapL0) ||
-        (num_levels > 1 && !cached_map(enc, MapKey{levels[1], 0, h, w, 3}, &mapL1)))
-      return GOSLAM_ELAUNCH;
+    // the tensor stores need 16-byte aligned level buffers
+    for (int i = 0; i < num_levels; ++i)
+      if (reinterpret_cast<uintptr_t>(levels[i]) & 15) return GOSLAM_EINVAL;
+    CUtensorMap* maps[4] = {&mapL0, &mapL1, &mapL2, &mapL3};
+    for (int i = 0; i < num_levels; ++i)
+      if (!cached_map(enc, MapKey{levels[i], 0, h, w, 2 + i}, maps[i])) return GOSLAM_ELAUNCH;
   }
   TcParams p{};
   for (int i = 0; i < 4; ++i) p.lvl[i] = i < num_levels ? levels[i] : nullptr;
@@ -721,8 +816,6 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
   p.pitch2 = pitch2_of(p.n_xb); p.pitch3 = 32;
   p.aligned = (w % 16 == 0 && h % 8 == 0) ? 1 : 0;
-  // Build-time switch (-DGOSLAM_TC_EXPERIMENT=1, profiling builds only): the shipped library has it at 0.
-  p.experiment = GOSLAM_TC_EXPERIMENT;
   // per-device: opt-in shared memory + SM count, looked up once per device
   static int sm_count[64];
   static std::mutex dev_mu;
@@ -747,9 +840,9 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   const int grid = p.n_items < sms ? p.n_items : sms;
   const int smem = smem_bytes(tiled != 0, p.n_xb);
   if (tiled)
-    corr_build_tc_kernel<true><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, p);
+    corr_build_tc_kernel<true><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
   else
-    corr_build_tc_kernel<false><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, p);
+    corr_build_tc_kernel<false><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

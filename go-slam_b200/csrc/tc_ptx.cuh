@@ -61,6 +61,37 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void*
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
                    (uint64_t)map), "r"(smem_u32(ssrc)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
+// L2 cache policies for the TMA copies below: evict_first for data written once and never re-read here,
+// evict_last for operands that later copies read again
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void tma_load_3d_hint(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1,
+                                                 int c2, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)), "l"((uint64_t)map),
+      "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_hint(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1,
+                                                 int c2, int c3, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)), "l"((uint64_t)map),
+      "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d_hint(const CUtensorMap* map, const void* ssrc, int c0, int c1, int c2,
+                                                  int c3, uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5}], [%1], %6;"
+               ::"l"((uint64_t)map), "r"(smem_u32(ssrc)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // the source shared memory of all but the newest N committed bulk groups may be overwritten
 template <int N = 0>
@@ -78,6 +109,11 @@ __device__ __forceinline__ void st_shared_u32(uint32_t saddr, uint32_t v) {
 }
 __device__ __forceinline__ void st_shared_u16(uint32_t saddr, uint16_t v) {
   asm volatile("st.shared.b16 [%0], %1;" ::"r"(saddr), "h"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr) : "memory");
+  return v;
 }
 // barrier over `count` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int count) {

@@ -36,3 +36,15 @@ for layout in layouts:
         lvl = sum((h >> i) * (w >> i) for i in range(4))
         gb = N * h * w * lvl * 2 / 1e9
         print(f"{h}x{w} {layout:8s} N={N:3d} {ms*1e3:8.1f} us  {ms*1e3/N:7.2f} us/edge  out={gb*1e3:7.1f} MB (algorithmic)  {gb/ms*1e3:7.1f} GB/s")
+        # the card's write ceiling beside it: a plain device fill of the same byte count
+        buf = torch.empty(int(gb * 1e9) // 2, dtype=torch.half, device=dev)
+        for _ in range(3):
+            buf.zero_()
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(20):
+            buf.zero_()
+        e1.record(); torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / 20
+        print(f"{h}x{w} {'fill':8s} N={N:3d} {ms*1e3:8.1f} us  {'':20s}out={gb*1e3:7.1f} MB  {gb/ms*1e3:7.1f} GB/s")
+        del buf
