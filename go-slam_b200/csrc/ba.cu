@@ -22,7 +22,7 @@
 //
 //   * Small windows (6P <= 96, every local window): ALL Gauss-Newton iterations of a call run in
 //     ONE cooperative kernel (ba_persistent_kernel) — linearise | grid barrier | reduced system |
-//     grid barrier | solve (block 0) | grid barrier, with the depth back-substitution of iteration
+//     arrivals -> solve (block 0) -> solved flag, with the depth back-substitution of iteration
 //     i fused into the linearisation of iteration i+1; larger systems and the multi-GPU split
 //     form (goslam_ba_phase1/2) run the same device functions as separate launches.
 //
@@ -48,7 +48,8 @@ struct BaWs {
   // graph tables (built once per call by ba_prep_kernel)
   int* slot_of_frame;  // [num]   slot in kx or -1
   int* kx;             // [num]   frame id of slot
-  int* counts;         // [8]     M, total_entries, total_pairs, grid-barrier counter, bad-argument flag
+  int* counts;         // [8]     M, total_entries, total_pairs, grid-barrier counter, bad-argument flag,
+                       //         system arrivals, solved iterations (the last three: cooperative kernel)
   int* row_ptr;        // [num+1] CSR over frame id: edges with ii == frame
   int* edge_idx;       // [N]
   int* entry_ptr;      // [num+1] per slot: Schur entries
@@ -62,6 +63,7 @@ struct BaWs {
   float* w;            // [num(slot),hw]
   float* part;         // [N,ntiles*kTP/32,27]  one partial per (edge, tile, warp)
   double* sys;         // [n*n + n]  reduced camera system (H row-major, then b)
+  double* sys_alt;     // [n*n + n]  cooperative kernel: odd iterations' system (zeroed while the other is in use)
   double* chol;        // [n*n]      factor scratch (global path)
   double* rhs;         // [n]        rhs / solution scratch (global path)
   float* dx;           // [P,6]
@@ -91,6 +93,7 @@ size_t ba_layout(const BaDims& d, void* base, size_t cap, BaWs* ws) {
   w.w = a.take<float>((size_t)d.num * d.hw);
   w.part = a.take<float>((size_t)(d.N > 0 ? d.N : 1) * ntiles * (kTP / 32) * kNRed);
   w.sys = a.take<double>((size_t)d.n * d.n + d.n);
+  w.sys_alt = a.take<double>((size_t)d.n * d.n + d.n);
   w.chol = a.take<double>((size_t)d.n * d.n);
   w.rhs = a.take<double>(d.n > 0 ? d.n : 1);
   w.dx = a.take<float>((size_t)(d.P > 0 ? d.P : 1) * 6);
@@ -155,10 +158,10 @@ ba_prep_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, B
                int eta_rows) {
   extern __shared__ int sm[];          // a[num] | b[num + 1] | c[num] | wsum[33]
   const int tid = threadIdx.x, nt = blockDim.x;
-  if (zero) {                          // single-kernel driver: reduced system and grid-barrier counter start at 0
+  if (zero) {                          // single-kernel driver: iteration 0's system and the sync counters start at 0
     const size_t nsys = (size_t)d.n * d.n + d.n;
     for (size_t i = tid; i < nsys; i += nt) ws.sys[i] = 0.0;
-    if (tid == 0) ws.counts[3] = 0;
+    if (tid == 0) { ws.counts[3] = 0; ws.counts[5] = 0; ws.counts[6] = 0; }
   }
   int* a = sm;                         // presence -> entries per slot -> entry_ptr
   int* b = sm + d.num;                 // degree -> row_ptr (kept)
@@ -240,18 +243,24 @@ ba_prep_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, B
   }
 }
 
+// One halving step of the transpose-reduction, then the next.  HALF is a template parameter so that
+// every index into v is a compile-time constant and v stays in registers (a loop over `half` left
+// v[32] in local memory: an LDL -> SHFL -> STL round trip per value).
+template <int HALF>
+__device__ __forceinline__ void transpose_reduce_step(float (&v)[32], int lane) {
+  const bool up = (lane & HALF) != 0;
+#pragma unroll
+  for (int i = 0; i < HALF; ++i) {
+    const float send = up ? v[i] : v[i + HALF];
+    const float keep = up ? v[i + HALF] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
+  }
+  if constexpr (HALF > 1) transpose_reduce_step<HALF / 2>(v, lane);
+}
+
 // 32 values per lane -> lane L returns sum over lanes of v[L]   (31 shuffles)
 __device__ __forceinline__ float warp_transpose_reduce32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool up = (lane & half) != 0;
-#pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float send = up ? v[i] : v[i + half];
-      const float keep = up ? v[i + half] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-    }
-  }
+  transpose_reduce_step<16>(v, lane);
   return v[0];
 }
 
@@ -427,12 +436,13 @@ struct SysSmem {
   double Hs[36], Ms[36], Ts[36], vs[6];
 };
 
-// items first, first + stride, ... ; NT threads per block (poses not __restrict__, see above)
+// items first, first + stride, ... ; NT threads per block (poses not __restrict__, see above);
+// accumulates into sys ([n*n + n], zeroed by the caller)
 template <int NT>
 __device__ __forceinline__ void system_items(const float* poses, const int64_t* __restrict__ ii,
                                              const int64_t* __restrict__ jj, const BaDims& d,
-                                             const BaWs& ws, int motion_only, int bid, int nb,
-                                             SysSmem& sm) {
+                                             const BaWs& ws, double* sys, int motion_only, int bid,
+                                             int nb, SysSmem& sm) {
   float (*red)[64] = sm.red;
   double* Hs = sm.Hs; double* Ms = sm.Ms; double* Ts = sm.Ts; double* vs = sm.vs;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -440,8 +450,8 @@ __device__ __forceinline__ void system_items(const float* poses, const int64_t* 
   const int npairs = motion_only ? 0 : ws.counts[2];
   constexpr int kChunk = 4 * NT;                     // pixels per Schur work unit (4 per thread)
   const int nchunk = (d.hw + kChunk - 1) / kChunk;
-  double* H = ws.sys;
-  double* bvec = ws.sys + (size_t)d.n * d.n;
+  double* H = sys;
+  double* bvec = sys + (size_t)d.n * d.n;
 
   // ---------------- pose blocks of the edges ----------------
   // Edges go to the blocks at the END of the grid: the Schur ranges below fill it from the front
@@ -482,9 +492,11 @@ __device__ __forceinline__ void system_items(const float* poses, const int64_t* 
       const int c = tid - 32;
       GsSE3 G;
       gs_edge_pose(poses, ix, jx, G);
-      float X[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, Y[6];
-      X[c] = 1.0f;
+      float X[6], Y[6];
+#pragma unroll
+      for (int r = 0; r < 6; ++r) X[r] = (r == c) ? 1.0f : 0.0f;     // constant indices: X stays in registers
       gs_adjT(G, X, Y);
+#pragma unroll
       for (int r = 0; r < 6; ++r) Ms[r * 6 + c] = (double)Y[r];
     }
     __syncthreads();
@@ -629,7 +641,7 @@ ba_system_kernel(const float* poses, const int64_t* __restrict__ ii,
                  const int64_t* __restrict__ jj, BaDims d, BaWs ws, int motion_only) {
   __shared__ SysSmem sm;
   if (ws.counts[4]) return;
-  system_items<256>(poses, ii, jj, d, ws, motion_only, blockIdx.x, gridDim.x, sm);
+  system_items<256>(poses, ii, jj, d, ws, ws.sys, motion_only, blockIdx.x, gridDim.x, sm);
 }
 
 // ------------------------------------------------------------------------------------
@@ -1412,10 +1424,16 @@ ba_backsub_kernel(float* disps, BaDims d, BaWs ws, int owner_lo, int owner_hi, f
 }
 
 // ------------------------------------------------------------------------------------
-// Small windows: ALL Gauss-Newton iterations of one call in ONE cooperative kernel.  The phases
-// are separated by grid barriers instead of kernel boundaries, and the depth back-substitution
-// of iteration i runs fused with the linearisation of iteration i+1 (same pixel, same thread).
-// 3 grid barriers per iteration replace 5 launches.
+// Small windows: ALL Gauss-Newton iterations of one call in ONE cooperative kernel, and the depth
+// back-substitution of iteration i runs fused with the linearisation of iteration i+1 (same pixel,
+// same thread).  Per iteration, instead of 5 launches:
+//   linearise -> system: one grid barrier (every system item reads partials of many blocks);
+//   system -> solve:     every block counts one arrival (release) and moves on; only block 0, which
+//                        solves, waits for all of them (acquire);
+//   solve -> next iteration: block 0 publishes the number of solved iterations (release) after dx
+//                        and the retracted poses are written; the other blocks wait for it (acquire).
+// The reduced system alternates between two buffers by iteration parity: the grid zeroes the next
+// iteration's buffer during the linearisation, so block 0 does not zero it on the serial path.
 // ------------------------------------------------------------------------------------
 #ifdef GOSLAM_BA_PROBE
 #define BA_PROBE(slot) do { if (threadIdx.x == 0 && blockIdx.x == 0) probe[slot] = clock64(); } while (0)
@@ -1423,26 +1441,46 @@ ba_backsub_kernel(float* disps, BaDims d, BaWs ws, int owner_lo, int owner_hi, f
 #define BA_PROBE(slot) do {} while (0)
 #endif
 
-__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& epoch) {
+// the block's writes so far are released to the grid; one arrival on *counter, no waiting
+__device__ __forceinline__ void block_arrive(unsigned* counter) {
   __syncthreads();
-  ++epoch;
   if (threadIdx.x == 0) {
     __threadfence();
     atomicAdd(counter, 1u);
-    const unsigned target = epoch * gridDim.x;
+  }
+}
+
+// wait until *word >= target (acquire): the block then sees everything released before it got there
+__device__ __forceinline__ void block_wait_at_least(const unsigned* word, unsigned target) {
+  if (threadIdx.x == 0) {
     unsigned v;
     do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(word) : "memory");
     } while (v < target);
     __threadfence();
   }
   __syncthreads();
 }
 
+// the block's writes so far are released to the grid together with *word = value
+__device__ __forceinline__ void block_publish(unsigned* word, unsigned value) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(word), "r"(value) : "memory");
+  }
+}
+
+__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& epoch) {
+  block_arrive(counter);
+  ++epoch;
+  block_wait_at_least(counter, epoch * gridDim.x);
+}
+
 __global__ void __launch_bounds__(kTP)
 ba_persistent_kernel(float* poses, float* disps, BaIn in, BaDims d, BaWs ws, int iterations, float lm,
                      float ep, int motion_only, float* dx_out, float* dz_out, int* status_out,
-                     unsigned* barrier) {
+                     unsigned* barrier, unsigned* arrived, unsigned* solved) {
   extern __shared__ double smd[];
   __shared__ SysSmem sys_sm;
   __shared__ SolveSmem solve_sm;
@@ -1458,7 +1496,7 @@ ba_persistent_kernel(float* poses, float* disps, BaIn in, BaDims d, BaWs ws, int
   const int units = M * nwt;
   const int ufirst = (threadIdx.x >> 5) * gridDim.x + blockIdx.x, ustep = (kTP / 32) * gridDim.x;
   const size_t nsys = (size_t)d.n * d.n + d.n;
-  if (dz_out) {                      // rows of frames without a depth update stay 0 (first written after 3 barriers)
+  if (dz_out) {                      // rows of frames without a depth update stay 0 (first written after the first grid barrier)
     const size_t ndz = (size_t)d.num * d.hw;
     for (size_t i = (size_t)blockIdx.x * kTP + threadIdx.x; i < ndz; i += (size_t)gridDim.x * kTP) dz_out[i] = 0.f;
   }
@@ -1474,10 +1512,15 @@ ba_persistent_kernel(float* poses, float* disps, BaIn in, BaDims d, BaWs ws, int
 #ifdef GOSLAM_BA_PROBE
     const long long tl0 = clock64();
 #endif
+    double* const sys = (it & 1) ? ws.sys_alt : ws.sys;
     for (int u = ufirst; u < units; u += ustep) {
       const int k = u / nwt, wt = u - k * nwt;
       if (it > 0 && !motion_only) backsub_tile(disps, d, ws, 0, d.num, dz_out, k, wt);
       linearize_tile(in, d, ws, motion_only, k, wt);
+    }
+    if (it + 1 < iterations) {        // the other buffer's last reader was the solve of iteration it - 1
+      double* const next = (it & 1) ? ws.sys : ws.sys_alt;
+      for (size_t i = (size_t)blockIdx.x * kTP + threadIdx.x; i < nsys; i += (size_t)gridDim.x * kTP) next[i] = 0.0;
     }
 #ifdef GOSLAM_BA_PROBE
     if (threadIdx.x == 0 && blockIdx.x < 1024) g_phase_cycles[0][blockIdx.x] = (int)(clock64() - tl0);
@@ -1488,23 +1531,24 @@ ba_persistent_kernel(float* poses, float* disps, BaIn in, BaDims d, BaWs ws, int
 #ifdef GOSLAM_BA_PROBE
     const long long ts0 = clock64();
 #endif
-    system_items<kTP>(poses, in.ii, in.jj, d, ws, motion_only, blockIdx.x, gridDim.x, sys_sm);
+    system_items<kTP>(poses, in.ii, in.jj, d, ws, sys, motion_only, blockIdx.x, gridDim.x, sys_sm);
 #ifdef GOSLAM_BA_PROBE
     if (threadIdx.x == 0 && blockIdx.x < 1024) g_phase_cycles[1][blockIdx.x] = (int)(clock64() - ts0);
 #endif
     BA_PROBE(3);
-    grid_barrier(barrier, epoch);
-    BA_PROBE(4);
+    block_arrive(arrived);
     if (blockIdx.x == 0) {
+      block_wait_at_least(arrived, (unsigned)(it + 1) * gridDim.x);
+      BA_PROBE(4);
       SysSrc local{};
-      local.p[0] = ws.sys; local.n = 1;
+      local.p[0] = sys; local.n = 1;
       solve_small(poses, d, ws, local, lm, ep, dx_out, status_out ? status_out + it : nullptr, smd,
                   solve_sm);
-      __syncthreads();
-      for (size_t i = threadIdx.x; i < nsys; i += kTP) ws.sys[i] = 0.0;   // for the next iteration
+      BA_PROBE(5);
+      block_publish(solved, it + 1);
+    } else {
+      block_wait_at_least(solved, it + 1);
     }
-    BA_PROBE(5);
-    grid_barrier(barrier, epoch);
     BA_PROBE(6);
 #ifdef GOSLAM_BA_PROBE
     if (threadIdx.x == 0 && blockIdx.x == 0 && it == iterations - 1) {
@@ -1522,7 +1566,7 @@ ba_persistent_kernel(float* poses, float* disps, BaIn in, BaDims d, BaWs ws, int
              g_solve_probe[1] - g_solve_probe[0], g_solve_probe[2] - g_solve_probe[1],
              g_solve_probe[3] - g_solve_probe[2], g_solve_probe[4] - g_solve_probe[3]);
     if (threadIdx.x == 0 && blockIdx.x == 0)
-      printf("[ba probe it=%d] linearize %lld | barrier %lld | system %lld | barrier %lld | solve %lld | barrier %lld (cycles)\n",
+      printf("[ba probe it=%d] linearize %lld | barrier %lld | system %lld | wait for arrivals %lld | solve %lld | publish %lld (cycles)\n",
              it, probe[1] - probe[0], probe[2] - probe[1], probe[3] - probe[2], probe[4] - probe[3],
              probe[5] - probe[4], probe[6] - probe[5]);
 #endif
@@ -1563,7 +1607,12 @@ void ba_persistent_kernel_attrs(BaDevice* dv, int dev) {
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
   cudaFuncSetAttribute(ba_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ba_persistent_kernel, kTP, smem_max);
-  constexpr int kWant = 2;    // 2 blocks/SM: chosen on the B200 version, not re-measured on the H100
+#ifndef GOSLAM_BA_BLOCKS_PER_SM     // build-time A/B switch (tools/build_variant.py), never set in the shipped library
+#define GOSLAM_BA_BLOCKS_PER_SM 2
+#endif
+  // 2 blocks/SM (H100 80GB HBM3, 700 W, main leg): 99.8 us per call against 111.9 us with 1 block/SM; the
+  // second block halves the linearise rounds and the Schur units per block, which outweighs its barrier arrivals
+  constexpr int kWant = GOSLAM_BA_BLOCKS_PER_SM;
   dv->blocks_per_sm = (!coop || occ < 1) ? 0 : (occ > kWant ? kWant : occ);
 }
 
@@ -1696,16 +1745,18 @@ int goslam_ba(float* poses, float* disps, const float* intrinsics, const float* 
     const int blocks_per_sm = dv.blocks_per_sm, sms = dv.sms;
     const size_t smem = ((size_t)d.n * d.n + 2 * d.n) * sizeof(double);
     if (blocks_per_sm > 0) {
-      // two launches per call: the table kernel (which also zeroes the reduced system and the barrier
-      // counter) and the cooperative kernel (which zeroes dz_out itself)
+      // two launches per call: the table kernel (which also zeroes the first reduced system and the
+      // sync counters) and the cooperative kernel (which zeroes dz_out itself)
       ba_prep_kernel<<<1, kPrepThreads, prep_smem_bytes(d.num), st>>>(ii, jj, d, ws, 1, motion_only ? 0 : eta_rows);
       GS_CHECK_LAUNCH();
       unsigned* barrier = reinterpret_cast<unsigned*>(ws.counts + 3);
+      unsigned* arrived = reinterpret_cast<unsigned*>(ws.counts + 5);
+      unsigned* solved = reinterpret_cast<unsigned*>(ws.counts + 6);
       BaIn in{poses, disps, intrinsics, disps_sens, targets, weights, eta, eta_rows, ii, jj};
       BaDims dd = d;
       BaWs wsv = ws;
       void* args[] = {&poses, &disps, &in, &dd, &wsv, &iterations, &lm, &ep, &motion_only,
-                      &dx_out, &dz_out, &status_out, &barrier};
+                      &dx_out, &dz_out, &status_out, &barrier, &arrived, &solved};
       const cudaError_t le = cudaLaunchCooperativeKernel((const void*)ba_persistent_kernel,
                                                          dim3(sms * blocks_per_sm), dim3(kTP), args, smem, st);
       if (le != cudaSuccess) { gs_note_cuda_error(le); return GOSLAM_ELAUNCH; }
