@@ -29,9 +29,11 @@ def install(force=True):
 
 
 def __getattr__(name):
-    """goslam_b200.FactorGraph / DepthVideo / CorrBlock / AltCorrBlock / InstantNeuS, imported on first use"""
+    """goslam_b200.FactorGraph / DepthVideo / MultiviewFilter / CorrBlock / AltCorrBlock / InstantNeuS, imported on
+    first use"""
     import importlib
-    where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video", "CorrBlock": ".modules.corr",
+    where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video",
+             "MultiviewFilter": ".multiview_filter", "CorrBlock": ".modules.corr",
              "AltCorrBlock": ".modules.corr", "InstantNeuS": ".neus"}
     if name in where:
         return getattr(importlib.import_module(where[name], __name__), name)

@@ -84,6 +84,10 @@ SIGNATURES = {
     "goslam_projmap": (c_int, [c_void_p] * 7 + [c_int] * 3 + [c_void_p]),
     "goslam_iproj": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
     "goslam_depth_filter": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p]),
+    "goslam_mvfilter_workspace_bytes": (c_size_t, [c_int] * 3),
+    "goslam_mvfilter_compute": (c_int, [c_void_p] * 4 + [c_float, c_int, c_int] + [c_int] * 3 +
+                                [c_void_p, c_size_t, c_void_p]),
+    "goslam_mvfilter_commit": (c_int, [c_void_p] * 3 + [c_size_t] + [c_int] * 3 + [c_void_p] * 8),
     "goslam_reproject": (c_int, [c_void_p] * 7 + [c_int] * 3 + [c_void_p]),
     "goslam_reproject_motion": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_void_p]),
     "goslam_ba_workspace_bytes": (c_size_t, [c_int] * 6),

@@ -5,6 +5,9 @@
 #include "common.cuh"
 #include "se3.cuh"
 
+#include <algorithm>
+#include <climits>
+
 namespace {
 
 constexpr int kThreads = 256;
@@ -199,25 +202,31 @@ reproject_kernel(const float* __restrict__ poses, const float* __restrict__ disp
 // ---------------------------------------------------------------------------------
 // iproj  (reference: src/lib/droid_kernels.cu:779-850)
 // ---------------------------------------------------------------------------------
+// world point of pixel (u, v) with inverse depth d under pose p = (t, q); shared with the multiview filter so that
+// its points are iproj's, bit for bit.  d = 0 gives inf / NaN components, as in the reference.
+__device__ __forceinline__ void iproj_point(const float* __restrict__ p, float fx, float fy, float cx, float cy,
+                                            float u, float v, float d, float* o) {
+  GsSE3 G;
+  G.t[0] = p[0]; G.t[1] = p[1]; G.t[2] = p[2];
+  G.q[0] = p[3]; G.q[1] = p[4]; G.q[2] = p[5]; G.q[3] = p[6];
+  float Xi[4] = {(u - cx) / fx, (v - cy) / fy, 1.f, d};
+  float Xj[4];
+  gs_act4(G, Xi, Xj);
+  o[0] = Xj[0] / Xj[3];
+  o[1] = Xj[1] / Xj[3];
+  o[2] = Xj[2] / Xj[3];
+}
+
 __global__ void __launch_bounds__(kThreads)
 iproj_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
              const float* __restrict__ intr, float* __restrict__ points, int ht, int wd) {
   const int f = blockIdx.y;
   const int k = blockIdx.x * kThreads + threadIdx.x;
   if (k >= ht * wd) return;
-  GsSE3 G;
-  const float* p = poses + 7 * (size_t)f;
-  G.t[0] = p[0]; G.t[1] = p[1]; G.t[2] = p[2];
-  G.q[0] = p[3]; G.q[1] = p[4]; G.q[2] = p[5]; G.q[3] = p[6];
   const float fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3];
-  const float u = (float)(k % wd), v = (float)(k / wd);
-  float Xi[4] = {(u - cx) / fx, (v - cy) / fy, 1.f, disps[(size_t)f * ht * wd + k]};
-  float Xj[4];
-  gs_act4(G, Xi, Xj);
   float* o = points + ((size_t)f * ht * wd + k) * 3;
-  o[0] = Xj[0] / Xj[3];
-  o[1] = Xj[1] / Xj[3];
-  o[2] = Xj[2] / Xj[3];
+  iproj_point(poses + 7 * (size_t)f, fx, fy, cx, cy, (float)(k % wd), (float)(k / wd), disps[(size_t)f * ht * wd + k],
+              o);
 }
 
 // ---------------------------------------------------------------------------------
@@ -226,16 +235,8 @@ iproj_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
 // its own 6 neighbour votes, so we loop the 6 neighbours inside one thread instead:
 // same counts, no atomics, no memset.
 // ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads)
-depth_filter_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
-                    const float* __restrict__ intr, const int64_t* __restrict__ inds,
-                    const float* __restrict__ thresh, float* __restrict__ counter,
-                    int num, int ht, int wd) {
-  const int b = blockIdx.y;
-  const int k = blockIdx.x * kThreads + threadIdx.x;
-  const int ix = (int)inds[b];
-  __shared__ GsSE3 G[6];
-  __shared__ int jxs[6];
+// relative poses frame ix -> its 6 neighbours ix-1, ix-2, ix-3, ix+3, ix+4, ix+5 (threads 0..5 of the block)
+__device__ __forceinline__ void vote_neighbours(const float* __restrict__ poses, int ix, int num, GsSE3* G, int* jxs) {
   if (threadIdx.x < 6) {
     const int nb = threadIdx.x;
     const int jx = (nb < 3) ? ix - nb - 1 : ix + nb;
@@ -246,13 +247,14 @@ depth_filter_kernel(const float* __restrict__ poses, const float* __restrict__ d
       gs_rel(pi, pi + 3, pj, pj + 3, G[nb]);
     }
   }
-  __syncthreads();
-  if (k >= ht * wd) return;
-  const float t = thresh[b];
-  const float fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3];
-  const int i = k / wd, j = k % wd;
+}
+
+// number of neighbours whose inverse depth agrees with pixel k = (i, j) of a frame with inverse depth d
+__device__ __forceinline__ float depth_votes(const GsSE3* G, const int* jxs, const float* __restrict__ disps,
+                                             float fx, float fy, float cx, float cy, float t, float d, int i, int j,
+                                             int num, int ht, int wd) {
   const float ui = (float)j, vi = (float)i;
-  float Xi[4] = {(ui - cx) / fx, (vi - cy) / fy, 1.f, disps[(size_t)ix * ht * wd + k]};
+  float Xi[4] = {(ui - cx) / fx, (vi - cy) / fy, 1.f, d};
   float count = 0.f;
 #pragma unroll
   for (int nb = 0; nb < 6; ++nb) {
@@ -279,7 +281,324 @@ depth_filter_kernel(const float* __restrict__ poses, const float* __restrict__ d
       else if (fabs(inv - 1.0 / d11) < t) count += 1.0f;
     }
   }
-  counter[(size_t)b * ht * wd + k] = count;
+  return count;
+}
+
+__global__ void __launch_bounds__(kThreads)
+depth_filter_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
+                    const float* __restrict__ intr, const int64_t* __restrict__ inds,
+                    const float* __restrict__ thresh, float* __restrict__ counter,
+                    int num, int ht, int wd) {
+  const int b = blockIdx.y;
+  const int k = blockIdx.x * kThreads + threadIdx.x;
+  const int ix = (int)inds[b];
+  __shared__ GsSE3 G[6];
+  __shared__ int jxs[6];
+  vote_neighbours(poses, ix, num, G, jxs);
+  __syncthreads();
+  if (k >= ht * wd) return;
+  const float t = thresh[b];
+  const float fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3];
+  const int i = k / wd, j = k % wd;
+  counter[(size_t)b * ht * wd + k] =
+      depth_votes(G, jxs, disps, fx, fy, cx, cy, t, disps[(size_t)ix * ht * wd + k], i, j, num, ht, wd);
+}
+
+// ---------------------------------------------------------------------------------
+// Multiview filter  (reference: src/multiview_filter.py:98-170, one pass of MultiviewFilter.forward).
+// Four launches over T frames at full resolution, no host synchronisation:
+//   mv_mean_kernel    per-frame mean inverse depth (fp64 sum in a fixed order, rounded to fp32);
+//                     block 0 also resets the reduction state of the pass.
+//   mv_vote_kernel    depth_filter's vote + mask1 = count >= visible_num && d > 0.01 * mean, mask1 bytes,
+//                     count and min / max of the mask1 world points (the first bound).
+//   mv_extend_kernel  extended mask (all / mask1 / box dilation of mask1), AND the strict in-bound test against
+//                     the first bound, final mask bytes, counts and min / max of the final points (second bound).
+//   mv_commit_kernel  (separate entry point, called under the mapping lock) gated on the device: priority,
+//                     poses / disps / mask / bound / filtered_id of the video, and a status record.
+// Min / max / counts are integer atomics (floats mapped to order-preserving ints), so the bounds are exact and the
+// pass is deterministic whatever the block order.  Points are recomputed in the extend pass, not stored.
+// ---------------------------------------------------------------------------------
+constexpr int kMvPerThread = 8;                      // pixels per thread of the vote / extend passes
+constexpr int kMvTile = kThreads * kMvPerThread;
+constexpr int kMvMeanThreads = 512;
+constexpr int kMvMaxRadius = 15;
+
+struct MvState {
+  int mn1[3], mx1[3];                 // first bound (mask1 points), order-preserving ints
+  int mn2[3], mx2[3];                 // second bound (final points)
+  unsigned long long n1, n_ext, n_fin;
+};
+constexpr size_t kMvStateBytes = 256;
+static_assert(sizeof(MvState) <= kMvStateBytes, "MvState");
+
+__host__ __device__ constexpr size_t mv_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+struct MvLayout {
+  size_t mean, mask1, fin, total;
+  __host__ __device__ MvLayout(int T, size_t hw) {
+    mean = kMvStateBytes;
+    mask1 = mean + mv_align((size_t)T * sizeof(float));
+    fin = mask1 + mv_align((size_t)T * hw);
+    total = fin + mv_align((size_t)T * hw);
+  }
+};
+
+// float -> int with the same order (-0 sorts below +0); the map is its own inverse
+__device__ __forceinline__ int mv_ord(float f) {
+  const int i = __float_as_int(f);
+  return i >= 0 ? i : i ^ 0x7fffffff;
+}
+__device__ __forceinline__ float mv_unord(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
+
+// get_bound_from_pointcloud(pts) with its default enlarge_scale = 1.0, in torch's fp32 op order
+// (src/multiview_filter.py:82-96): len = (max - min) * 0, bound = [min - len / 2, max + len / 2]
+__device__ __forceinline__ void mv_bound(const int* omn, const int* omx, float* lo, float* hi) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float mn = mv_unord(omn[c]), mx = mv_unord(omx[c]);
+    const float len = __fmul_rn(__fsub_rn(mx, mn), 0.0f);
+    lo[c] = __fadd_rn(mn, __fdiv_rn(-len, 2.0f));
+    hi[c] = __fadd_rn(mx, __fdiv_rn(len, 2.0f));
+  }
+}
+
+// per-thread partial of one pass: points (count + min / max per axis) and, in the extend pass, extended pixels
+struct MvAcc {
+  int mn[3], mx[3];
+  unsigned n, e;
+  __device__ MvAcc() : mn{INT_MAX, INT_MAX, INT_MAX}, mx{INT_MIN, INT_MIN, INT_MIN}, n(0), e(0) {}
+  __device__ void add(const float* p) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const int o = mv_ord(p[c]);
+      mn[c] = min(mn[c], o);
+      mx[c] = max(mx[c], o);
+    }
+    ++n;
+  }
+};
+
+// block reduction of MvAcc, then one set of atomics per block (skipped when the block saw nothing).
+// Every thread of the block must call it.
+__device__ __forceinline__ void mv_flush(MvAcc& a, int* gmn, int* gmx, unsigned long long* gn,
+                                         unsigned long long* ge) {
+  __shared__ MvAcc part[kThreads / 32];
+  const unsigned full = 0xffffffffu;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    a.mn[c] = __reduce_min_sync(full, a.mn[c]);
+    a.mx[c] = __reduce_max_sync(full, a.mx[c]);
+  }
+  a.n = __reduce_add_sync(full, a.n);
+  a.e = __reduce_add_sync(full, a.e);
+  const int warp = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) part[warp] = a;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    MvAcc b = part[0];
+    for (int w = 1; w < kThreads / 32; ++w) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        b.mn[c] = min(b.mn[c], part[w].mn[c]);
+        b.mx[c] = max(b.mx[c], part[w].mx[c]);
+      }
+      b.n += part[w].n;
+      b.e += part[w].e;
+    }
+    if (b.n) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        atomicMin(gmn + c, b.mn[c]);
+        atomicMax(gmx + c, b.mx[c]);
+      }
+      atomicAdd(gn, (unsigned long long)b.n);
+    }
+    if (ge && b.e) atomicAdd(ge, (unsigned long long)b.e);
+  }
+}
+
+__global__ void __launch_bounds__(kMvMeanThreads)
+mv_mean_kernel(const float* __restrict__ disps, float* __restrict__ mean, MvState* __restrict__ st, int T, int hw) {
+  const int f = blockIdx.x;
+  if (f == 0 && threadIdx.x == 0) {
+    for (int c = 0; c < 3; ++c) {
+      st->mn1[c] = st->mn2[c] = INT_MAX;
+      st->mx1[c] = st->mx2[c] = INT_MIN;
+    }
+    st->n1 = st->n_ext = st->n_fin = 0ull;
+  }
+  if (f >= T) return;
+  // fixed order: thread t sums pixels t, t + 512, ... in fp64, then a fixed shuffle tree and a warp-0 tree
+  const float* d = disps + (size_t)f * hw;
+  double s = 0.0;
+  for (int k = threadIdx.x; k < hw; k += kMvMeanThreads) s += (double)d[k];
+  __shared__ double red[kMvMeanThreads / 32];
+#pragma unroll
+  for (int off = 16; off; off >>= 1) s += __shfl_down_sync(0xffffffffu, s, off);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    s = threadIdx.x < kMvMeanThreads / 32 ? red[threadIdx.x] : 0.0;
+#pragma unroll
+    for (int off = 8; off; off >>= 1) s += __shfl_down_sync(0xffffffffu, s, off);
+    if (threadIdx.x == 0) mean[f] = (float)(s / (double)hw);
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+mv_vote_kernel(const float* __restrict__ poses, const float* __restrict__ poses_world,
+               const float* __restrict__ disps, const float* __restrict__ intr, const float* __restrict__ mean,
+               float thresh, float visible, unsigned char* __restrict__ mask1, MvState* __restrict__ st, int T,
+               int ht, int wd) {
+  const int f = blockIdx.y;
+  const int hw = ht * wd;
+  __shared__ GsSE3 G[6];
+  __shared__ int jxs[6];
+  vote_neighbours(poses, f, T, G, jxs);
+  __syncthreads();
+  const float fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3];
+  const float dmin = __fmul_rn(0.01f, mean[f]);       // torch: 0.01 * mean in fp32
+  const float* dsp = disps + (size_t)f * hw;
+  const float* pw = poses_world + 7 * (size_t)f;
+  MvAcc acc;
+  for (int r = 0; r < kMvPerThread; ++r) {
+    const int k = blockIdx.x * kMvTile + r * kThreads + threadIdx.x;
+    if (k >= hw) break;
+    const int i = k / wd, j = k % wd;
+    const float d = dsp[k];
+    const float count = depth_votes(G, jxs, disps, fx, fy, cx, cy, thresh, d, i, j, T, ht, wd);
+    const bool m = count >= visible && d > dmin;
+    mask1[(size_t)f * hw + k] = m;
+    if (m) {
+      float p[3];
+      iproj_point(pw, fx, fy, cx, cy, (float)j, (float)i, d, p);
+      acc.add(p);
+    }
+  }
+  mv_flush(acc, st->mn1, st->mx1, &st->n1, nullptr);
+}
+
+// radius < 0: every pixel ('inf'); 0: mask1; > 0: mask1 dilated by a (2r+1)^2 box with zero padding
+// (F.conv2d(mask, ones(k, k), padding=k // 2).bool()).
+__global__ void __launch_bounds__(kThreads)
+mv_extend_kernel(const float* __restrict__ poses_world, const float* __restrict__ disps, const float* __restrict__ intr,
+                 const unsigned char* __restrict__ mask1, unsigned char* __restrict__ fin, MvState* __restrict__ st,
+                 int radius, int ht, int wd) {
+  const int f = blockIdx.y;
+  const int hw = ht * wd;
+  float lo[3], hi[3];
+  mv_bound(st->mn1, st->mx1, lo, hi);
+  const float fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3];
+  const float* dsp = disps + (size_t)f * hw;
+  const unsigned char* m1 = mask1 + (size_t)f * hw;
+  const float* pw = poses_world + 7 * (size_t)f;
+  MvAcc acc;
+  for (int r = 0; r < kMvPerThread; ++r) {
+    const int k = blockIdx.x * kMvTile + r * kThreads + threadIdx.x;
+    if (k >= hw) break;
+    const int i = k / wd, j = k % wd;
+    bool e;
+    if (radius < 0) {
+      e = true;
+    } else if (radius == 0) {
+      e = m1[k];
+    } else {
+      e = false;
+      const int y0 = max(i - radius, 0), y1 = min(i + radius, ht - 1);
+      const int x0 = max(j - radius, 0), x1 = min(j + radius, wd - 1);
+      for (int y = y0; y <= y1 && !e; ++y)
+        for (int x = x0; x <= x1; ++x)
+          if (m1[y * wd + x]) { e = true; break; }
+    }
+    bool keep = false;
+    if (e) {
+      ++acc.e;
+      float p[3];
+      iproj_point(pw, fx, fy, cx, cy, (float)j, (float)i, dsp[k], p);
+      // strict, as in_bound (src/multiview_filter.py:64-79): inf / NaN points of d = 0 fail every comparison
+      keep = p[0] > lo[0] && p[0] < hi[0] && p[1] > lo[1] && p[1] < hi[1] && p[2] > lo[2] && p[2] < hi[2];
+      if (keep) acc.add(p);
+    }
+    fin[(size_t)f * hw + k] = keep;
+  }
+  mv_flush(acc, st->mn2, st->mx2, &st->n_fin, &st->n_ext);
+}
+
+// quaternion -> (roll, pitch, yaw) of MultiviewFilter.pose_dist, op for op in fp32 (src/multiview_filter.py:30-52);
+// explicit roundings keep nvcc from contracting what torch evaluates as separate kernels
+__device__ __forceinline__ void mv_euler(const float* p, float* e) {
+  const float x = p[3], y = p[4], z = p[5], w = p[6];
+  const float t0 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(w, x), __fmul_rn(y, z)));
+  const float t1 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))));
+  e[0] = atan2f(t0, t1);
+  float t2 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(w, y), __fmul_rn(z, x)));
+  t2 = t2 < -1.0f ? -1.0f : (t2 > 1.0f ? 1.0f : t2);     // torch.clamp keeps NaN
+  e[1] = asinf(t2);
+  const float t3 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(w, z), __fmul_rn(x, y)));
+  const float t4 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, y), __fmul_rn(z, z))));
+  e[2] = atan2f(t3, t4);
+}
+
+// 1 * |dt|_1 + 2 * |d euler|_1 (BundleFusion Sec. 5.3, src/multiview_filter.py:54-61)
+__device__ __forceinline__ float mv_pose_dist(const float* p0, const float* p1) {
+  float e0[3], e1[3];
+  mv_euler(p0, e0);
+  mv_euler(p1, e1);
+  const float st = __fadd_rn(__fadd_rn(fabsf(__fsub_rn(p0[0], p1[0])), fabsf(__fsub_rn(p0[1], p1[1]))),
+                             fabsf(__fsub_rn(p0[2], p1[2])));
+  const float sr = __fadd_rn(__fadd_rn(fabsf(__fsub_rn(e0[0], e1[0])), fabsf(__fsub_rn(e0[1], e1[1]))),
+                             fabsf(__fsub_rn(e0[2], e1[2])));
+  return __fadd_rn(__fmul_rn(1.0f, st), __fmul_rn(2.0f, sr));
+}
+
+// The reference returns a second time when extended_masks.sum() < 100 (src/multiview_filter.py:142-143).  That
+// cannot happen once masks.sum() >= 100: every extension mode contains mask1 (all pixels, mask1 itself, or a
+// dilation whose box includes the centre pixel), so the gate below needs only the mask1 count.  An empty final
+// point set is where the reference's torch.min raises; nothing is committed and the status says why.
+__global__ void __launch_bounds__(kThreads)
+mv_commit_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
+                 const unsigned char* __restrict__ fin, const MvState* __restrict__ st, int T, size_t n,
+                 float* __restrict__ poses_filtered, float* __restrict__ disps_filtered,
+                 float* __restrict__ mask_filtered, float* __restrict__ update_priority,
+                 int* __restrict__ filtered_id, float* __restrict__ bound, int64_t* __restrict__ status) {
+  const size_t gid = (size_t)blockIdx.x * kThreads + threadIdx.x;
+  const bool commit = st->n1 >= 100ull && st->n_fin > 0ull;
+  if (gid == 0) {
+    status[0] = (int64_t)st->n1;
+    status[1] = (int64_t)st->n_ext;
+    status[2] = (int64_t)st->n_fin;
+    status[3] = commit ? 1 : 0;
+  }
+  if (!commit) return;
+  if (gid < (size_t)T) {
+    float* pf = poses_filtered + 7 * gid;
+    const float* p = poses + 7 * gid;
+    update_priority[gid] = __fadd_rn(update_priority[gid], mv_pose_dist(pf, p));
+#pragma unroll
+    for (int c = 0; c < 7; ++c) pf[c] = p[c];
+  }
+  if (gid == 0) {
+    float lo[3], hi[3];
+    mv_bound(st->mn2, st->mx2, lo, hi);
+    for (int c = 0; c < 3; ++c) {
+      bound[2 * c] = lo[c];
+      bound[2 * c + 1] = hi[c];
+    }
+    *filtered_id = T;
+  }
+  // mask and inverse depth of the T frames: 4 pixels per thread, grid-stride, scalar tail
+  const size_t n4 = n / 4;
+  const size_t stride = (size_t)gridDim.x * kThreads;
+  for (size_t q = gid; q < n4; q += stride) {
+    const uchar4 m = reinterpret_cast<const uchar4*>(fin)[q];
+    reinterpret_cast<float4*>(mask_filtered)[q] =
+        make_float4(m.x ? 1.f : 0.f, m.y ? 1.f : 0.f, m.z ? 1.f : 0.f, m.w ? 1.f : 0.f);
+    reinterpret_cast<float4*>(disps_filtered)[q] = reinterpret_cast<const float4*>(disps)[q];
+  }
+  for (size_t q = 4 * n4 + gid; q < n; q += stride) {
+    mask_filtered[q] = fin[q] ? 1.f : 0.f;
+    disps_filtered[q] = disps[q];
+  }
 }
 
 }  // namespace
@@ -363,6 +682,57 @@ int goslam_depth_filter(const float* poses, const float* disps, const float* int
   dim3 grid(gs_cdiv(ht * wd, kThreads), K);
   depth_filter_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, ix,
                                                                    thresh, counter, num, ht, wd);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+size_t goslam_mvfilter_workspace_bytes(int T, int ht, int wd) {
+  if (T < 0 || T > 65535 || ht <= 0 || wd <= 0) return 0;
+  return MvLayout(T, (size_t)ht * wd).total;
+}
+
+int goslam_mvfilter_compute(const float* poses, const float* poses_world, const float* disps,
+                            const float* intrinsic, float filter_thresh, int visible_num, int kernel_size, int T,
+                            int ht, int wd, void* workspace, size_t workspace_bytes, void* stream) {
+  if (T < 0 || T > 65535 || ht <= 0 || wd <= 0 || kernel_size < 0) return GOSLAM_EINVAL;
+  if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
+  const int radius = kernel_size == 0 ? -1 : (kernel_size < 2 ? 0 : kernel_size / 2);
+  if (radius > kMvMaxRadius) return GOSLAM_EINVAL;
+  const int hw = ht * wd;
+  const MvLayout L(T, (size_t)hw);
+  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  char* ws = static_cast<char*>(workspace);
+  MvState* st = reinterpret_cast<MvState*>(ws);
+  float* mean = reinterpret_cast<float*>(ws + L.mean);
+  unsigned char* mask1 = reinterpret_cast<unsigned char*>(ws + L.mask1);
+  unsigned char* fin = reinterpret_cast<unsigned char*>(ws + L.fin);
+  cudaStream_t s = (cudaStream_t)stream;
+  mv_mean_kernel<<<T > 0 ? T : 1, kMvMeanThreads, 0, s>>>(disps, mean, st, T, hw);
+  GS_CHECK_LAUNCH();
+  if (T == 0) return GOSLAM_OK;
+  const dim3 grid(gs_cdiv(hw, kMvTile), T);
+  mv_vote_kernel<<<grid, kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, mean, filter_thresh,
+                                           (float)visible_num, mask1, st, T, ht, wd);
+  GS_CHECK_LAUNCH();
+  mv_extend_kernel<<<grid, kThreads, 0, s>>>(poses_world, disps, intrinsic, mask1, fin, st, radius, ht, wd);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+int goslam_mvfilter_commit(const float* poses, const float* disps, const void* workspace, size_t workspace_bytes,
+                           int T, int ht, int wd, float* poses_filtered, float* disps_filtered, float* mask_filtered,
+                           float* update_priority, int* filtered_id, float* bound, int64_t* status, void* stream) {
+  if (T < 0 || T > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
+  const MvLayout L(T, (size_t)ht * wd);
+  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  const char* ws = static_cast<const char*>(workspace);
+  const size_t n = (size_t)T * ht * wd;
+  const size_t want = std::max<size_t>((n / 4 + kThreads - 1) / kThreads, (size_t)gs_cdiv(T, kThreads));
+  const int blocks = (int)std::min<size_t>(std::max<size_t>(want, 1), 4096);
+  mv_commit_kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
+      poses, disps, reinterpret_cast<const unsigned char*>(ws + L.fin), reinterpret_cast<const MvState*>(ws), T, n,
+      poses_filtered, disps_filtered, mask_filtered, update_priority, filtered_id, bound, status);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

@@ -158,6 +158,27 @@ int goslam_iproj(const float* poses, const float* disps, const float* intrinsics
 int goslam_depth_filter(const float* poses, const float* disps, const float* intrinsics,
                         const int64_t* ix, const float* thresh, float* counter,
                         int K, int num, int ht, int wd, void* stream);
+/* Multiview filter: one pass of MultiviewFilter.forward (src/multiview_filter.py:98-170) over
+ * the first T keyframes at full resolution ht x wd, in two calls on one stream.
+ *   compute: poses [T,7] (w2c snapshot, for depth_filter's votes), poses_world [T,7]
+ *     (w2w * SE3(poses).inv(), for iproj's points), disps [T,ht,wd], intrinsic [4] (scaled to
+ *     full resolution), filter_thresh, visible_num, kernel_size (0 = 'inf', < 2 = no dilation,
+ *     else a box of (k/2)*2+1, radius at most 15).  Writes only the workspace.
+ *   commit: reads the same poses / disps and the workspace; only if the mask1 count is >= 100
+ *     and the final point set is non-empty, it adds pose_dist(poses_filtered, poses) to
+ *     update_priority[:T], then writes poses_filtered[:T], disps_filtered[:T], mask_filtered[:T]
+ *     (0/1 floats), filtered_id[0] = T and bound [3,2].  Always writes
+ *     status[4] = {mask1 count, extended count, final count, committed}.
+ * workspace_bytes returns 0 for invalid sizes. */
+size_t goslam_mvfilter_workspace_bytes(int T, int ht, int wd);
+int goslam_mvfilter_compute(const float* poses, const float* poses_world, const float* disps,
+                            const float* intrinsic, float filter_thresh, int visible_num,
+                            int kernel_size, int T, int ht, int wd, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int goslam_mvfilter_commit(const float* poses, const float* disps, const void* workspace,
+                           size_t workspace_bytes, int T, int ht, int wd, float* poses_filtered,
+                           float* disps_filtered, float* mask_filtered, float* update_priority,
+                           int* filtered_id, float* bound, int64_t* status, void* stream);
 /* reproject = pops.projective_transform(jacobian=False) as called by DepthVideo.reproject
  * (src/depth_video.py:207-217, src/geom/projective_ops.py:114-144) with the lietorch SE3
  * algebra restated from src/lib/droid_kernels.cu:58-107.  intrinsics_all [num,4] (per
