@@ -25,6 +25,10 @@
 // fragment; warp 8 = TMA producer, which keeps a 4-stage ring of (A, B) chunks ahead of the MMAs.
 // fp16 operands, fp32 accumulation, fp32 gate arithmetic, fp16 state — what the reference's autocast region
 // computes (src/factor_graph.py:198, torch.cuda.amp.autocast) with one rounding less per gate.
+// The whole operator (goslam_update_op) rounds to fp16 exactly where it stores: operands (weights except the fp32 w_glo,
+// net, inp, corr, flow in the 7x7 im2col), the encoder outputs c1, c2, f1, f2, the GRU's z, r*net and net' (glo, r and q
+// stay fp32), the hidden layer, a1, the scatter-mean, a2 and upmask; delta, weight and eta are written as fp32.
+// oracle/update_oracle.py (round16=True) restates this in float64.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <mutex>
@@ -188,7 +192,6 @@ conv_tc_kernel(const __grid_constant__ ConvMaps maps, const ConvParams p) {
         asm volatile("bar.sync 2, 256;" ::: "memory");
       }
       if (p.epi == EPI_ACT) {
-        const int act = p.act;
 #pragma unroll
         for (int J = 0; J < N / 8; ++J) {
           const int ch = nt * N + 8 * J + 2 * q;       // output channel of acc[4J + 2*e2 + {0,1}]
@@ -198,8 +201,9 @@ conv_tc_kernel(const __grid_constant__ ConvMaps maps, const ConvParams p) {
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
               float v = acc[4 * J + 2 * e2 + u] + svec[ch + u];
-              // small fused heads: the tile's first 8 channels may switch to act2
-              if (p.split > 0 && ch + u - nt * N < 8 && ch + u >= p.split && p.act2 == ACT_SIGMOID) v = sigmoidf_(v);
+              // small fused heads: channels >= split take act2 instead of act.  A split layer has cout <= 8, so only
+              // J = 0 holds stored channels; testing J (a compile-time constant) keeps every other column's act uniform
+              const int act = (J == 0 && p.split > 0 && ch + u >= p.split) ? p.act2 : p.act;
               if (act == ACT_RELU) v = fmaxf(v, 0.f);
               else if (act == ACT_SIGMOID) v = sigmoidf_(v);
               else if (act == ACT_SOFTPLUS) v = (v > 20.f) ? v : log1pf(__expf(v));
@@ -399,61 +403,10 @@ __global__ void transpose_pad_f16_kernel(const __half* __restrict__ src, __half*
   }
 }
 
-// flow_encoder.0 (src/droid_net.py:84): 7x7 convolution of the 4 motion channels to 128 + ReLU.  K = 196 is too thin for
-// the tensor-core path's 64-channel chunks; CUDA cores: block = 8x16 output patch, thread = (pixel, half of the output
-// channels), the 14x22x4 input halo and the [196][128] weights (fp32) in shared memory, 64 accumulators per thread.
+// flow_encoder.0 (src/droid_net.py:84): 7x7 convolution of the 4 motion channels to 128 + ReLU on tensor cores.
 //   in  [B,4,h,w] f32 (the motion features as FactorGraph hands them over), out [B,h,w,128] f16 NHWC
-constexpr int kF7Halo = (kPY + 6) * (kPX + 6) * 4;
-__global__ void __launch_bounds__(256)
-flow7x7_kernel(const float* __restrict__ in, const float* __restrict__ wgt /*[196][128]: k = (ky*7+kx)*4+ci*/,
-               const float* __restrict__ bias, __half* __restrict__ out, int h, int w) {
-  extern __shared__ float sm7[];
-  float* sw = sm7;                       // [196][128]
-  float* si = sm7 + 196 * 128;           // [14][22][4]
-  const int n_xb = gs_cdiv_dev(w, kPX), n_yb = gs_cdiv_dev(h, kPY);
-  const int xb = blockIdx.x % n_xb, yb = (blockIdx.x / n_xb) % n_yb, b = blockIdx.x / (n_xb * n_yb);
-  for (int i = threadIdx.x; i < 196 * 128; i += 256) sw[i] = wgt[i];
-  for (int i = threadIdx.x; i < kF7Halo; i += 256) {
-    const int ci = i & 3, xx = (i >> 2) % (kPX + 6), yy = (i >> 2) / (kPX + 6);
-    const int gx = xb * kPX + xx - 3, gy = yb * kPY + yy - 3;
-    si[i] = (gx >= 0 && gx < w && gy >= 0 && gy < h) ? in[(((size_t)b * 4 + ci) * h + gy) * w + gx] : 0.f;
-  }
-  __syncthreads();
-  const int pix = threadIdx.x & 127, chh = threadIdx.x >> 7;      // 64 output channels each
-  const int py = pix / kPX, px = pix % kPX;
-  float acc[64];
-#pragma unroll
-  for (int c = 0; c < 64; ++c) acc[c] = bias[chh * 64 + c];
-  for (int ky = 0; ky < 7; ++ky)
-    for (int kx = 0; kx < 7; ++kx) {
-      const float4 v = *reinterpret_cast<const float4*>(si + ((py + ky) * (kPX + 6) + px + kx) * 4);
-      const float* wr = sw + ((ky * 7 + kx) * 4) * 128 + chh * 64;
-#pragma unroll
-      for (int c = 0; c < 64; c += 4) {
-        const float4 w0 = *reinterpret_cast<const float4*>(wr + c);
-        const float4 w1 = *reinterpret_cast<const float4*>(wr + 128 + c);
-        const float4 w2 = *reinterpret_cast<const float4*>(wr + 256 + c);
-        const float4 w3 = *reinterpret_cast<const float4*>(wr + 384 + c);
-        acc[c] += v.x * w0.x + v.y * w1.x + v.z * w2.x + v.w * w3.x;
-        acc[c + 1] += v.x * w0.y + v.y * w1.y + v.z * w2.y + v.w * w3.y;
-        acc[c + 2] += v.x * w0.z + v.y * w1.z + v.z * w2.z + v.w * w3.z;
-        acc[c + 3] += v.x * w0.w + v.y * w1.w + v.z * w2.w + v.w * w3.w;
-      }
-    }
-  const int y = yb * kPY + py, x = xb * kPX + px;
-  if (y < h && x < w) {
-    __half* dst = out + (((size_t)b * h + y) * w + x) * 128 + chh * 64;
-#pragma unroll
-    for (int c = 0; c < 64; c += 8) {
-      __half2 hv[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) hv[j] = __floats2half2_rn(fmaxf(acc[c + 2 * j], 0.f), fmaxf(acc[c + 2 * j + 1], 0.f));
-      *reinterpret_cast<uint4*>(dst + c) = *reinterpret_cast<const uint4*>(hv);
-    }
-  }
-}
-
-// Tensor-core version: im2col in shared memory.  K = 49 taps x 4 channels = 196, zero-padded to 256 = four 64-wide
+constexpr int kF7Halo = (kPY + 6) * (kPX + 6) * 4;   // 14x22x4 input halo of an 8x16 output patch
+// im2col in shared memory.  K = 49 taps x 4 channels = 196, zero-padded to 256 = four 64-wide
 // chunks.  The 128 builder threads (one per output pixel of the 8x16 patch) write their im2col row straight into the
 // K-major SWIZZLE_128B operand layout the TMA would have produced (row r of a chunk at r*128 B inside 8-row / 1024-byte
 // atoms, its 16-byte pieces XOR-ed with r % 8); the weights [128][256] come in once per CTA by TMA; two warpgroups
@@ -772,7 +725,8 @@ int goslam_conv2d_nhwc(const goslam_conv_desc* d, int B, int h, int w, void* str
   if (!d || B < 0 || h <= 0 || w <= 0 || d->n_in < 1 || d->n_in > kMaxIn) return GOSLAM_EINVAL;
   if ((d->taps != 1 && d->taps != 9) || d->cout < 1 || d->cout_pad < d->cout || d->cout_pad % 16) return GOSLAM_EINVAL;
   const int N = d->cout_pad <= kMaxN ? d->cout_pad : (d->cout_pad % 192 == 0 ? 192 : (d->cout_pad % 256 == 0 ? 256 : 128));
-  if (d->cout_pad % N) return GOSLAM_EINVAL;
+  // the epilogue stages the whole bias vector in shared memory
+  if (d->cout_pad % N || d->cout_pad > kVecMax) return GOSLAM_EINVAL;
   if (B == 0) return GOSLAM_OK;
   EncodeTiledFn enc = conv_encode_fn();
   if (!enc) return GOSLAM_ELAUNCH;

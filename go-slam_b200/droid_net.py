@@ -36,9 +36,9 @@ def upsample_disp(disp, mask):
 # ------------------------------------------------------------------------------------------------------
 # The update operator (SURVEY §8f-4): UpdateModule / GraphAgg with the reference's parameter names
 # (src/droid_net.py:33-140), so the `update.*` entries of pretrained/droid.pth load with load_state_dict.
-# The ConvGRU — two thirds of the operator's arithmetic — runs on the wgmma kernel (modules/gru.py); the
-# encoders, heads and the per-frame aggregation are still torch convolutions, evaluated channels-last so that
-# the GRU reads and writes their tensors in place (a channels-last [B,C,h,w] tensor IS the kernel's NHWC).
+# The whole forward is one library call (goslam_update_op, csrc/conv_tc.cu): every 1x1 / 3x3 layer and the
+# ConvGRU on the wgmma implicit-GEMM kernel, the 7x7 motion encoder on a tensor-core im2col kernel, and GraphAgg's
+# per-frame mean on a deterministic scatter-mean kernel, all in NHWC half precision.
 # ------------------------------------------------------------------------------------------------------
 import torch.nn as nn  # noqa: E402
 
@@ -85,10 +85,10 @@ class GraphAgg(nn.Module):
 
 
 class UpdateModule(nn.Module):
-    """src/droid_net.py:70-140 with the reference's parameter names.  Every layer except the 7x7 convolution on the
-    4 motion channels runs on the wgmma implicit-GEMM kernel in NHWC half precision:
+    """src/droid_net.py:70-140 with the reference's parameter names.  Every layer runs on a wgmma kernel in NHWC half
+    precision:
         corr (196 ch, zero-padded to 256) -1x1-> 128 -3x3-> 128          goslam_conv2d_nhwc x2
-        motion (4 ch) -7x7 (torch, channels-last)-> 128 -3x3-> 64         torch + goslam_conv2d_nhwc
+        motion (4 ch) -7x7 (im2col + wgmma)-> 128 -3x3-> 64               flow7x7_tc_kernel + goslam_conv2d_nhwc
         ConvGRU(net, inp, corr, flow)                                     goslam_conv_gru (3 passes)
         delta.0 | weight.0 stacked to 256 outputs, then the two 2-channel heads (fp32 out)   x3
         GraphAgg: 3x3 -> per-source-frame mean -> 3x3 -> {eta 3x3 + softplus, upmask 1x1 -> 576}   x4

@@ -458,7 +458,8 @@ int goslam_nchw_to_nhwc_f16_pad(const void* src, void* dst, int B, int C, int Cp
  * concatenated along channels (each may be a channel slice of a wider tensor), fused bias + activation.
  *   in[i]: [B,h,w,cin_stride[i]] f16, channels cin_off[i] .. cin_off[i]+cin[i] used (all multiples of 64)
  *   weight f16 [taps][cout_pad][sum cin] (tap = 3*ky + kx), bias f32 [cout_pad]; cout_pad multiple of 16 (rows
- *   cout..cout_pad-1 zero) and <= 256 or a multiple of 128 / 192 / 256
+ *   cout..cout_pad-1 zero) and <= 256 or a multiple of 128 / 192 / 256; at most 1024 (the bias vector is staged in
+ *   shared memory), larger layers return GOSLAM_EINVAL
  *   act: 0 none, 1 ReLU, 2 sigmoid, 3 softplus; result * out_scale
  *   out: NHWC [B,h,w,out_stride] f16 (out_f32 = 0; stride and offset multiples of 8) or f32, channels
  *   out_offset .. out_offset + cout written. */

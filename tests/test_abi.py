@@ -79,6 +79,15 @@ def test_argument_validation_without_gpu(lib):
                          1e-4, 0.1, 0, null, null, null, null, 0, null) == -1     # eta missing
     assert lib.goslam_ba(null, null, null, null, null, null, null, 0, null, null, 4, 8, 4, 4, 1, 8, 2,
                          1e-4, 0.1, 1, null, null, null, null, 0, null) == -3     # no workspace
+    # a conv layer wider than the 1024-entry shared-memory bias vector (1152 = 6 x 192 and 1280 = 5 x 256 are otherwise
+    # valid tilings) is rejected as a shape error, even with B = 0 (a library that accepted it returns 0 for the empty
+    # batch, so this never reaches a device)
+    from goslam_b200 import _lib
+    for cout_pad in (1152, 1280):
+        d = _lib.ConvDesc()
+        d.cin[0], d.cin_stride[0], d.n_in = 64, 64, 1
+        d.taps, d.cout, d.cout_pad, d.out_scale, d.out_stride = 1, cout_pad, cout_pad, 1.0, cout_pad
+        assert lib.goslam_conv2d_nhwc(ctypes.byref(d), 0, 8, 16, null) == -1, cout_pad
 
 
 def test_hashgrid_layout_matches_oracle(lib):

@@ -76,7 +76,10 @@ def test_conv_gru_shapes_vs_torch(shape):
 
 def test_layout_helpers_round_trip():
     from goslam_b200.modules.gru import to_nchw, to_nhwc, to_nhwc_padded
-    for shape in [(3, 70, 11, 13), (5, 128, 40, 80), (2, 576, 30, 40), (2, 64, 12, 20), (3, 128, 9, 16)]:   # generic + 64x64-tile paths
+    # generic + 64x64-tile paths; (2, 128, 9, 13): hw % 16 != 0 with C % 16 == 0; (2, 48, 8, 16): hw % 16 == 0 with
+    # C % 64 != 0, which sends NHWC -> NCHW down the generic path
+    for shape in [(3, 70, 11, 13), (5, 128, 40, 80), (2, 576, 30, 40), (2, 64, 12, 20), (3, 128, 9, 16), (2, 128, 9, 13),
+                  (2, 48, 8, 16)]:
         x = torch.randn(*shape, device=dev()).half()
         y = to_nhwc(x)
         assert y.shape == (shape[0], shape[2], shape[3], shape[1]) and torch.equal(y, x.permute(0, 2, 3, 1).contiguous())
@@ -88,9 +91,10 @@ def test_layout_helpers_round_trip():
 
 
 def test_update_module_vs_reference_golden():
-    """goslam_b200.droid_net.UpdateModule (wgmma ConvGRU + channels-last torch encoders / heads / GraphAgg, autocast)
-    against the reference UpdateModule's fp32 outputs (tests/golden/update_module.npz): same parameter names (the
-    `update.*` keys of pretrained/droid.pth load), same five outputs and shapes."""
+    """goslam_b200.droid_net.UpdateModule (the whole operator in one goslam_update_op call: wgmma encoders, ConvGRU,
+    heads and GraphAgg in fp16 with fp32 accumulation) against the reference UpdateModule's fp32 outputs
+    (tests/golden/update_module.npz): same parameter names (the `update.*` keys of pretrained/droid.pth load), same
+    five outputs and shapes.  The tight per-layer and whole-operator checks are in test_gpu_update_op.py."""
     from goslam_b200.droid_net import UpdateModule
     g = np.load(os.path.join(HERE, "golden", "update_module.npz"))
     torch.manual_seed(78)
