@@ -116,6 +116,16 @@ SIGNATURES = {
     "goslam_neus_mlp_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 10 + [c_int, c_int] +
                                  [ctypes.POINTER(NeusMlpBwdOut), c_void_p]),
     "goslam_hashgrid_layout": (c_int64, [c_void_p, c_void_p, c_void_p]),
+    "goslam_neus_sdf_grid": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 3 + [c_int] * 3 + [c_void_p, c_void_p]),
+    "goslam_mc_workspace_bytes": (c_size_t, [c_int] * 3),
+    "goslam_mc_count": (c_int, [c_void_p] + [c_int] * 3 + [ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "goslam_mc_emit": (c_int, [c_void_p] + [c_int] * 3 + [ctypes.c_double] + [c_void_p] * 3 + [c_size_t] +
+                       [c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "goslam_mesh_cull_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "goslam_mesh_cull_count": (c_int, [c_void_p, c_int64, c_void_p, c_int64] + [c_void_p] * 3 + [c_size_t, c_void_p, c_void_p]),
+    "goslam_mesh_cull_emit": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_int64, c_void_p,
+                                      c_int64, c_void_p]),
+    "goslam_neus_vertex_color": (c_int, [ctypes.POINTER(NeusParams), c_void_p, c_int64, c_void_p, c_void_p]),
     "goslam_sample_z": (c_int, [c_void_p] * 7 + [c_int] * 4 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "goslam_cvx_upsample": (c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p]),
     "goslam_proximity_workspace_bytes": (c_size_t, [c_int] * 3),

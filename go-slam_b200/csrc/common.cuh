@@ -37,6 +37,17 @@ struct GsArena {
   bool ok() const { return off <= cap && (base != nullptr || off == 0); }
 };
 
+// a / b for 0 <= a < 2^51 and b >= 1 through the double reciprocal inv_b = 1.0 / b: the product is within one of the
+// quotient, one correction step makes it exact.  A few instructions where the 64-bit integer division is a long
+// emulated sequence.
+__device__ __forceinline__ long long gs_div_fast(long long a, long long b, double inv_b) {
+  long long q = (long long)((double)a * inv_b);
+  const long long r = a - q * b;
+  if (r < 0) --q;
+  else if (r >= b) ++q;
+  return q;
+}
+
 __device__ __forceinline__ float gs_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

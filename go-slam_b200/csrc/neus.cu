@@ -274,6 +274,178 @@ __device__ __forceinline__ void encode_level(int l, const bool HASHED, const __h
   genc[2] = fmaf(L.scale, gz, genc[2]);
 }
 
+// The network's weights in shared memory, staged once per (persistent) block by all kThreadsN threads.
+__device__ __forceinline__ void stage_net_weights(Smem& sm, const goslam_neus_params& p, int tid) {
+  const __half* w = reinterpret_cast<const __half*>(p.mlp_w);
+  for (int i = tid; i < kHid * kIn; i += kThreadsN) sm.W1[(i / kIn) * kInPad + i % kIn] = w[i];
+  for (int i = tid; i < kHid * kHid; i += kThreadsN)
+    sm.W2[(i / kHid) * kHidPad + i % kHid] = w[kHid * kIn + i];
+  for (int i = tid; i < kOutW * kHid; i += kThreadsN)
+    sm.W3[(i / kHid) * kHidPad + i % kHid] = w[kHid * kIn + kHid * kHid + i];
+  for (int i = tid; i < 32 * 35; i += kThreadsN) {
+    const int o = i / 35, k = i % 35;
+    const float wv = p.sdf_w[i];
+    if (k < 3) {
+      sm.sdfWxyz[k * 32 + o] = wv;
+    } else {
+      const __half hi = __float2half_rn(wv);
+      sm.sdfWhi[o * kEncPad + (k - 3)] = hi;
+      sm.sdfWlo[o * kEncPad + (k - 3)] = __float2half_rn(wv - __half2float(hi));
+      if (o == 0) sm.gy[k - 3] = __half2float(hi);
+    }
+  }
+  for (int i = tid; i < 32 * (kEncPad - 32); i += kThreadsN) {   // zero the row padding
+    const int o = i / (kEncPad - 32), k = 32 + i % (kEncPad - 32);
+    sm.sdfWhi[o * kEncPad + k] = __float2half_rn(0.f);
+    sm.sdfWlo[o * kEncPad + k] = __float2half_rn(0.f);
+  }
+  for (int i = tid; i < 32; i += kThreadsN) sm.sdfB[i] = p.sdf_b[i];
+  for (int i = tid; i < 99; i += kThreadsN) sm.colB[i] = p.color_B[i];
+}
+
+// SDF head of a warp's 32 samples: out[32] = Linear(35,32)([xn | enc]) for this lane's sample, the encoding rows
+// read from sl.actB (stride kEncPad), the product enc (W_hi + W_lo)^T on tensor cores through an fp32 tile in sl.actA.
+__device__ __forceinline__ void sdf_head(const Smem& sm, WarpSlab& sl, int lane, const float (&xn)[3], float (&out)[32]) {
+  float* outf = reinterpret_cast<float*>(sl.actA);     // [32][33] fp32 tile
+  {
+    float acc4[2][4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc4[mt][nt][q] = 0.f;
+    const int lrr = lane & 15, lcc = (lane >> 4) * 8;
+    const int br = lane & 7, bc = ((lane >> 3) & 1) * 8;
+#pragma unroll
+    for (int kt = 0; kt < 2; ++kt) {
+      unsigned af[2][4];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+        ldmatrix_x4(af[mt], sl.actB + (mt * 16 + lrr) * kEncPad + kt * 16 + lcc);
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) {
+        unsigned bh[2], bl[2];
+        ldmatrix_x2(bh, sm.sdfWhi + (nt * 8 + br) * kEncPad + kt * 16 + bc);
+        ldmatrix_x2(bl, sm.sdfWlo + (nt * 8 + br) * kEncPad + kt * 16 + bc);
+        mma16816(acc4[0][nt], af[0], bl);
+        mma16816(acc4[1][nt], af[1], bl);
+        mma16816(acc4[0][nt], af[0], bh);
+        mma16816(acc4[1][nt], af[1], bh);
+      }
+    }
+    const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) {
+        const int col = nt * 8 + 2 * t;
+        outf[(mt * 16 + g) * 33 + col] = acc4[mt][nt][0];
+        outf[(mt * 16 + g) * 33 + col + 1] = acc4[mt][nt][1];
+        outf[(mt * 16 + g + 8) * 33 + col] = acc4[mt][nt][2];
+        outf[(mt * 16 + g + 8) * 33 + col + 1] = acc4[mt][nt][3];
+      }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int o4 = 0; o4 < 8; ++o4) {
+    const float4 bb = reinterpret_cast<const float4*>(sm.sdfB)[o4];
+    const float4 w0 = reinterpret_cast<const float4*>(sm.sdfWxyz)[o4];
+    const float4 w1 = reinterpret_cast<const float4*>(sm.sdfWxyz + 32)[o4];
+    const float4 w2 = reinterpret_cast<const float4*>(sm.sdfWxyz + 64)[o4];
+    const float* of = outf + lane * 33 + 4 * o4;
+    out[4 * o4 + 0] = of[0] + (bb.x + w0.x * xn[0] + w1.x * xn[1] + w2.x * xn[2]);
+    out[4 * o4 + 1] = of[1] + (bb.y + w0.y * xn[0] + w1.y * xn[1] + w2.y * xn[2]);
+    out[4 * o4 + 2] = of[2] + (bb.z + w0.z * xn[0] + w1.z * xn[1] + w2.z * xn[2]);
+    out[4 * o4 + 3] = of[3] + (bb.w + w0.w * xn[0] + w1.w * xn[1] + w2.w * xn[2]);
+  }
+  __syncwarp();                                  // everyone has read outf before actA is reused
+}
+
+// This lane's colour-network input row in sl.actA: [sin(p B)(33) | normal(3) | feat(31) | 1-padding(13)].
+__device__ __forceinline__ void mlp_row(const Smem& sm, WarpSlab& sl, int lane, const float (&pt)[3], const float (&g3)[3],
+                                        const float (&out)[32], bool inb) {
+  // the first 32 embedding columns in a rolled loop (4 per trip: the kernel is instruction-
+  // fetch sensitive, see kNeusHUnroll), column 32 with the static tail of the row
+  __half* rowh = sl.actA + lane * kInPad;                            // 176-byte rows: 16-B aligned
+#pragma unroll 1
+  for (int j4 = 0; j4 < 8; ++j4) {
+    float sn[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int j = 4 * j4 + u;
+      sn[u] = fast_sin(pt[0] * sm.colB[j] + pt[1] * sm.colB[33 + j] + pt[2] * sm.colB[66 + j]);
+    }
+    *reinterpret_cast<uint2*>(rowh + 4 * j4) =
+        make_uint2(h2_as_u32(__floats2half2_rn(sn[0], sn[1])), h2_as_u32(__floats2half2_rn(sn[2], sn[3])));
+  }
+  float row[kIn - 32];                                               // columns 32 .. 79
+  row[0] = fast_sin(pt[0] * sm.colB[32] + pt[1] * sm.colB[65] + pt[2] * sm.colB[98]);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) row[1 + c] = g3[c];
+#pragma unroll
+  for (int i = 0; i < 31; ++i) row[4 + i] = inb ? out[1 + i] : 0.f;
+#pragma unroll
+  for (int i = 35; i < kIn - 32; ++i) row[i] = 1.0f;
+  uint4* rowA = reinterpret_cast<uint4*>(rowh + 32);
+#pragma unroll
+  for (int v8 = 0; v8 < (kIn - 32) / 8; ++v8) {
+    uint4 u;
+    u.x = h2_as_u32(__floats2half2_rn(row[8 * v8 + 0], row[8 * v8 + 1]));
+    u.y = h2_as_u32(__floats2half2_rn(row[8 * v8 + 2], row[8 * v8 + 3]));
+    u.z = h2_as_u32(__floats2half2_rn(row[8 * v8 + 4], row[8 * v8 + 5]));
+    u.w = h2_as_u32(__floats2half2_rn(row[8 * v8 + 6], row[8 * v8 + 7]));
+    rowA[v8] = u;
+  }
+}
+
+// The warp-wide colour network on tensor cores over the 32 rows in sl.actA, then the sigmoid: rgbv = this lane's
+// colour, rounded like tcnn's half output and torch.sigmoid(half); 0 where !inb.  Also stored to rgb_keep[idx]
+// when rgb_keep is set and keep holds.
+__device__ __forceinline__ void color_mlp(const Smem& sm, WarpSlab& sl, int lane, bool inb, float (&rgbv)[3],
+                                          float* rgb_keep, bool keep, size_t idx) {
+  float accm[2][8][4];
+  warp_layer<8, kIn / 16, kInPad, kInPad>(sl.actA, sm.W1, accm, lane);
+  store_relu_half<8, kHidPad>(accm, sl.actB, lane);
+  __syncwarp();
+  warp_layer<8, kHid / 16, kHidPad, kHidPad>(sl.actB, sm.W2, accm, lane);
+  __syncwarp();
+  store_relu_half<8, kInPad>(accm, sl.actA, lane);
+  __syncwarp();
+  float acc3[2][2][4];
+  warp_layer<2, kHid / 16, kInPad, kHidPad>(sl.actA, sm.W3, acc3, lane);
+  __syncwarp();
+  float* scratch = reinterpret_cast<float*>(sl.actB);   // 32 x 4 floats
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt) {
+    if (t < 2) {
+      scratch[(mt * 16 + g) * 4 + 2 * t] = acc3[mt][0][0];
+      scratch[(mt * 16 + g) * 4 + 2 * t + 1] = acc3[mt][0][1];
+      scratch[(mt * 16 + g + 8) * 4 + 2 * t] = acc3[mt][0][2];
+      scratch[(mt * 16 + g + 8) * 4 + 2 * t + 1] = acc3[mt][0][3];
+    }
+  }
+  __syncwarp();
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float x = __half2float(__float2half_rn(scratch[lane * 4 + c]));   // tcnn output is half
+    const float sg = 1.0f / (1.0f + expf(-x));
+    rgbv[c] = inb ? __half2float(__float2half_rn(sg)) : 0.f;                // torch.sigmoid(half)
+    if (rgb_keep && keep) rgb_keep[idx * 3 + c] = rgbv[c];
+  }
+  __syncwarp();
+}
+
+// normalized_3d_coordinate (src/InstantNeuS.py:12-32) of one coordinate, op by op like the reference's separate torch
+// kernels: xn = clamp((p - b0) / (b1 - b0) * 2 - 1, -1, 1), the clamp's gradient mask times d xn / d p, and (xn + 1) / 2
+__device__ __forceinline__ void normalise_coord(float p, float b0, float b1, float& xn, float& dscale, float& x01) {
+  const float raw = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(p, b0), __fsub_rn(b1, b0)), 2.0f), 1.0f);
+  xn = fminf(fmaxf(raw, -1.0f), 1.0f);
+  dscale = (raw >= -1.0f && raw <= 1.0f) ? 2.0f / (b1 - b0) : 0.0f;
+  x01 = __fdiv_rn(__fadd_rn(xn, 1.0f), 2.0f);
+}
+
 __global__ void __launch_bounds__(kThreadsN, 1)
 neus_forward_kernel(const NeusArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -292,33 +464,7 @@ neus_forward_kernel(const NeusArgs a) {
   }
 
   // ---- stage the network weights once per block (persistent) ----
-  {
-    const __half* w = reinterpret_cast<const __half*>(a.p.mlp_w);
-    for (int i = tid; i < kHid * kIn; i += kThreadsN) sm.W1[(i / kIn) * kInPad + i % kIn] = w[i];
-    for (int i = tid; i < kHid * kHid; i += kThreadsN)
-      sm.W2[(i / kHid) * kHidPad + i % kHid] = w[kHid * kIn + i];
-    for (int i = tid; i < kOutW * kHid; i += kThreadsN)
-      sm.W3[(i / kHid) * kHidPad + i % kHid] = w[kHid * kIn + kHid * kHid + i];
-    for (int i = tid; i < 32 * 35; i += kThreadsN) {
-      const int o = i / 35, k = i % 35;
-      const float wv = a.p.sdf_w[i];
-      if (k < 3) {
-        sm.sdfWxyz[k * 32 + o] = wv;
-      } else {
-        const __half hi = __float2half_rn(wv);
-        sm.sdfWhi[o * kEncPad + (k - 3)] = hi;
-        sm.sdfWlo[o * kEncPad + (k - 3)] = __float2half_rn(wv - __half2float(hi));
-        if (o == 0) sm.gy[k - 3] = __half2float(hi);
-      }
-    }
-    for (int i = tid; i < 32 * (kEncPad - 32); i += kThreadsN) {   // zero the row padding
-      const int o = i / (kEncPad - 32), k = 32 + i % (kEncPad - 32);
-      sm.sdfWhi[o * kEncPad + k] = __float2half_rn(0.f);
-      sm.sdfWlo[o * kEncPad + k] = __float2half_rn(0.f);
-    }
-    for (int i = tid; i < 32; i += kThreadsN) sm.sdfB[i] = a.p.sdf_b[i];
-    for (int i = tid; i < 99; i += kThreadsN) sm.colB[i] = a.p.color_B[i];
-  }
+  stage_net_weights(sm, a.p, tid);
   __syncthreads();
 
   WarpSlab& sl = sm.slab[warp];
@@ -372,13 +518,7 @@ neus_forward_kernel(const NeusArgs a) {
       if (inb) {
         float x01[3];
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float b0 = a.p.bound[2 * c], b1 = a.p.bound[2 * c + 1];
-          const float raw = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(pt[c], b0), __fsub_rn(b1, b0)), 2.0f), 1.0f);
-          xn[c] = fminf(fmaxf(raw, -1.0f), 1.0f);
-          dscale[c] = (raw >= -1.0f && raw <= 1.0f) ? 2.0f / (b1 - b0) : 0.0f;
-          x01[c] = __fdiv_rn(__fadd_rn(xn[c], 1.0f), 2.0f);
-        }
+        for (int c = 0; c < 3; ++c) normalise_coord(pt[c], a.p.bound[2 * c], a.p.bound[2 * c + 1], xn[c], dscale[c], x01[c]);
 #pragma unroll kNeusHUnroll
         for (int l = 0; l < kLevels; ++l) {                 // one copy of the gather/interpolation code
           __half2 e;
@@ -398,61 +538,8 @@ neus_forward_kernel(const NeusArgs a) {
       __syncwarp();
 
       // ---- phase 1b: SDF head  out[32 x 32] = enc (W_hi + W_lo)^T  on tensor cores ----
-      float* outf = reinterpret_cast<float*>(sl.actA);     // [32][33] fp32 tile
-      {
-        float acc4[2][4][4];
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc4[mt][nt][q] = 0.f;
-        const int lrr = lane & 15, lcc = (lane >> 4) * 8;
-        const int br = lane & 7, bc = ((lane >> 3) & 1) * 8;
-#pragma unroll
-        for (int kt = 0; kt < 2; ++kt) {
-          unsigned af[2][4];
-#pragma unroll
-          for (int mt = 0; mt < 2; ++mt)
-            ldmatrix_x4(af[mt], sl.actB + (mt * 16 + lrr) * kEncPad + kt * 16 + lcc);
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt) {
-            unsigned bh[2], bl[2];
-            ldmatrix_x2(bh, sm.sdfWhi + (nt * 8 + br) * kEncPad + kt * 16 + bc);
-            ldmatrix_x2(bl, sm.sdfWlo + (nt * 8 + br) * kEncPad + kt * 16 + bc);
-            mma16816(acc4[0][nt], af[0], bl);
-            mma16816(acc4[1][nt], af[1], bl);
-            mma16816(acc4[0][nt], af[0], bh);
-            mma16816(acc4[1][nt], af[1], bh);
-          }
-        }
-        const int g = lane >> 2, t = lane & 3;
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt) {
-            const int col = nt * 8 + 2 * t;
-            outf[(mt * 16 + g) * 33 + col] = acc4[mt][nt][0];
-            outf[(mt * 16 + g) * 33 + col + 1] = acc4[mt][nt][1];
-            outf[(mt * 16 + g + 8) * 33 + col] = acc4[mt][nt][2];
-            outf[(mt * 16 + g + 8) * 33 + col + 1] = acc4[mt][nt][3];
-          }
-      }
-      __syncwarp();
       float out[32];
-#pragma unroll
-      for (int o4 = 0; o4 < 8; ++o4) {
-        const float4 bb = reinterpret_cast<const float4*>(sm.sdfB)[o4];
-        const float4 w0 = reinterpret_cast<const float4*>(sm.sdfWxyz)[o4];
-        const float4 w1 = reinterpret_cast<const float4*>(sm.sdfWxyz + 32)[o4];
-        const float4 w2 = reinterpret_cast<const float4*>(sm.sdfWxyz + 64)[o4];
-        const float* of = outf + lane * 33 + 4 * o4;
-        out[4 * o4 + 0] = of[0] + (bb.x + w0.x * xn[0] + w1.x * xn[1] + w2.x * xn[2]);
-        out[4 * o4 + 1] = of[1] + (bb.y + w0.y * xn[0] + w1.y * xn[1] + w2.y * xn[2]);
-        out[4 * o4 + 2] = of[2] + (bb.z + w0.z * xn[0] + w1.z * xn[1] + w2.z * xn[2]);
-        out[4 * o4 + 3] = of[3] + (bb.w + w0.w * xn[0] + w1.w * xn[1] + w2.w * xn[2]);
-      }
-      __syncwarp();                                  // everyone has read outf before actA is reused
+      sdf_head(sm, sl, lane, xn, out);
 
       if (inb) {
         sdf = out[0];
@@ -492,41 +579,10 @@ neus_forward_kernel(const NeusArgs a) {
 
       // ---- MLP input row: [sin(p B)(33) | normal(3) | feat(31) | 1-padding(13)] ----
       {
-        // the first 32 embedding columns in a rolled loop (4 per trip: the kernel is instruction-
-        // fetch sensitive, see kNeusHUnroll), column 32 with the static tail of the row
-        __half* rowh = sl.actA + lane * kInPad;                            // 176-byte rows: 16-B aligned
-#pragma unroll 1
-        for (int j4 = 0; j4 < 8; ++j4) {
-          float sn[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int j = 4 * j4 + u;
-            sn[u] = fast_sin(pt[0] * sm.colB[j] + pt[1] * sm.colB[33 + j] + pt[2] * sm.colB[66 + j]);
-          }
-          *reinterpret_cast<uint2*>(rowh + 4 * j4) =
-              make_uint2(h2_as_u32(__floats2half2_rn(sn[0], sn[1])), h2_as_u32(__floats2half2_rn(sn[2], sn[3])));
-        }
-        float row[kIn - 32];                                               // columns 32 .. 79
-        row[0] = fast_sin(pt[0] * sm.colB[32] + pt[1] * sm.colB[65] + pt[2] * sm.colB[98]);
-#pragma unroll
-        for (int c = 0; c < 3; ++c) row[1 + c] = g3[c];
-#pragma unroll
-        for (int i = 0; i < 31; ++i) row[4 + i] = inb ? out[1 + i] : 0.f;
-#pragma unroll
-        for (int i = 35; i < kIn - 32; ++i) row[i] = 1.0f;
-        uint4* rowA = reinterpret_cast<uint4*>(rowh + 32);
-#pragma unroll
-        for (int v8 = 0; v8 < (kIn - 32) / 8; ++v8) {
-          uint4 u;
-          u.x = h2_as_u32(__floats2half2_rn(row[8 * v8 + 0], row[8 * v8 + 1]));
-          u.y = h2_as_u32(__floats2half2_rn(row[8 * v8 + 2], row[8 * v8 + 3]));
-          u.z = h2_as_u32(__floats2half2_rn(row[8 * v8 + 4], row[8 * v8 + 5]));
-          u.w = h2_as_u32(__floats2half2_rn(row[8 * v8 + 6], row[8 * v8 + 7]));
-          rowA[v8] = u;
-        }
+        mlp_row(sm, sl, lane, pt, g3, out, inb);
         if (a.o.mlp_in && valid) {                   // training pass: keep the MLP input row (160 B)
           uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(a.o.mlp_in) + gidx * kIn);
-          const uint4* src = reinterpret_cast<const uint4*>(rowh);
+          const uint4* src = reinterpret_cast<const uint4*>(sl.actA + lane * kInPad);
 #pragma unroll
           for (int v = 0; v < kIn / 8; ++v) dst[v] = src[v];
         }
@@ -534,40 +590,8 @@ neus_forward_kernel(const NeusArgs a) {
       __syncwarp();
 
       // ---- warp-wide MLP on tensor cores ----
-      float rgbv[3] = {0.f, 0.f, 0.f};
-      {
-        float accm[2][8][4];
-        warp_layer<8, kIn / 16, kInPad, kInPad>(sl.actA, sm.W1, accm, lane);
-        store_relu_half<8, kHidPad>(accm, sl.actB, lane);
-        __syncwarp();
-        warp_layer<8, kHid / 16, kHidPad, kHidPad>(sl.actB, sm.W2, accm, lane);
-        __syncwarp();
-        store_relu_half<8, kInPad>(accm, sl.actA, lane);
-        __syncwarp();
-        float acc3[2][2][4];
-        warp_layer<2, kHid / 16, kInPad, kHidPad>(sl.actA, sm.W3, acc3, lane);
-        __syncwarp();
-        float* scratch = reinterpret_cast<float*>(sl.actB);   // 32 x 4 floats
-        const int g = lane >> 2, t = lane & 3;
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          if (t < 2) {
-            scratch[(mt * 16 + g) * 4 + 2 * t] = acc3[mt][0][0];
-            scratch[(mt * 16 + g) * 4 + 2 * t + 1] = acc3[mt][0][1];
-            scratch[(mt * 16 + g + 8) * 4 + 2 * t] = acc3[mt][0][2];
-            scratch[(mt * 16 + g + 8) * 4 + 2 * t + 1] = acc3[mt][0][3];
-          }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float x = __half2float(__float2half_rn(scratch[lane * 4 + c]));   // tcnn output is half
-          const float sg = 1.0f / (1.0f + expf(-x));
-          rgbv[c] = inb ? __half2float(__float2half_rn(sg)) : 0.f;                // torch.sigmoid(half)
-          if (a.o.rgb && valid) a.o.rgb[gidx * 3 + c] = rgbv[c];
-        }
-        __syncwarp();
-      }
+      float rgbv[3];
+      color_mlp(sm, sl, lane, inb, rgbv, a.o.rgb, valid, gidx);
 
       // ---- incremental front-to-back compositing (segmented scan over the rays in this tile) ----
       {
@@ -660,6 +684,115 @@ __global__ void neus_finalize_kernel(const float* blk_gerr, const unsigned* blk_
   for (int i = 0; i < nblk; ++i) { g += (double)blk_gerr[i]; c += blk_count[i]; }
   *gradient_error = (float)(g / (double)total_samples);
   if (mode == 0) *flag = (c == 0) ? 1 : 0;
+}
+
+// ======================================================================================================
+// Mesh extraction (InstantNeuS.extract_fields / extract_color, src/InstantNeuS.py:402-455): the marcher's device
+// code evaluated on a lattice and on mesh vertices.  Marching cubes and the cull are in mesh.cu.
+// ======================================================================================================
+struct SdfGridArgs {
+  goslam_neus_params p;
+  const float* xs; const float* ys; const float* zs;   // torch.linspace tables, computed by the caller
+  int nx, ny, nz;
+  long long n;
+  double inv_nyz, inv_nz;                              // reciprocals for gs_div_fast
+  float* u;                                            // [nx, ny, nz], z fastest
+};
+
+// u = -sdf(p) at p = (xs[i], ys[j], zs[k]) inside the strict realtime_bound test, -100 outside.  One thread per
+// point; consecutive threads walk z, so neighbours share the coarse levels' cells.  Only row 0 of the SDF head.
+__global__ void __launch_bounds__(256) neus_sdf_grid_kernel(const SdfGridArgs a) {
+  __shared__ float w0[35], gy_unused[32];
+  __shared__ float b0;
+  if (threadIdx.x < 35) w0[threadIdx.x] = a.p.sdf_w[threadIdx.x];
+  if (threadIdx.x < 32) gy_unused[threadIdx.x] = 0.f;
+  if (threadIdx.x == 0) b0 = a.p.sdf_b[0];
+  __syncthreads();
+  const long long L = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (L >= a.n) return;
+  const long long nyz = (long long)a.ny * a.nz;
+  const long long i = gs_div_fast(L, nyz, a.inv_nyz);
+  const long long r = L - i * nyz;
+  const long long j = gs_div_fast(r, a.nz, a.inv_nz), k = r - j * a.nz;
+  const float pt[3] = {a.xs[i], a.ys[j], a.zs[k]};
+  const bool inb = pt[0] < a.p.rt_bound[1] && pt[0] > a.p.rt_bound[0] && pt[1] < a.p.rt_bound[3] &&
+                   pt[1] > a.p.rt_bound[2] && pt[2] < a.p.rt_bound[5] && pt[2] > a.p.rt_bound[4];
+  if (!inb) { a.u[L] = -100.0f; return; }
+  float xn[3], dscale[3], x01[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) normalise_coord(pt[c], a.p.bound[2 * c], a.p.bound[2 * c + 1], xn[c], dscale[c], x01[c]);
+  const __half2* table = reinterpret_cast<const __half2*>(a.p.grid);
+  float genc[3] = {0.f, 0.f, 0.f};                    // the normal is not needed: dead after inlining
+  float acc = 0.f;
+#pragma unroll kNeusHUnroll
+  for (int l = 0; l < kLevels; ++l) {
+    __half2 e;
+    encode_level(l, l >= kDenseLevels, table, x01, gy_unused, e, genc);
+    const float2 ef = __half22float2(e);
+    acc = fmaf(w0[3 + 2 * l], ef.x, acc);
+    acc = fmaf(w0[4 + 2 * l], ef.y, acc);
+  }
+  a.u[L] = -(acc + (b0 + w0[0] * xn[0] + w0[1] * xn[1] + w0[2] * xn[2]));
+}
+
+struct VertexColorArgs {
+  goslam_neus_params p;
+  const double* verts;
+  long long n;
+  unsigned char* rgb;    // [n, 3]
+};
+
+// extract_color for vertices rounded to fp32: the forward's per-sample path (encoding with the analytic normal
+// through the normalised grid and the clamp's mask, SDF head, colour network on mma.sync, sigmoid) with every
+// vertex in bound (no realtime_bound mask), then uint8(clip(c, 0, 1) * 255) with truncation.  A warp takes 32
+// vertices at a time; blocks are persistent and stage the weights once.
+__global__ void __launch_bounds__(kThreadsN, 1) neus_vertex_color_kernel(const VertexColorArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  stage_net_weights(sm, a.p, tid);
+  __syncthreads();
+  WarpSlab& sl = sm.slab[warp];
+  const __half2* table = reinterpret_cast<const __half2*>(a.p.grid);
+  const long long ntiles = (a.n + 31) / 32;
+  for (long long tile = (long long)blockIdx.x * kWarpsN + warp; tile < ntiles; tile += (long long)gridDim.x * kWarpsN) {
+    const long long i = tile * 32 + lane;
+    const bool inb = i < a.n;
+    float pt[3] = {0.f, 0.f, 0.f}, xn[3] = {0.f, 0.f, 0.f}, dscale[3] = {0.f, 0.f, 0.f}, x01[3];
+    float genc[3] = {0.f, 0.f, 0.f}, g3[3] = {0.f, 0.f, 0.f};
+    __half2* encrow = reinterpret_cast<__half2*>(sl.actB + lane * kEncPad);
+    if (inb) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        pt[c] = __double2float_rn(a.verts[i * 3 + c]);
+        normalise_coord(pt[c], a.p.bound[2 * c], a.p.bound[2 * c + 1], xn[c], dscale[c], x01[c]);
+      }
+#pragma unroll kNeusHUnroll
+      for (int l = 0; l < kLevels; ++l) {
+        __half2 e;
+        encode_level(l, l >= kDenseLevels, table, x01, sm.gy, e, genc);
+        encrow[l] = e;
+      }
+    } else {
+#pragma unroll
+      for (int l = 0; l < kLevels; ++l) encrow[l] = __float2half2_rn(0.f);
+    }
+    __syncwarp();
+    float out[32];
+    sdf_head(sm, sl, lane, xn, out);
+    if (inb) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) g3[c] = (sm.sdfWxyz[c * 32] + 0.5f * genc[c]) * dscale[c];
+    }
+    mlp_row(sm, sl, lane, pt, g3, out, inb);
+    __syncwarp();
+    float rgbv[3];
+    color_mlp(sm, sl, lane, inb, rgbv, nullptr, false, 0);
+    if (inb) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) a.rgb[i * 3 + c] = (unsigned char)(fminf(fmaxf(rgbv[c], 0.f), 1.f) * 255.0f);
+    }
+  }
 }
 
 // ======================================================================================================
@@ -1198,6 +1331,8 @@ int neus_device_init() {
   if (cudaMemcpyToSymbol(c_lvl, lc, sizeof(lc)) != cudaSuccess) return GOSLAM_ELAUNCH;
   if (cudaFuncSetAttribute(neus_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(Smem)) != cudaSuccess) return GOSLAM_ELAUNCH;
+  if (cudaFuncSetAttribute(neus_vertex_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(Smem)) != cudaSuccess) return GOSLAM_ELAUNCH;
   if (cudaFuncSetAttribute(neus_mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(MlpBwdSmem)) != cudaSuccess) return GOSLAM_ELAUNCH;
   ready[dev] = true;
@@ -1324,6 +1459,36 @@ int goslam_neus_grid_backward(const goslam_neus_params* params, const float* ray
   const long long blocks = (a.n + 255) / 256;
   if (blocks > 0x7fffffffLL) return GOSLAM_EINVAL;
   neus_grid_bwd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+int goslam_neus_sdf_grid(const goslam_neus_params* params, const float* xs, const float* ys, const float* zs, int nx,
+                         int ny, int nz, float* u, void* stream) {
+  if (!params || !xs || !ys || !zs || !u || nx < 1 || ny < 1 || nz < 1 || (long long)nx * ny * nz > (1ll << 40))
+    return GOSLAM_EINVAL;
+  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  SdfGridArgs a{};
+  a.p = *params; a.xs = xs; a.ys = ys; a.zs = zs; a.nx = nx; a.ny = ny; a.nz = nz; a.u = u;
+  a.n = (long long)nx * ny * nz;
+  a.inv_nyz = 1.0 / ((double)ny * nz);
+  a.inv_nz = 1.0 / (double)nz;
+  neus_sdf_grid_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+int goslam_neus_vertex_color(const goslam_neus_params* params, const double* verts, int64_t n, unsigned char* rgb,
+                             void* stream) {
+  if (!params || n < 0 || (n > 0 && (!verts || !rgb))) return GOSLAM_EINVAL;
+  if (n == 0) return GOSLAM_OK;
+  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  VertexColorArgs a{};
+  a.p = *params; a.verts = verts; a.n = n; a.rgb = rgb;
+  const long long groups = (n + 31) / 32;
+  const long long blocks = (groups + kWarpsN - 1) / kWarpsN;
+  neus_vertex_color_kernel<<<(unsigned)(blocks < kNumSms ? blocks : kNumSms), kThreadsN, sizeof(Smem),
+                             (cudaStream_t)stream>>>(a);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

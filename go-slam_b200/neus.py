@@ -280,6 +280,162 @@ class InstantNeuS(nn.Module):
         out['sdf_variance'] = torch.full((R, 1), 1.0 / inv_s, **f32)
         return out
 
+    # ---- mesh extraction (src/InstantNeuS.py:258-274, 402-492) ------------------------------------------------
+    @torch.no_grad()
+    def in_bound(self, pts, bound):
+        """strict per-axis test of pts [n,3] against bound [3,2] (src/InstantNeuS.py:258-274)"""
+        bound = bound.to(pts.device)
+        mask_x = (pts[:, 0] < bound[0, 1]) & (pts[:, 0] > bound[0, 0])
+        mask_y = (pts[:, 1] < bound[1, 1]) & (pts[:, 1] > bound[1, 0])
+        mask_z = (pts[:, 2] < bound[2, 1]) & (pts[:, 2] > bound[2, 0])
+        return (mask_x & mask_y & mask_z).bool()
+
+    def _device(self):
+        dev = self.bound.device
+        if dev.type != 'cuda':
+            raise RuntimeError("InstantNeuS mesh extraction: the network must be on a CUDA device (no CPU fallback)")
+        return dev
+
+    def _sdf_grid(self, bound_min, bound_max, resolution):
+        """u [res]^3 f32 on the device for the lattice torch.linspace(bound_min[a], bound_max[a], res) (computed on the
+        CPU, as the reference does), normalised by [bound_min, bound_max], masked by realtime_bound"""
+        dev = self._device()
+        res = int(resolution)
+        if res < 1:
+            raise ValueError("resolution must be positive")
+        tabs = torch.cat([torch.linspace(float(bound_min[a]), float(bound_max[a]), res) for a in range(3)])
+        tabs = tabs.pin_memory().to(dev, non_blocking=True)
+        p, keep, _ = self._params_struct()
+        for a in range(3):
+            p.bound[2 * a], p.bound[2 * a + 1] = float(bound_min[a]), float(bound_max[a])
+        u = torch.empty((res, res, res), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            rc = _lib.load().goslam_neus_sdf_grid(ctypes.byref(p), _lib.ptr(tabs[:res]), _lib.ptr(tabs[res:2 * res]),
+                                                  _lib.ptr(tabs[2 * res:]), res, res, res, _lib.ptr(u), _lib.stream_ptr())
+        _lib.check(rc, "neus_sdf_grid")
+        return u
+
+    @torch.no_grad()
+    def extract_fields(self, bound_min, bound_max, resolution: int):
+        """numpy f32 [res]^3: -sdf on the lattice, -100 outside realtime_bound (src/InstantNeuS.py:423-455); one launch and
+        one device-to-host copy"""
+        bmin = torch.as_tensor(bound_min).detach().float().cpu().tolist()
+        bmax = torch.as_tensor(bound_max).detach().float().cpu().tolist()
+        return self._sdf_grid(bmin, bmax, resolution).cpu().numpy()
+
+    def _vertex_colors(self, verts, bound):
+        """uint8 [V,3] colours of f64 device vertices, the network normalised by `bound` (6 floats, x-major)"""
+        dev = verts.device
+        p, keep, _ = self._params_struct()
+        for i in range(6):
+            p.bound[i] = bound[i]
+        rgb = torch.empty((verts.shape[0], 3), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            rc = _lib.load().goslam_neus_vertex_color(ctypes.byref(p), _lib.ptr(verts), verts.shape[0], _lib.ptr(rgb),
+                                                      _lib.stream_ptr())
+        _lib.check(rc, "neus_vertex_color")
+        return rgb
+
+    @torch.no_grad()
+    def extract_color(self, bound, vertices):
+        """numpy uint8 [V,3] vertex colours of numpy vertices (src/InstantNeuS.py:402-420)"""
+        dev = self._device()
+        b = torch.as_tensor(bound).detach().float().cpu().reshape(-1).tolist()
+        verts = torch.as_tensor(vertices, dtype=torch.float64).reshape(-1, 3).to(dev).contiguous()
+        return self._vertex_colors(verts, b).cpu().numpy()
+
+    @torch.no_grad()
+    def extract_mesh(self, resolution, threshold, c2w_ref=None, color=True):
+        """extract_geometry on the device: (vertices [V,3] f64, faces [F,3] i64, colours [V,3] u8 or None), CUDA tensors.
+        Field -> marching cubes -> world scaling -> c2w_ref -> bound cull -> colours of the kept vertices.  Two host
+        synchronisations: the two count reads (and one on the first call after the bounds change)."""
+        import numpy as np
+        dev = self._device()
+        res = int(resolution)
+        self._params_struct()                                # refreshes the host copies of the bounds
+        b, rb = self._host_cache[1], self._host_cache[2]
+        bmin, bmax = [b[0], b[2], b[4]], [b[1], b[3], b[5]]
+        u = self._sdf_grid(bmin, bmax, res)
+        verts, faces = marching_cubes(u, threshold, bmin, bmax)
+        del u
+        if c2w_ref is not None:
+            # np.matmul(c2w_ref[None], [v, 1][:, :, None])[:, :3, 0] in float64
+            c = torch.as_tensor(c2w_ref).detach().to(dev, torch.float64)
+            verts = ((verts[:, 0:1] * c[:3, 0] + verts[:, 1:2] * c[:3, 1]) + verts[:, 2:3] * c[:3, 2]) + c[:3, 3]
+        # bound cull: thresholds in float32, as numpy computes `bound[:, 0] - eps` on the float32 array
+        rt = np.array(rb, np.float32).reshape(3, 2)
+        eps = 0.01
+        out_v, out_f = cull_mesh(verts, faces, (rt[:, 0] - eps).tolist(), (rt[:, 1] + eps).tolist())
+        del verts, faces
+        rgb = self._vertex_colors(out_v, b) if color else None
+        return out_v, out_f, rgb
+
+    @torch.no_grad()
+    def extract_geometry(self, resolution: int, threshold: float, c2w_ref=None, save_path='./mesh.ply', color=False):
+        """the reference's extract_geometry (src/InstantNeuS.py:458-497): a trimesh.Trimesh of the culled mesh, exported to
+        save_path unless it is None.  Runs extract_mesh; the arrays come back in one device-to-host copy."""
+        import trimesh          # the reference imports it at module level
+        verts, faces, rgb = self.extract_mesh(resolution, threshold, c2w_ref=c2w_ref, color=color)
+        host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (verts, faces, rgb) if t is not None]
+        for h, t in zip(host, (verts, faces, rgb)):
+            h.copy_(t, non_blocking=True)
+        torch.cuda.current_stream(verts.device).synchronize()
+        vertex_colors = host[2].numpy() if color else None
+        mesh = trimesh.Trimesh(host[0].numpy(), host[1].numpy(), vertex_colors=vertex_colors)
+        if save_path is not None:
+            mesh.export(save_path)
+        return mesh
+
+
+def marching_cubes(u, iso, bound_min, bound_max):
+    """marching cubes of the f32 CUDA field u [nx,ny,nz] at level iso (inside iff u > iso), on the generated tables of
+    csrc/mc_tables.cuh: (vertices [V,3] f64 in world coordinates v / (n - 1.0) * (float32)(bound_max - bound_min) +
+    bound_min, faces [F,3] i64), CUDA tensors.  Reads the two counts back (one host synchronisation)."""
+    lib = _lib.load()
+    u = u.detach().float().contiguous()
+    nx, ny, nz = u.shape
+    dev = u.device
+    i64 = dict(dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        st = _lib.stream_ptr()
+        ws = torch.empty(lib.goslam_mc_workspace_bytes(nx, ny, nz), dtype=torch.uint8, device=dev)
+        counts = torch.empty(2, **i64)
+        _lib.check(lib.goslam_mc_count(_lib.ptr(u), nx, ny, nz, float(iso), _lib.ptr(ws), ws.numel(), _lib.ptr(counts), st),
+                   "mc_count")
+        nv, nf = counts.tolist()
+        verts = torch.empty((nv, 3), dtype=torch.float64, device=dev)
+        faces = torch.empty((nf, 3), **i64)
+        lo = (ctypes.c_float * 3)(*[float(v) for v in bound_min])
+        hi = (ctypes.c_float * 3)(*[float(v) for v in bound_max])
+        _lib.check(lib.goslam_mc_emit(_lib.ptr(u), nx, ny, nz, float(iso), lo, hi, _lib.ptr(ws), ws.numel(),
+                                      _lib.ptr(verts), nv, _lib.ptr(faces), nf, st), "mc_emit")
+    return verts, faces
+
+
+def cull_mesh(verts, faces, lo, hi):
+    """keep the vertices with lo <= v <= hi (lo, hi: 3 float32 values each), the faces whose three vertices are kept,
+    then drop unreferenced vertices; stable orders, faces re-indexed (update_faces + remove_unreferenced_vertices).
+    CUDA tensors in and out; reads the two counts back (one host synchronisation)."""
+    lib = _lib.load()
+    verts = verts.detach().to(torch.float64).contiguous()
+    faces = faces.detach().to(torch.int64).contiguous()
+    nv, nf = verts.shape[0], faces.shape[0]
+    dev = verts.device
+    with torch.cuda.device(dev):
+        st = _lib.stream_ptr()
+        ws = torch.empty(lib.goslam_mesh_cull_workspace_bytes(nv, nf), dtype=torch.uint8, device=dev)
+        counts = torch.empty(2, dtype=torch.int64, device=dev)
+        lo = (ctypes.c_float * 3)(*[float(v) for v in lo])
+        hi = (ctypes.c_float * 3)(*[float(v) for v in hi])
+        _lib.check(lib.goslam_mesh_cull_count(_lib.ptr(verts), nv, _lib.ptr(faces), nf, lo, hi, _lib.ptr(ws), ws.numel(),
+                                              _lib.ptr(counts), st), "mesh_cull_count")
+        kv, kf = counts.tolist()
+        out_v = torch.empty((kv, 3), dtype=torch.float64, device=dev)
+        out_f = torch.empty((kf, 3), dtype=torch.int64, device=dev)
+        _lib.check(lib.goslam_mesh_cull_emit(_lib.ptr(verts), nv, _lib.ptr(faces), nf, _lib.ptr(ws), ws.numel(),
+                                             _lib.ptr(out_v), kv, _lib.ptr(out_f), kf, st), "mesh_cull_emit")
+    return out_v, out_f
+
 
 class _NeusFunction(torch.autograd.Function):
     """InstantNeuS.forward as one autograd node (what autograd + tiny-cuda-nn do for the reference,

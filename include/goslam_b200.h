@@ -371,6 +371,49 @@ int goslam_neus_mlp_backward(const goslam_neus_params* params, const void* mlp_i
                              const float* d_mlp_out, const float* d_sdf, const float* d_grad, const float* rays_o,
                              const float* rays_d, const float* z_mid, const float* scale, int R, int S,
                              const goslam_neus_mlp_bwd_out* out, void* stream);
+/* ------------------------------------------------------------------------------------
+ * Mesh extraction: InstantNeuS.extract_fields / extract_geometry / extract_color (src/InstantNeuS.py:402-492).
+ * The pipeline is sdf_grid -> mc_count -> (caller reads the two counts, allocates) -> mc_emit -> mesh_cull_count
+ * -> (reads, allocates) -> mesh_cull_emit -> neus_vertex_color.  Pointers are device pointers unless marked host.
+ *
+ * goslam_neus_sdf_grid — u[i,j,k] (f32 [nx,ny,nz], z fastest) = -sdf(xs[i], ys[j], zs[k]) where the point passes the
+ *   strict params->rt_bound test, -100 elsewhere; the sdf is normalised by params->bound (row 0 of the SDF head, the
+ *   marcher's hash-grid gather).  xs, ys, zs are the caller's torch.linspace tables (the kernel does not recompute them).
+ *
+ * goslam_mc_count / goslam_mc_emit — marching cubes on u at level iso (inside iff (double)u > iso), tables generated by
+ *   tools/gen_mc_tables.py.  count writes counts[0] = vertices, counts[1] = faces (device int64) and leaves its state
+ *   in the workspace (goslam_mc_workspace_bytes(nx,ny,nz) bytes, 1.125 bytes per lattice point plus a little), which
+ *   emit reads: call emit with the same u, shape, iso and workspace.  emit writes verts [V,3] f64 in world coordinates
+ *   (the index-space position, one vertex per crossing lattice edge in ascending edge id 3*linear+axis, mapped by
+ *   v / (n_axis - 1.0) * (double)(float)(bound_max - bound_min) + (double)bound_min; bound_min / bound_max are host
+ *   float[3]) and faces [F,3] int64 (by cell, x-major, z fastest, then table order); it writes at most max_verts /
+ *   max_faces rows.  nx, ny, nz >= 2.
+ *
+ * goslam_mesh_cull_count / goslam_mesh_cull_emit — keep a vertex iff lo[c] <= v[c] <= hi[c] for all c (lo, hi: host
+ *   float[3], compared in f64), a face iff its three vertices are kept, then drop the vertices no kept face references;
+ *   orders are stable and faces are re-indexed.  count writes counts[0] = kept vertices, counts[1] = kept faces and
+ *   leaves its state in the workspace (goslam_mesh_cull_workspace_bytes) for emit, which writes at most max_out_verts /
+ *   max_out_faces rows.
+ *
+ * goslam_neus_vertex_color — extract_color: rgb [n,3] uint8 = uint8(clip(c, 0, 1) * 255) of the colour network at the
+ *   vertices rounded to f32 (normal and feature from the hash grid normalised by params->bound; no rt_bound mask).
+ * ---------------------------------------------------------------------------------- */
+int goslam_neus_sdf_grid(const goslam_neus_params* params, const float* xs, const float* ys, const float* zs, int nx,
+                         int ny, int nz, float* u, void* stream);
+size_t goslam_mc_workspace_bytes(int nx, int ny, int nz);
+int goslam_mc_count(const float* u, int nx, int ny, int nz, double iso, void* workspace, size_t workspace_bytes,
+                    int64_t* counts, void* stream);
+int goslam_mc_emit(const float* u, int nx, int ny, int nz, double iso, const float* bound_min, const float* bound_max,
+                   const void* workspace, size_t workspace_bytes, double* verts, int64_t max_verts, int64_t* faces,
+                   int64_t max_faces, void* stream);
+size_t goslam_mesh_cull_workspace_bytes(int64_t n_verts, int64_t n_faces);
+int goslam_mesh_cull_count(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, const float* lo,
+                           const float* hi, void* workspace, size_t workspace_bytes, int64_t* counts, void* stream);
+int goslam_mesh_cull_emit(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, const void* workspace,
+                          size_t workspace_bytes, double* out_verts, int64_t max_out_verts, int64_t* out_faces,
+                          int64_t max_out_faces, void* stream);
+int goslam_neus_vertex_color(const goslam_neus_params* params, const double* verts, int64_t n, unsigned char* rgb,
+                             void* stream);
 /* hash-grid geometry helper (host side, no GPU): fills offsets[17] (in PARAMS, i.e.
  * entries*2), resolutions[16], scales[16]; returns total number of f16 params. */
 int64_t goslam_hashgrid_layout(int64_t* offsets, int* resolutions, float* scales);
