@@ -126,6 +126,17 @@ SIGNATURES = {
     "goslam_mesh_cull_emit": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_int64, c_void_p,
                                       c_int64, c_void_p]),
     "goslam_neus_vertex_color": (c_int, [ctypes.POINTER(NeusParams), c_void_p, c_int64, c_void_p, c_void_p]),
+    "goslam_mesh_cull_mask_count": (c_int, [c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
+                                            c_void_p]),
+    "goslam_mesh_cull_vertex_ids": (c_int, [c_int64, c_int64, c_void_p, c_size_t, c_void_p, c_int64, c_void_p]),
+    "goslam_mesh_depth_render": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p] + [c_int] * 3 +
+                                 [ctypes.c_double] * 6 + [c_void_p, c_void_p]),
+    "goslam_mesh_view_masks": (c_int, [c_void_p, c_int64, c_void_p, c_void_p] + [c_int] * 3 + [c_float] * 6 +
+                               [c_void_p] * 3),
+    "goslam_mesh_components_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "goslam_mesh_components_count": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "goslam_mesh_components_keep": (c_int, [c_int64, c_int64, ctypes.c_double, c_int, c_void_p, c_size_t, c_void_p,
+                                            c_void_p]),
     "goslam_sample_z": (c_int, [c_void_p] * 7 + [c_int] * 4 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "goslam_cvx_upsample": (c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p]),
     "goslam_proximity_workspace_bytes": (c_size_t, [c_int] * 3),

@@ -347,6 +347,35 @@ __global__ void __launch_bounds__(256) cull_face_kernel(const double* verts, lon
   }
 }
 
+// a face is kept iff face_mask[f] (when given) and vert_mask of its three vertices (when given): trimesh's
+// update_faces(mask[faces].all(1)) of src/mesher.py:198,213,228
+__global__ void __launch_bounds__(256) cull_mask_face_kernel(long long nv, const long long* faces, long long nf,
+                                                             const unsigned char* face_mask, const unsigned char* vert_mask,
+                                                             unsigned* fkeep, unsigned* vref) {
+  const long long f = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= nf) return;
+  long long v[3];
+  bool keep = !face_mask || face_mask[f];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    v[j] = faces[f * 3 + j];
+    if (v[j] < 0 || v[j] >= nv) { keep = false; continue; }
+    if (vert_mask && !vert_mask[v[j]]) keep = false;
+  }
+  fkeep[f] = keep ? 1u : 0u;
+  if (keep) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j) vref[v[j]] = 1u;
+  }
+}
+
+__global__ void __launch_bounds__(256) cull_vertex_ids_kernel(long long nv, const unsigned* vref, const u64* voff, long long* ids,
+                                                              long long max_ids) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nv || !vref[i] || (long long)voff[i] >= max_ids) return;
+  ids[voff[i]] = i;
+}
+
 __global__ void __launch_bounds__(256) cull_vertex_emit_kernel(const double* verts, long long nv, const unsigned* vref,
                                                                const u64* voff, double* out, long long max_out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -470,6 +499,41 @@ int goslam_mesh_cull_emit(const double* verts, int64_t n_verts, const int64_t* f
   if (n_faces > 0 && max_out_faces > 0) {
     cull_face_emit_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>((const long long*)faces, n_faces, w.fkeep, w.foff, w.voff,
                                                                     (long long*)out_faces, max_out_faces);
+    GS_CHECK_LAUNCH();
+  }
+  return GOSLAM_OK;
+}
+
+int goslam_mesh_cull_mask_count(int64_t n_verts, const int64_t* faces, int64_t n_faces, const unsigned char* face_mask,
+                                const unsigned char* vert_mask, void* workspace, size_t workspace_bytes, int64_t* counts,
+                                void* stream) {
+  if (n_verts < 0 || n_faces < 0 || (n_faces > 0 && !faces) || !counts) return GOSLAM_EINVAL;
+  CullWork w;
+  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, workspace, &w)) return GOSLAM_EWORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_verts > 0 && cudaMemsetAsync(w.vref, 0, (size_t)n_verts * sizeof(unsigned), st) != cudaSuccess) {
+    gs_note_cuda_error(cudaGetLastError());
+    return GOSLAM_ELAUNCH;
+  }
+  if (n_faces > 0) {
+    cull_mask_face_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(n_verts, (const long long*)faces, n_faces, face_mask,
+                                                                     vert_mask, w.fkeep, w.vref);
+    GS_CHECK_LAUNCH();
+  }
+  int rc = exclusive_scan(U32Load{w.vref}, n_verts, w.voff, w.tiles, (long long*)counts, st);
+  if (rc != GOSLAM_OK) return rc;
+  return exclusive_scan(U32Load{w.fkeep}, n_faces, w.foff, w.tiles, (long long*)counts + 1, st);
+}
+
+int goslam_mesh_cull_vertex_ids(int64_t n_verts, int64_t n_faces, const void* workspace, size_t workspace_bytes, int64_t* ids,
+                                int64_t max_ids, void* stream) {
+  if (n_verts < 0 || n_faces < 0 || max_ids < 0 || (max_ids > 0 && !ids)) return GOSLAM_EINVAL;
+  CullWork w;
+  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, const_cast<void*>(workspace), &w))
+    return GOSLAM_EWORKSPACE;
+  if (n_verts > 0 && max_ids > 0) {
+    cull_vertex_ids_kernel<<<blocks_for(n_verts, 256), 256, 0, (cudaStream_t)stream>>>(n_verts, w.vref, w.voff,
+                                                                                       (long long*)ids, max_ids);
     GS_CHECK_LAUNCH();
   }
   return GOSLAM_OK;

@@ -414,6 +414,46 @@ int goslam_mesh_cull_emit(const double* verts, int64_t n_verts, const int64_t* f
                           int64_t max_out_faces, void* stream);
 int goslam_neus_vertex_color(const goslam_neus_params* params, const double* verts, int64_t n, unsigned char* rgb,
                              void* stream);
+/* ------------------------------------------------------------------------------------
+ * Mesh culling against the camera views: Mesher.cull_mesh (src/mesher.py:56-240).  Device pointers unless marked host.
+ *
+ * goslam_mesh_cull_mask_count — the count pass of goslam_mesh_cull_count with a keep rule given by masks: a face is kept
+ *   iff face_mask[f] != 0 and vert_mask[v] != 0 for its three vertices (u8; either may be NULL, meaning all kept).  Fills
+ *   the goslam_mesh_cull_workspace_bytes workspace for goslam_mesh_cull_emit and goslam_mesh_cull_vertex_ids, which writes
+ *   the old index (int64) of every kept vertex in output order (at most max_ids) so that per-vertex attributes follow.
+ *
+ * goslam_mesh_depth_render — extract_depth_from_mesh: depth [K,H,W] f32 of the mesh (verts [V,3] f64, faces [F,3] i64)
+ *   seen from c2w [K,4,4] f32 (OpenCV camera-to-world), pinhole fx, fy, cx, cy.  Camera coordinates R^T (p - t) in f64,
+ *   clip against z = znear, pixel (r, c) samples (c + 0.5, r + 0.5), inclusive coverage of either winding, perspective-
+ *   correct z, fragments with z > zfar dropped, the nearest fragment kept; 0 where no fragment lands.  K <= 65535.
+ *
+ * goslam_mesh_view_masks — point_masks over one chunk of views: ORs into seen[V] and forecast[V] (u8, zeroed once by the
+ *   caller) with w2c [K,4,4] f32 (torch.inverse(c2w)) and depth [K,H,W] of the same views; the reference's f32 arithmetic,
+ *   grid_sample bilinear / border / align_corners=True, front = d > 0 ? z < d + eps : true.
+ *
+ * goslam_mesh_components_count / goslam_mesh_components_keep — get_connected_mesh: faces are adjacent when they share an
+ *   edge that belongs to exactly two faces; a component is kept iff its area (f64) > threshold * the mesh's area, or, with
+ *   largest != 0, only the component of largest area (ties: the one with the smallest face id).  count writes counts[0] =
+ *   number of components (device int64) and leaves its state in the workspace (goslam_mesh_components_workspace_bytes,
+ *   which needs a device to size CUB's scratch and returns 0 without one); keep takes that number from the host and writes
+ *   face_keep[F] (u8), the input of goslam_mesh_cull_mask_count.  Faces must index [0, n_verts); F < 2^31.
+ * ---------------------------------------------------------------------------------- */
+int goslam_mesh_cull_mask_count(int64_t n_verts, const int64_t* faces, int64_t n_faces, const unsigned char* face_mask,
+                                const unsigned char* vert_mask, void* workspace, size_t workspace_bytes, int64_t* counts,
+                                void* stream);
+int goslam_mesh_cull_vertex_ids(int64_t n_verts, int64_t n_faces, const void* workspace, size_t workspace_bytes, int64_t* ids,
+                                int64_t max_ids, void* stream);
+int goslam_mesh_depth_render(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, const float* c2w,
+                             int K, int H, int W, double fx, double fy, double cx, double cy, double znear, double zfar,
+                             float* depth, void* stream);
+int goslam_mesh_view_masks(const double* verts, int64_t n_verts, const float* w2c, const float* depth, int K, int H, int W,
+                           float fx, float fy, float cx, float cy, float radius, float eps, unsigned char* seen,
+                           unsigned char* forecast, void* stream);
+size_t goslam_mesh_components_workspace_bytes(int64_t n_verts, int64_t n_faces);
+int goslam_mesh_components_count(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, void* workspace,
+                                 size_t workspace_bytes, int64_t* counts, void* stream);
+int goslam_mesh_components_keep(int64_t n_faces, int64_t n_components, double threshold, int largest, void* workspace,
+                                size_t workspace_bytes, unsigned char* face_keep, void* stream);
 /* hash-grid geometry helper (host side, no GPU): fills offsets[17] (in PARAMS, i.e.
  * entries*2), resolutions[16], scales[16]; returns total number of f16 params. */
 int64_t goslam_hashgrid_layout(int64_t* offsets, int* resolutions, float* scales);
