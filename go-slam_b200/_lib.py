@@ -152,6 +152,12 @@ SIGNATURES = {
     "goslam_update_op_workspace_bytes": (c_size_t, [c_int] * 4),
     "goslam_update_op": (c_int, [ctypes.POINTER(UpdateWeights)] + [c_void_p] * 5 + [c_int] * 4 + [c_void_p] * 5 +
                          [c_void_p, c_size_t, c_void_p]),
+    "goslam_mapping_snapshot_workspace_bytes": (c_size_t, [c_int] * 3),
+    "goslam_mapping_snapshot": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_float, c_void_p,
+                                                                        c_size_t, c_void_p, c_void_p]),
+    "goslam_mapping_rays": (c_int, [c_void_p, c_size_t] + [c_int] * 3 + [c_void_p, c_void_p, c_int64, c_int] +
+                            [c_void_p] * 3 + [ctypes.c_double] * 4 + [c_void_p] * 4 + [c_int64, c_void_p]),
+    "goslam_mapping_all_rays": (c_int, [c_void_p, c_int, c_int] + [ctypes.c_double] * 4 + [c_void_p] * 3),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

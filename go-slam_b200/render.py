@@ -13,6 +13,7 @@ import torch
 
 from . import _lib
 from .droid_backends import _workspace
+from .mapping import all_rays
 
 _tables = {}
 
@@ -69,3 +70,39 @@ class Renderer(object):
         z_vals, dists = sample_z(rays_o, rays_d, net.bound, gt_depth, self.N_samples, self.N_surface,
                                  self.perturb, self.lindisp)
         return self.eval_points(rays_o, rays_d, z_vals, dists, net, render_params)
+
+    def render_img(self, net, c2w, device, gt_depth=None):
+        """the reference's render_img (src/render.py:177-237): the whole image's rays in one launch
+        (goslam_mapping_all_rays), then one sample_z + forward per ray_batch_size chunk.  The chunking is kept
+        because it shows in the result: the far clamp uses each chunk's own gt_depth.max(), each chunk draws its own
+        perturb_rand, the forward's mask fix-up is per chunk, and gradient_error comes out as [n_chunks].
+        c2w: [4,4] tensor or ndarray."""
+        with torch.no_grad():
+            H, W = self.H, self.W
+            if not torch.is_tensor(c2w):
+                c2w = torch.from_numpy(c2w)
+            rays_o, rays_d = all_rays(H, W, (self.fx, self.fy, self.cx, self.cy), c2w.to(device))
+            render_params = {
+                'global_step': -1,
+                'gt_depth': None,
+                'stratified': False,
+                'update_state': False,
+                'compute_sdf_smooth_error': False,
+            }
+            render_out = {}
+            step = self.ray_batch_size
+            gt_depth = gt_depth.reshape(-1)        # the reference requires gt_depth here too
+            for i in range(0, H * W, step):
+                out = self.render_batch_ray(rays_o=rays_o[i:i + step], rays_d=rays_d[i:i + step], net=net,
+                                            render_params=render_params, device=device,
+                                            gt_depth=gt_depth[i:i + step])
+                if len(render_out) == 0:
+                    render_out = out
+                    continue
+                for k, v in out.items():
+                    if torch.is_tensor(v):
+                        render_out[k] = torch.cat([render_out[k], v], dim=0)
+                    else:
+                        assert v is None, type(v)
+                        render_out[k] = v
+            return render_out

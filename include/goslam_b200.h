@@ -588,6 +588,49 @@ int goslam_update_op(const goslam_update_weights* weights, const void* net, cons
                      float* delta, float* weight, float* eta, void* upmask, void* workspace,
                      size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Mapping hand-over and ray sampling: Mapper.__call__'s per-frame DepthVideo.get_mapping_item
+ * (src/depth_video.py:153-173) and per-iteration build_rays (src/nerf_func.py:115-181), and render_img's
+ * build_all_rays (:184-221).  Device pointers unless marked host.
+ *
+ * goslam_mapping_snapshot — reads the live buffers images [buffer,3,H,W], mask_filtered, disps_filtered [buffer,H,W]
+ *   (f32) for the F distinct frames frames[F] (device int32) and writes, per frame f (its "slot"), the pixels whose mask
+ *   value is non-zero (NaN included, as `.bool()`) as compact records in raster order: pixel id y*W + x (int32) and
+ *   (r, g, b, depth) (f32) with depth = 1.0f / (disp + 1e-7f), both IEEE-rounded.  A count pass over 1024-pixel tiles,
+ *   a per-frame scan of the tile counts, then an emit pass that places each tile's records at its prefix.  counts[f]
+ *   (device int32) = N_f.  The same launch sequence multiplies update_priority[frames[f]] by decay occurrences[f]
+ *   times (device int32), one f32-rounded multiply at a time.  Frames outside [0, buffer) give N_f = 0 and no decay.
+ *   Workspace: goslam_mapping_snapshot_workspace_bytes(F, H, W) =
+ *     2 * align256(4 * F * ceil(H*W / 1024)) + align256(4 * F * H*W) + align256(16 * F * H*W)
+ *   (0 for F <= 0, F > 65535, H or W <= 0, or H*W > 2^26).  The records live in the workspace; nothing reads the live
+ *   buffers after the three launches.
+ *
+ * goslam_mapping_rays — one training iteration's batch from a snapshot workspace (same F, H, W): n_entries entries
+ *   (host arrays slots[], counts[] = the slot's N_f, draw[]), concatenated in entry order.  draw[e] > 0 takes draw[e]
+ *   records at indices draws[...] (device int64, consecutive per entry in entry order, clamped to [0, N_f - 1]);
+ *   draw[e] == 0 takes all N_f records in raster order.  Per ray, with c2w [F,4,4] (row-major f32, indexed by slot),
+ *   x = column, y = row as exact floats, and from the host doubles fx..cy the f32 values cx' = (float)cx and
+ *   rfx = (float)(1.0 / fx) that torch's CUDA `(x - cx) / fx` uses with Python-float intrinsics:
+ *     dirs = ((x - cx') * rfx, (y - cy') * rfy, 1)
+ *     rays_d[r] = (dirs.x * R[r][0] + dirs.y * R[r][1]) + R[r][2]   each product and sum rounded, no FMA
+ *     rays_o = t,   depth = the record's depth,   color = the record's rgb
+ *   into rays_o, rays_d, color [R,3] and depth [R] (f32), R = sum over entries of (draw > 0 ? draw : N_f) <= max_rays.
+ *   Lists longer than 64 entries are launched in chunks of 64.
+ *
+ * goslam_mapping_all_rays — rays_o, rays_d [H*W,3] of every pixel of one image in raster order under c2w [4,4] (device),
+ *   the arithmetic of goslam_mapping_rays.
+ * ---------------------------------------------------------------------------------- */
+size_t goslam_mapping_snapshot_workspace_bytes(int F, int H, int W);
+int goslam_mapping_snapshot(const float* images, const float* mask, const float* disps, float* update_priority, int buffer,
+                            int H, int W, const int* frames, const int* occurrences, int F, float decay, void* workspace,
+                            size_t workspace_bytes, int* counts, void* stream);
+int goslam_mapping_rays(const void* workspace, size_t workspace_bytes, int F, int H, int W, const float* c2w,
+                        const int64_t* draws, int64_t n_draws, int n_entries, const int* slots, const int* counts,
+                        const int* draw, double fx, double fy, double cx, double cy, float* rays_o, float* rays_d, float* depth,
+                        float* color, int64_t max_rays, void* stream);
+int goslam_mapping_all_rays(const float* c2w, int H, int W, double fx, double fy, double cx, double cy, float* rays_o,
+                            float* rays_d, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
