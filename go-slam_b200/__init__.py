@@ -29,12 +29,12 @@ def install(force=True):
 
 
 def __getattr__(name):
-    """goslam_b200.FactorGraph / DepthVideo / MultiviewFilter / CorrBlock / AltCorrBlock / InstantNeuS, imported on
-    first use"""
+    """goslam_b200.FactorGraph / DepthVideo / MultiviewFilter / MotionFilter / CorrBlock / AltCorrBlock / BasicEncoder /
+    InstantNeuS, imported on first use"""
     import importlib
     where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video",
-             "MultiviewFilter": ".multiview_filter", "CorrBlock": ".modules.corr",
-             "AltCorrBlock": ".modules.corr", "InstantNeuS": ".neus"}
+             "MultiviewFilter": ".multiview_filter", "MotionFilter": ".motion_filter", "CorrBlock": ".modules.corr",
+             "AltCorrBlock": ".modules.corr", "BasicEncoder": ".modules.extractor", "InstantNeuS": ".neus"}
     if name in where:
         return getattr(importlib.import_module(where[name], __name__), name)
     raise AttributeError("module %r has no attribute %r" % (__name__, name))

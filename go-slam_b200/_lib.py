@@ -61,6 +61,14 @@ class ConvDesc(ctypes.Structure):
                 ("split", c_int), ("act2", c_int), ("out2", c_void_p)]
 
 
+class EncoderConv(ctypes.Structure):
+    _fields_ = [("w", c_void_p), ("b", c_void_p)]
+
+
+class EncoderWeights(ctypes.Structure):
+    _fields_ = [("stem", EncoderConv), ("block", (EncoderConv * 3) * 6), ("out", EncoderConv)]
+
+
 # name -> (restype, argtypes); every symbol include/goslam_b200.h declares
 SIGNATURES = {
     "goslam_version": (c_int, []),
@@ -158,6 +166,9 @@ SIGNATURES = {
     "goslam_mapping_rays": (c_int, [c_void_p, c_size_t] + [c_int] * 3 + [c_void_p, c_void_p, c_int64, c_int] +
                             [c_void_p] * 3 + [ctypes.c_double] * 4 + [c_void_p] * 4 + [c_int64, c_void_p]),
     "goslam_mapping_all_rays": (c_int, [c_void_p, c_int, c_int] + [ctypes.c_double] * 4 + [c_void_p] * 3),
+    "goslam_encoder_workspace_bytes": (c_size_t, [c_int] * 4),
+    "goslam_basic_encoder": (c_int, [ctypes.POINTER(EncoderWeights), c_int, c_int, c_void_p, c_int, c_void_p, c_void_p] +
+                             [c_int] * 3 + [c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

@@ -631,6 +631,42 @@ int goslam_mapping_rays(const void* workspace, size_t workspace_bytes, int F, in
 int goslam_mapping_all_rays(const float* c2w, int H, int W, double fx, double fy, double cx, double cy, float* rays_o,
                             float* rays_d, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Feature / context encoder: DroidNet's BasicEncoder forward (src/modules/extractor.py) for norm_fn 'instance'
+ * (fnet: InstanceNorm2d, biased variance, eps 1e-5, no affine) and 'none' (cnet).  Device pointers.
+ *
+ * Weights, one goslam_encoder_conv per nn.Conv2d: w f16 [cout][Kpad] with k = (ky * ks + kx) * cin + ci (the
+ * reference's [cout][cin][ky][kx] permuted to [cout][ky][kx][cin]), Kpad = K except the stem's 147 zero-padded to 160;
+ * b f32 [cout].
+ *   stem        conv1, 7x7 stride 2, 3 -> 32
+ *   block[i]    i = 0..5: layer1.0, layer1.1, layer2.0, layer2.1, layer3.0, layer3.1 (32, 32, 64, 64, 128, 128 out);
+ *               [0] conv1 3x3 (stride 2 for i = 2, 4), [1] conv2 3x3, [2] downsample.0 1x1 stride 2 (i = 2, 4 only;
+ *               ignored otherwise)
+ *   out         conv2, 1x1, 128 -> out_dim
+ *
+ * goslam_basic_encoder — image [B,3,H,W] NCHW (f32, or f16 if image_is_f16); mean, stdv [3] f32 or both NULL: the stem
+ *   reads (x - mean[c]) / stdv[c] in f32 (rounded to f16 after each op for an f16 image), then rounds to f16.
+ *   out_dim % 32 == 0.  Output f16 NCHW: out [B,out_dim,H/8,W/8]; with split (out_dim == 256) out = tanh of channels
+ *   0-127 and out2 = relu of channels 128-255, each [B,128,H/8,W/8], both from the f16-rounded conv output.
+ *   H and W must be multiples of 8 (H*W <= 2^24), B >= 1; otherwise GOSLAM_EINVAL.  About 40 launches on `stream`, no
+ *   host synchronisation; deterministic (instance statistics are merged per tile in a fixed order).
+ *   Workspace: goslam_encoder_workspace_bytes(B, H, W, norm) (0 for an invalid shape or norm).
+ * ---------------------------------------------------------------------------------- */
+#define GOSLAM_NORM_NONE 0
+#define GOSLAM_NORM_INSTANCE 1
+typedef struct goslam_encoder_conv {
+  const void* w; const float* b;
+} goslam_encoder_conv;
+typedef struct goslam_encoder_weights {
+  goslam_encoder_conv stem;
+  goslam_encoder_conv block[6][3];
+  goslam_encoder_conv out;
+} goslam_encoder_weights;
+size_t goslam_encoder_workspace_bytes(int B, int H, int W, int norm);
+int goslam_basic_encoder(const goslam_encoder_weights* weights, int norm, int out_dim, const void* image, int image_is_f16,
+                         const float* mean, const float* stdv, int B, int H, int W, void* out, void* out2, int split,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);

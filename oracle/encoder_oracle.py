@@ -1,0 +1,175 @@
+"""BasicEncoder (src/modules/extractor.py) restated with torch.nn.functional, and the pieces of a MotionFilter replay.
+
+Two modes of `basic_encoder`:
+  float64      every op in f64 (the yardstick);
+  autocast     the same functional graph under torch.autocast("cuda") with f32 weights: every op gets the dtype and
+               rounding point the reference's nn modules get when DroidNet runs them (MotionFilter's autocast).
+Weights are a state_dict with the reference's key names (`conv1.weight`, `layer2.0.downsample.0.bias`, ...).
+"""
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+MEAN = (0.485, 0.456, 0.406)
+STDV = (0.229, 0.224, 0.225)
+
+
+def _norm(x, inst):
+    return F.instance_norm(x, eps=1e-5) if inst else x
+
+
+def _block(sd, p, x, inst, stride):
+    y = F.relu(_norm(F.conv2d(x, sd[p + "conv1.weight"], sd[p + "conv1.bias"], stride, 1), inst))
+    y = F.relu(_norm(F.conv2d(y, sd[p + "conv2.weight"], sd[p + "conv2.bias"], 1, 1), inst))
+    if stride > 1:
+        x = _norm(F.conv2d(x, sd[p + "downsample.0.weight"], sd[p + "downsample.0.bias"], stride), inst)
+    return F.relu(x + y)
+
+
+def _graph(sd, x, inst):
+    x = F.relu(_norm(F.conv2d(x, sd["conv1.weight"], sd["conv1.bias"], 2, 3), inst))
+    for layer, stride in ((1, 1), (2, 2), (3, 2)):
+        x = _block(sd, "layer%d.0." % layer, x, inst, stride)
+        x = _block(sd, "layer%d.1." % layer, x, inst, 1)
+    return F.conv2d(x, sd["conv2.weight"], sd["conv2.bias"])
+
+
+def basic_encoder(sd, norm_fn, x, mean=None, std=None, autocast=False):
+    """x [B, 3, H, W] -> [B, out_dim, H/8, W/8].  mean / std: (x - mean) / std first, in f32 (autocast) or f64.
+    float64 mode returns f64; autocast mode returns what the reference's autocast graph returns (f16)."""
+    if norm_fn not in ("instance", "none"):
+        raise NotImplementedError(norm_fn)
+    inst = norm_fn == "instance"
+    dt = torch.float32 if autocast else torch.float64
+    sd = {k: v.detach().to(x.device, dt) for k, v in sd.items()}
+    x = x.to(dt)
+    if mean is not None:
+        x = (x - torch.tensor(mean, dtype=dt, device=x.device)[:, None, None]) / \
+            torch.tensor(std, dtype=dt, device=x.device)[:, None, None]
+    with torch.no_grad():
+        if not autocast:
+            return _graph(sd, x, inst)
+        with torch.autocast("cuda"):
+            return _graph(sd, x, inst)
+
+
+def context_split(out):
+    """MotionFilter.__context_encoder's split of the 256-channel cnet output"""
+    net, inp = out.split([128, 128], dim=1)
+    return net.tanh(), inp.relu()
+
+
+def errors(got, ref):
+    """(max-abs, rms) of got - ref, both relative to ref's RMS"""
+    d = (got.double() - ref.double())
+    rms = ref.double().pow(2).mean().sqrt().item()
+    return d.abs().max().item() / rms, d.pow(2).mean().sqrt().item() / rms
+
+
+def contract_ok(got, autocast_out, ref64):
+    """the kernel's error against f64 is at most 2x the autocast path's, plus one f16 ulp of the output's scale"""
+    e_k = errors(got, ref64)
+    e_a = errors(autocast_out, ref64)
+    scale = ref64.double().abs().max().item()
+    rms = ref64.double().pow(2).mean().sqrt().item()
+    floor = float(np.spacing(np.float16(scale))) / rms
+    return all(k <= 2.0 * a + floor for k, a in zip(e_k, e_a)), e_k, e_a
+
+
+def seeded_params(module, seed):
+    """fill every parameter in sorted-name order with U(-b, b), b = 1/sqrt(fan_in) (nn.Conv2d's default scale): the
+    same values for the reference's module and ours, whatever their construction order"""
+    g = torch.Generator().manual_seed(seed)
+    params = dict(module.named_parameters())
+    with torch.no_grad():
+        for name in sorted(params):
+            p = params[name]
+            fan_in = p[0].numel() if p.dim() > 1 else max(1, p.numel())
+            b = 1.0 / np.sqrt(fan_in)
+            p.copy_(((torch.rand(p.shape, generator=g, dtype=torch.float64) * 2 - 1) * b).to(p.dtype))
+    return module
+
+
+SHIFTS = (0, 0, 1, 1, 9, 9, 10, 18, 18, 19, 27, 28)
+
+
+def sequence(H=128, W=128, seed=5, shifts=SHIFTS):
+    """a seeded synthetic RGB sequence [len(shifts), 3, H, W] (values k/255, f32): one smooth random field (a 40 x 40
+    bicubic lattice, so that its features decorrelate over a few feature pixels) cropped at offset (s // 2, s) for
+    each shift s: repeated frames, 1-pixel steps and 8-9 pixel jumps"""
+    g = torch.Generator().manual_seed(seed)
+    pad = max(shifts) + 8
+    low = torch.rand(1, 3, 40, 40, generator=g, dtype=torch.float64)
+    field = F.interpolate(low, size=(H + pad, W + pad), mode="bicubic", align_corners=True)[0].clamp(0, 1)
+    imgs = [field[:, s // 2:s // 2 + H, s:s + W] for s in shifts]
+    return (torch.round(torch.stack(imgs) * 255.0) / 255.0).float()
+
+
+def motion_update_params(update, seed):
+    """update-operator weights for the motion-filter replay: seeded_params, then a gate that responds to motion.
+    Random weights alone give nearly the same mean flow on every frame, so:
+      corr_encoder.0   every output = 1 + 0.2 * (mean of the level-0 window - its centre tap): the correlation's
+                       zero-displacement peak above its level (static frame) drives it to 0 through the ReLU, a
+                       frame moved by a few feature pixels leaves it near 1;
+      gru              z = sigmoid(5) with no other input, and q reads only the correlation features (net, inp, flow
+                       and the global-context terms zeroed), so net' ~ q;
+      delta head       seeded, biases zeroed: the flow is ~0 where q ~ 0.
+    The mean flow is then ~0.005-0.01 for repeated frames and 1-pixel steps and ~0.04 for 8-9 pixel jumps."""
+    seeded_params(update, seed)
+    with torch.no_grad():
+        c = update.corr_encoder[0]
+        c.weight.zero_()
+        c.bias.fill_(1.0)
+        c.weight[:, 0:49] = 0.2 / 49.0
+        c.weight[:, 24] -= 0.2
+        gru = update.gru
+        gru.convz.weight.zero_()
+        gru.convz.bias.fill_(5.0)
+        gru.convq.weight[:, :256].zero_()
+        gru.convq.weight[:, 384:].zero_()
+        gru.convq.bias.zero_()
+        for name in ("convz_glo", "convr_glo", "convq_glo"):
+            getattr(gru, name).weight.zero_()
+            getattr(gru, name).bias.zero_()
+        update.delta[0].bias.zero_()
+        update.delta[2].bias.zero_()
+    return update
+
+
+class RecordingVideo:
+    """the part of DepthVideo MotionFilter uses: `counter.value` and `append`, recorded"""
+
+    class _Counter:
+        value = 0
+
+    def __init__(self):
+        self.counter = self._Counter()
+        self.items = []
+
+    def append(self, *item):
+        self.items.append(item)
+        self.counter.value += 1
+
+
+def coords_grid(ht, wd, device):
+    y, x = torch.meshgrid(torch.arange(ht, device=device).float(), torch.arange(wd, device=device).float(), indexing="ij")
+    return torch.stack([x, y], dim=-1)
+
+
+def track_step(fnet_sd, cnet_sd, update, corr_block, state, image, thresh, mean=MEAN, std=STDV):
+    """MotionFilter.track's work for one frame, restated with the autocast oracle encoders (for timing and
+    cross-checks).  state: dict with net / inp / fmap of the last keyframe, or empty.  Returns (accepted, delta mean)."""
+    gmap = basic_encoder(fnet_sd, "instance", image, mean, std, autocast=True)
+    ht, wd = gmap.shape[-2:]
+    if not state:
+        state["net"], state["inp"] = context_split(basic_encoder(cnet_sd, "none", image[:1], mean, std, autocast=True))
+        state["fmap"] = gmap
+        return True, None
+    corr = corr_block(state["fmap"][None, [0]], gmap[None, [0]])(coords_grid(ht, wd, image.device)[None, None])
+    _, delta, _ = update(state["net"][None], state["inp"][None], corr)
+    dm = delta.norm(dim=-1).mean().item()
+    if dm > thresh:
+        state["net"], state["inp"] = context_split(basic_encoder(cnet_sd, "none", image[:1], mean, std, autocast=True))
+        state["fmap"] = gmap
+        return True, dm
+    return False, dm
