@@ -30,7 +30,7 @@ class NeusOut(ctypes.Structure):
         ("color", c_void_p), ("depth", c_void_p), ("depth_variance", c_void_p),
         ("normal", c_void_p), ("weight_sum", c_void_p), ("sdf", c_void_p), ("z_mid", c_void_p),
         ("gradient_error", c_void_p), ("alpha", c_void_p), ("grad", c_void_p), ("pos", c_void_p),
-        ("rgb", c_void_p), ("mlp_in", c_void_p), ("enc", c_void_p),
+        ("rgb", c_void_p), ("mlp_in", c_void_p), ("enc", c_void_p), ("fallback", c_void_p),
     ]
 
 
@@ -118,9 +118,9 @@ SIGNATURES = {
     "goslam_neus_workspace_bytes": (c_size_t, [c_int, c_int]),
     "goslam_neus_forward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 4 + [c_int, c_int] +
                             [ctypes.POINTER(NeusOut), c_void_p, c_size_t, c_void_p]),
-    "goslam_neus_composite_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 12 + [c_int64, c_int, c_int] +
+    "goslam_neus_composite_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 13 + [c_int64, c_int64, c_int, c_int] +
                                        [c_void_p] * 5),
-    "goslam_neus_grid_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 4 + [c_int, c_int] + [c_void_p] * 6),
+    "goslam_neus_grid_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 5 + [c_int64, c_int, c_int] + [c_void_p] * 6),
     "goslam_neus_mlp_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 10 + [c_int, c_int] +
                                  [ctypes.POINTER(NeusMlpBwdOut), c_void_p]),
     "goslam_hashgrid_layout": (c_int64, [c_void_p, c_void_p, c_void_p]),

@@ -80,7 +80,7 @@ struct NeusArgs {
   int R, S;
   float* blk_gerr;        // [grid] partial sums of the eikonal term
   unsigned* blk_count;    // [grid] in-bound sample counts
-  int* flag;              // [1] written by the finalize kernel: 1 = nothing in bound
+  int* flag;              // [1] written by the finalize kernel: 1 = nothing in bound (out.fallback when set)
   int mode;               // 0 main pass, 1 fix-up pass (mask[:100] = True)
   int rays_per_group;     // rays one warp composites together (rays_per_group * S <= kMaxGroup)
 };
@@ -446,6 +446,14 @@ __device__ __forceinline__ void normalise_coord(float p, float b0, float b1, flo
   x01 = __fdiv_rn(__fadd_rn(xn, 1.0f), 2.0f);
 }
 
+// Whether sample `gidx` of a call (its index in [R,S] order) goes through the network: strictly inside realtime_bound,
+// or, when no sample of the whole call is (`forced`, the forward's fallback flag), one of the first 100 — the reference's
+// `pts_mask[:100] = True` (src/InstantNeuS.py:311-312).  The forward and both backward kernels decide with this.
+__device__ __forceinline__ bool sample_in_bound(const float (&pt)[3], const float* rt, long long gidx, bool forced) {
+  const bool inb = pt[0] < rt[1] && pt[0] > rt[0] && pt[1] < rt[3] && pt[1] > rt[2] && pt[2] < rt[5] && pt[2] > rt[4];
+  return inb || (forced && gidx < 100);
+}
+
 __global__ void __launch_bounds__(kThreadsN, 1)
 neus_forward_kernel(const NeusArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -506,10 +514,7 @@ neus_forward_kernel(const NeusArgs a) {
           dir[c] = a.rays_d[(size_t)ray * 3 + c];
           pt[c] = __fadd_rn(a.rays_o[(size_t)ray * 3 + c], __fmul_rn(dir[c], zm));
         }
-        inb = pt[0] < a.p.rt_bound[1] && pt[0] > a.p.rt_bound[0] &&
-              pt[1] < a.p.rt_bound[3] && pt[1] > a.p.rt_bound[2] &&
-              pt[2] < a.p.rt_bound[5] && pt[2] > a.p.rt_bound[4];
-        if (a.mode == 1 && gidx < 100) inb = true;
+        inb = sample_in_bound(pt, a.p.rt_bound, (long long)gidx, a.mode == 1);
       }
 
       // ---- phase 1a: hash-grid encoding (thread per sample) -> enc row in actB ----
@@ -811,6 +816,8 @@ struct CompBwdArgs {
   const float* alpha; const float* rgb; const float* sdf; const float* grad; const float* z_mid;   // saved by the forward
   const float* d_color; const float* d_depth; const float* d_sdf;                                  // upstream (may be null)
   const float* d_gerr;               // dL/d gradient_error[0] (device scalar, may be null)
+  const int* fallback;               // the forward's nothing-in-bound flag (device, may be null = 0)
+  long long sample0;                 // index of this call's first sample within the forward call
   float gerr_norm;                   // 1 / (number of samples gradient_error averages over)
   float* d_mlp_out;                  // [R,S,3]
   float* d_sdf_out;                  // [R,S]
@@ -865,6 +872,7 @@ __global__ void __launch_bounds__(256) neus_composite_bwd_kernel(const CompBwdAr
   }
   const float inv_s = a.p.inv_s, car = a.p.cos_anneal_ratio;
   const float eik = a.d_gerr ? __ldg(a.d_gerr) * a.gerr_norm : 0.f;
+  const bool forced = a.fallback && __ldg(a.fallback) != 0;
   float run = 0.f, dinv = 0.f;
 #pragma unroll
   for (int c = 0; c < kCompChunks; ++c) {
@@ -887,8 +895,7 @@ __global__ void __launch_bounds__(256) neus_composite_bwd_kernel(const CompBwdAr
         float pt[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) pt[k] = __fadd_rn(o[k], __fmul_rn(dir[k], zm));
-        const bool inb = pt[0] < a.p.rt_bound[1] && pt[0] > a.p.rt_bound[0] && pt[1] < a.p.rt_bound[3] &&
-                         pt[1] > a.p.rt_bound[2] && pt[2] < a.p.rt_bound[5] && pt[2] > a.p.rt_bound[4];
+        const bool inb = sample_in_bound(pt, a.p.rt_bound, a.sample0 + (long long)gi, forced);
         float dx[3] = {0.f, 0.f, 0.f}, dsdf = 0.f, dg[3] = {0.f, 0.f, 0.f};
         if (inb) {
           const float d_alpha = G[c] * T[c] - suffix / (1.0f - al[c] + 1e-7f);
@@ -945,6 +952,8 @@ struct GridBwdArgs {
   const float* d_grad;               // [n,3]   dL/d normal (all paths)
   float* grid_grad;                  // [entries*2], accumulated
   float* d_w0;                       // [35] dL/dW_sdf[0,:] through the normal, accumulated
+  const int* fallback;               // the forward's nothing-in-bound flag (device, may be null = 0)
+  long long sample0;                 // index of this call's first sample within the forward call
   long long n; int S;
 };
 
@@ -961,8 +970,7 @@ __global__ void __launch_bounds__(256) neus_grid_bwd_kernel(const GridBwdArgs a)
     float pt[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) pt[c] = __fadd_rn(a.rays_o[ray * 3 + c], __fmul_rn(a.rays_d[ray * 3 + c], zm));
-    act = pt[0] < a.p.rt_bound[1] && pt[0] > a.p.rt_bound[0] && pt[1] < a.p.rt_bound[3] && pt[1] > a.p.rt_bound[2] &&
-          pt[2] < a.p.rt_bound[5] && pt[2] > a.p.rt_bound[4];
+    act = sample_in_bound(pt, a.p.rt_bound, a.sample0 + i, a.fallback && __ldg(a.fallback) != 0);
     if (act) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
@@ -1379,6 +1387,7 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, c
   a.blk_gerr = ar.take<float>(kNumSms * 4);
   a.blk_count = ar.take<unsigned>(kNumSms * 4);
   a.flag = reinterpret_cast<int*>(ar.take<int>(1));
+  if (out->fallback) a.flag = out->fallback;      // the backward reads the decision from there
   // rays per warp work item: make G*S a multiple of 32 when that fits the slab, else pad
   int G = 32 / std::__gcd(S, 32);
   if (G * S > kMaxGroup) G = kMaxGroup / S;
@@ -1400,16 +1409,19 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, c
 int goslam_neus_composite_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
                                    const float* dists, const float* alpha, const float* rgb, const float* sdf,
                                    const float* grad, const float* z_mid, const float* d_color, const float* d_depth,
-                                   const float* d_sdf, const float* d_gradient_error, long long total_samples, int R, int S,
+                                   const float* d_sdf, const float* d_gradient_error, const int* fallback,
+                                   long long total_samples, long long sample0, int R, int S,
                                    float* d_mlp_out, float* d_sdf_out, float* d_grad, float* d_inv_s, void* stream) {
   if (!params || !rays_o || !rays_d || !dists || !alpha || !rgb || !sdf || !grad || !z_mid || !d_mlp_out || !d_sdf_out ||
-      !d_grad || !d_inv_s || R < 0 || S <= 0 || S > 32 * kCompChunks || total_samples < (long long)R * S)
+      !d_grad || !d_inv_s || R < 0 || S <= 0 || S > 32 * kCompChunks || sample0 < 0 ||
+      total_samples < sample0 + (long long)R * S)
     return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
   CompBwdArgs a{};
   a.p = *params; a.rays_o = rays_o; a.rays_d = rays_d; a.dists = dists;
   a.alpha = alpha; a.rgb = rgb; a.sdf = sdf; a.grad = grad; a.z_mid = z_mid;
   a.d_color = d_color; a.d_depth = d_depth; a.d_sdf = d_sdf; a.d_gerr = d_gradient_error;
+  a.fallback = fallback; a.sample0 = sample0;
   a.gerr_norm = total_samples > 0 ? (float)(1.0 / (double)total_samples) : 0.f;
   a.d_mlp_out = d_mlp_out; a.d_sdf_out = d_sdf_out; a.d_grad = d_grad; a.d_inv_s = d_inv_s;
   a.R = R; a.S = S;
@@ -1446,15 +1458,18 @@ int goslam_neus_mlp_backward(const goslam_neus_params* params, const void* mlp_i
 }
 
 int goslam_neus_grid_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
-                              const float* z_vals, const float* dists, int R, int S, const float* d_enc,
-                              const float* d_enc_scale, const float* d_grad, float* grid_grad, float* d_w0, void* stream) {
-  if (!params || !rays_o || !rays_d || !z_vals || !dists || !d_enc || !d_grad || !grid_grad || !d_w0 || R < 0 || S <= 0)
+                              const float* z_vals, const float* dists, const int* fallback, long long sample0, int R, int S,
+                              const float* d_enc, const float* d_enc_scale, const float* d_grad, float* grid_grad, float* d_w0,
+                              void* stream) {
+  if (!params || !rays_o || !rays_d || !z_vals || !dists || !d_enc || !d_grad || !grid_grad || !d_w0 || R < 0 || S <= 0 ||
+      sample0 < 0)
     return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
   { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
   GridBwdArgs a{};
   a.p = *params; a.rays_o = rays_o; a.rays_d = rays_d; a.z_vals = z_vals; a.dists = dists;
   a.d_enc = d_enc; a.d_enc_scale = d_enc_scale; a.d_grad = d_grad; a.grid_grad = grid_grad; a.d_w0 = d_w0;
+  a.fallback = fallback; a.sample0 = sample0;
   a.n = (long long)R * S; a.S = S;
   const long long blocks = (a.n + 255) / 256;
   if (blocks > 0x7fffffffLL) return GOSLAM_EINVAL;

@@ -266,10 +266,12 @@ class InstantNeuS(nn.Module):
         if train:
             f16 = dict(dtype=torch.float16, device=dev)
             self.last_debug.update(rgb=torch.empty((R, S, 3), **f32), mlp_in=torch.empty((R, S, MLP_IN_PAD), **f16),
-                                   enc=torch.empty((R, S, N_LEVELS * N_FEAT), **f16))
+                                   enc=torch.empty((R, S, N_LEVELS * N_FEAT), **f16),
+                                   fallback=torch.empty((1,), dtype=torch.int32, device=dev))
             o.rgb = self.last_debug['rgb'].data_ptr()
             o.mlp_in = self.last_debug['mlp_in'].data_ptr()
             o.enc = self.last_debug['enc'].data_ptr()
+            o.fallback = self.last_debug['fallback'].data_ptr()
         lib = _lib.load()
         with torch.cuda.device(dev):
             ws = _workspace(lib.goslam_neus_workspace_bytes(R, S), dev)
@@ -446,10 +448,15 @@ class _NeusFunction(torch.autograd.Function):
               -> goslam_neus_grid_backward (hash-grid scatter + the second-order path through the analytic normal).
               Chunked over rays to bound the activations."""
     CHUNK_RAYS = 1 << 16
+    MAX_SAMPLES = 128            # goslam_neus_composite_backward keeps up to 4 chunks of 32 samples of a ray in registers
     KEYS = ('color', 'depth', 'sdf', 'gradient_error', 'depth_variance', 'normal', 'weight_sum', 'z_vals', 'sdf_variance')
 
     @staticmethod
     def forward(ctx, net, rays_o, rays_d, z_vals, dists, grid, mlp, sdf_w, sdf_b, color_B, variance):
+        if z_vals.shape[1] > _NeusFunction.MAX_SAMPLES:
+            raise RuntimeError("InstantNeuS.forward under grad: the renderer backward supports at most %d samples per ray, "
+                               "got %d (the forward alone, under torch.no_grad(), takes up to 288)"
+                               % (_NeusFunction.MAX_SAMPLES, z_vals.shape[1]))
         ctx.set_materialize_grads(False)
         rays_o, rays_d = rays_o.detach().float().contiguous(), rays_d.detach().float().contiguous()
         z_vals, dists = z_vals.detach().float().contiguous(), dists.detach().float().contiguous()
@@ -460,14 +467,15 @@ class _NeusFunction(torch.autograd.Function):
         ctx.pstruct = net._params_struct()          # (struct, tensors it points to, inv_s) at forward time
         ctx.save_for_backward(rays_o, rays_d, z_vals, dists, saved['alpha'], saved['grad'], saved['rgb'], saved['mlp_in'],
                               saved['enc'], saved['pos'], out['sdf'], out['z_vals'], sdf_w.detach(), color_B.detach(),
-                              mlp.detach())
+                              mlp.detach(), saved['fallback'])
         vals = tuple(out[k] for k in _NeusFunction.KEYS)
         ctx.mark_non_differentiable(*vals[4:])
         return vals
 
     @staticmethod
     def backward(ctx, d_color, d_depth, d_sdf, d_gerr, *_non_differentiable):
-        (rays_o, rays_d, z_vals, dists, alpha, grad, rgb, mlp_in, enc, pos, sdf, z_mid, sdf_w, color_B, mlp) = ctx.saved_tensors
+        (rays_o, rays_d, z_vals, dists, alpha, grad, rgb, mlp_in, enc, pos, sdf, z_mid, sdf_w, color_B, mlp,
+         fallback) = ctx.saved_tensors
         net = ctx.net
         p, keep, inv_s = ctx.pstruct
         dev = z_vals.device
@@ -506,7 +514,7 @@ class _NeusFunction(torch.autograd.Function):
                     _lib.ptr(sdf[sl]), _lib.ptr(grad[sl]), _lib.ptr(z_mid[sl]),
                     None if dc is None else _lib.ptr(dc), None if dd is None else _lib.ptr(dd),
                     None if dsu is None else _lib.ptr(dsu), None if d_gerr is None else _lib.ptr(d_gerr),
-                    ctypes.c_int64(R * S), r1 - r0, S,
+                    _lib.ptr(fallback), ctypes.c_int64(R * S), ctypes.c_int64(r0 * S), r1 - r0, S,
                     _lib.ptr(d_y), _lib.ptr(d_s), _lib.ptr(d_g), _lib.ptr(g_inv_s), _lib.stream_ptr())
                 _lib.check(rc, "neus_composite_backward")
                 amax = torch.maximum(d_y.abs().max(), d_s.abs().max()).clamp_min(1e-30)
@@ -537,12 +545,12 @@ class _NeusFunction(torch.autograd.Function):
                 g_sdf_b += gs[:, 35]
                 d_enc = torch.mm(d_out, Wsdf_enc, out_dtype=torch.float32)             # [n, 32] f32, still scaled
                 rc = lib.goslam_neus_grid_backward(ctypes.byref(p), _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(zv), _lib.ptr(ds),
-                                                   r1 - r0, S, _lib.ptr(d_enc), _lib.ptr(sc), _lib.ptr(d_gt), _lib.ptr(g_grid),
+                                                   _lib.ptr(fallback), ctypes.c_int64(r0 * S), r1 - r0, S, _lib.ptr(d_enc), _lib.ptr(sc), _lib.ptr(d_gt), _lib.ptr(g_grid),
                                                    _lib.ptr(g_w0), _lib.stream_ptr())
                 _lib.check(rc, "neus_grid_backward")
         g_sdf_w[0] += g_w0
-        # samples outside the real-time bound: the forward zeroed their rows' effect (rgb = 0, alpha = 0), the kernels
-        # return zeros for them, so the GEMMs above see zero rows.
+        # samples the forward kept out of the network (outside the real-time bound and not among the first 100 of a
+        # nothing-in-bound call): rgb = 0, alpha = 0, the kernels return zeros for them, so the GEMMs above see zero rows.
         sf = net.variance_network.scale_factor
         raw = float(torch.exp(net.variance_network.variance.detach().float() * sf))
         g_var = (g_inv_s[0] * inv_s * sf) if 1e-6 <= raw <= 1e6 else torch.zeros((), **f32)

@@ -314,6 +314,10 @@ typedef struct goslam_neus_out {
   float* rgb;            /* [R,S,3]  colour of every sample after the sigmoid (0 outside the bound) */
   void* mlp_in;          /* [R,S,80] f16: the colour network's input row [sin(pB) 33 | normal 3 | feat 31 | 1.0 x 13] */
   void* enc;             /* [R,S,32] f16: hash-grid encoding (0 outside the bound) */
+  /* optional: int [1], set to 1 when no sample of the call lies inside realtime_bound, else 0.  Then, like the
+   * reference (src/InstantNeuS.py:311-312), the first 100 samples of the call ([R,S] order) go through the network as
+   * if in bound.  Pass it to the backward entries so they use the same sample set.  NULL: kept in the workspace. */
+  int* fallback;
 } goslam_neus_out;
 
 size_t goslam_neus_workspace_bytes(int R, int S);
@@ -334,7 +338,13 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o,
  *        of samples gradient_error was averaged over (R*S of the WHOLE forward call when this call covers a slice of it).
  *   out: d_mlp_out [R,S,3] (w.r.t. the colour network's first three outputs, before the sigmoid), d_sdf_out [R,S],
  *        d_grad [R,S,3] (w.r.t. the SDF normal: alpha path + eikonal), d_inv_s [1] (ACCUMULATED: zero it first).
- *   Samples outside the real-time bound get zeros (the forward gives them constants).  S <= 128.
+ *   Samples the forward kept out of the network get zeros (the forward gives them constants): those outside the
+ *   real-time bound, unless *fallback (the forward's goslam_neus_out.fallback; NULL = 0) forced them in.  sample0 = the
+ *   index of this call's first sample within the forward call (r0 * S when this call covers rays r0..); the forced
+ *   samples are the forward call's first 100.  S <= 128.
+ *
+ * Both backward entries decide "in bound" exactly as the forward did, from the recomputed position, fallback and
+ * sample0.
  *
  * goslam_neus_grid_backward — per sample: scatters dL/d(encoding) [R*S,32] (divided by *d_enc_scale when given) and the part of dL/d(normal) [R*S,3] that
  *   flows through the hash grid into grid_grad [n_params] f32 (ACCUMULATED), and accumulates into d_w0 [35] the gradient
@@ -345,11 +355,12 @@ int goslam_neus_composite_backward(const goslam_neus_params* params, const float
                                    const float* dists, const float* alpha, const float* rgb, const float* sdf,
                                    const float* grad, const float* z_mid, const float* d_color,
                                    const float* d_depth, const float* d_sdf, const float* d_gradient_error,
-                                   long long total_samples, int R, int S, float* d_mlp_out, float* d_sdf_out, float* d_grad,
-                                   float* d_inv_s, void* stream);
+                                   const int* fallback, long long total_samples, long long sample0, int R, int S,
+                                   float* d_mlp_out, float* d_sdf_out, float* d_grad, float* d_inv_s, void* stream);
 int goslam_neus_grid_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
-                              const float* z_vals, const float* dists, int R, int S, const float* d_enc,
-                              const float* d_enc_scale, const float* d_grad, float* grid_grad, float* d_w0, void* stream);
+                              const float* z_vals, const float* dists, const int* fallback, long long sample0, int R, int S,
+                              const float* d_enc, const float* d_enc_scale, const float* d_grad, float* grid_grad,
+                              float* d_w0, void* stream);
 /* goslam_neus_mlp_backward — the row-wise half of the colour network's backward (tcnn FullyFusedMLP 80->64->64->16, no
  * biases, ReLU, fp16) in one pass per 32-sample warp tile on mma.sync: recomputes H1, H2 from the kept input rows,
  * dH2 = (dY W3).[H2>0], dH1 = (dH2 W2).[H1>0], dX = dH1 W1, and from dX per sample: dE = dX[:33] cos(p B) (embedding),

@@ -91,7 +91,7 @@ def mapping_loss(net, out, rays_color, rays_depth, w_color=1.0, w_sdf=None, w_ei
 
 
 def composite_backward_closed_form(alpha, rgb, sdf, grad, z_mid, dists, dirs, inb, inv_s, d_color, d_depth, d_sdf, d_gerr,
-                                   cos_anneal_ratio=1.0):
+                                   cos_anneal_ratio=1.0, total_samples=None):
     """The closed form neus_composite_bwd_kernel implements (csrc/neus.cu), in float64 numpy, for ONE call of
     InstantNeuS.forward: given the per-sample alpha / rgb (after the sigmoid) / sdf / normal the forward produced and the
     upstream gradients of color [R,3], depth [R,1], sdf [R,S] and gradient_error (scalar), returns
@@ -101,7 +101,14 @@ def composite_backward_closed_form(alpha, rgb, sdf, grad, z_mid, dists, dirs, in
       dL/dalpha_s = G_s T_s - (sum_{k>s} G_k w_k) / (1 - alpha_s + 1e-7)
       alpha = clip((p - n + 1e-5)/(p + 1e-5), 0, 1), p = sigmoid((sdf - h) inv_s), n = sigmoid((sdf + h) inv_s),
       h = iter_cos * dist / 2, iter_cos = -(relu(-tc/2 + 1/2)(1 - car) + relu(-tc) car), tc = dir . normal
-      gradient_error = mean over ALL samples of (|normal| - 1)^2 [in bound]"""
+      gradient_error = mean over ALL samples of (|normal| - 1)^2 [in bound]
+    total_samples: the number of samples gradient_error averages over when these rays are a slice of a larger call
+    (default R*S).  d_color / d_depth / d_gerr may be None (zero)."""
+    R0, S0 = np.shape(alpha)
+    d_color = np.zeros((R0, 3)) if d_color is None else d_color
+    d_depth = np.zeros((R0, 1)) if d_depth is None else d_depth
+    d_gerr = 0.0 if d_gerr is None else float(d_gerr)
+    total_samples = R0 * S0 if total_samples is None else total_samples
     f8 = np.float64
     alpha, rgb, sdf, grad, z_mid, dists, dirs = [np.asarray(x, f8) for x in (alpha, rgb, sdf, grad, z_mid, dists, dirs)]
     inb = np.asarray(inb, bool)
@@ -131,7 +138,7 @@ def composite_backward_closed_form(alpha, rgb, sdf, grad, z_mid, dists, dirs, in
     d_tc = d_h * dists / 2.0 * ((r0 > 0) * 0.5 * (1 - car) + (r1 > 0) * car)
     d_normal = d_tc[..., None] * dirs[:, None, :]
     gn = np.linalg.norm(grad, axis=-1)
-    eik = d_gerr / (R * S) * 2.0 * (gn - 1.0) / np.where(gn > 0, gn, 1.0)
+    eik = d_gerr / total_samples * 2.0 * (gn - 1.0) / np.where(gn > 0, gn, 1.0)
     d_normal = d_normal + np.where((gn > 0)[..., None], eik[..., None] * grad, 0.0)
     if d_sdf is not None:
         d_sdf_out = d_sdf_out + np.asarray(d_sdf, f8)
@@ -139,7 +146,7 @@ def composite_backward_closed_form(alpha, rgb, sdf, grad, z_mid, dists, dirs, in
     return np.where(m, d_x, 0.0), np.where(inb, d_sdf_out, 0.0), np.where(m, d_normal, 0.0), d_inv_s
 
 
-def grid_backward_closed_form(x01, table, d_enc, q, gy):
+def grid_backward_closed_form(x01, table, d_enc, q, gy, with_abs=False):
     """The closed form neus_grid_bwd_kernel implements (csrc/neus.cu), float64 numpy.  For samples x01 [n,3] in [0,1],
     table [entries,2] (fp16 values), d_enc [n,32] = dL/d(encoding), q [n,3] = dL/d(d sdf / d x01) (the upstream gradient of
     the input-gradient of the scalar field enc . gy), gy [32]:
@@ -147,7 +154,10 @@ def grid_backward_closed_form(x01, table, d_enc, q, gy):
     returns (dL/d table [entries,2], dL/d gy [32]).  Per level l, corner c with trilinear weight w_c and index i_c:
       dL/d table[i_c, f] += d_enc[2l+f] w_c + gy[2l+f] scale_l (q . grad_u w_c),
       dL/d gy[2l+f]      += scale_l sum_c table[i_c, f] (q . grad_u w_c),
-    grad_u w_c along axis a = (+1 if the corner takes the upper cell face on a else -1) x the other two axes' weights."""
+    grad_u w_c along axis a = (+1 if the corner takes the upper cell face on a else -1) x the other two axes' weights.
+    with_abs=True also returns, per entry and feature, the sum of |contribution| over the samples and corners that touch
+    it (with sdot's three axis terms summed unsigned), and per gy entry the same sum of |table value x sdot|: the scale
+    against which fp32 arithmetic and a reduction in any order are measured."""
     f8 = np.float64
     metas, _ = no.hashgrid_meta()
     x01 = np.asarray(x01, np.float32)
@@ -155,6 +165,8 @@ def grid_backward_closed_form(x01, table, d_enc, q, gy):
     d_enc, q, gy = np.asarray(d_enc, f8), np.asarray(q, f8), np.asarray(gy, f8)
     g_tab = np.zeros_like(tab)
     g_gy = np.zeros(32, f8)
+    a_tab = np.zeros_like(tab)
+    a_gy = np.zeros(32, f8)
     with np.errstate(over="ignore"):
         for l, m in enumerate(metas):
             pg, fr, scale = no._pos(m, x01)
@@ -167,6 +179,15 @@ def grid_backward_closed_form(x01, table, d_enc, q, gy):
                                        + (1 if bits[2] else -1) * q[:, 2] * wa[0] * wa[1])
                 gi = m["offset"] + no._grid_index(m, *[pg[:, d] + np.uint32(bits[d]) for d in range(3)])
                 for f in range(2):
-                    np.add.at(g_tab[:, f], gi, d_enc[:, 2 * l + f] * w + gy[2 * l + f] * sdot)
+                    contrib = d_enc[:, 2 * l + f] * w + gy[2 * l + f] * sdot
+                    np.add.at(g_tab[:, f], gi, contrib)
                     g_gy[2 * l + f] += (tab[gi, f] * sdot).sum()
+                    if with_abs:
+                        # sdot's three terms are each ~scale |q| and may cancel: their unsigned sum is the fp32 scale
+                        sabs = float(scale) * (np.abs(q[:, 0]) * wa[1] * wa[2] + np.abs(q[:, 1]) * wa[0] * wa[2]
+                                               + np.abs(q[:, 2]) * wa[0] * wa[1])
+                        np.add.at(a_tab[:, f], gi, np.abs(d_enc[:, 2 * l + f] * w) + np.abs(gy[2 * l + f]) * sabs)
+                        a_gy[2 * l + f] += (np.abs(tab[gi, f]) * sabs).sum()
+    if with_abs:
+        return g_tab, g_gy, a_tab, a_gy
     return g_tab, g_gy

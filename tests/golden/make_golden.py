@@ -299,6 +299,83 @@ def gen_neus_grad():
         tinycudann.Encoding, tinycudann.Network = old
 
 
+NEUS_GRAD_CASES = (          # (tag, R, S, n_uniform, ray seed, nothing in bound)
+    ("s24", 10, 24, 8, 31, False),
+    ("s48", 8, 48, 16, 32, False),
+    ("s72", 6, 72, 24, 33, False),
+    ("fallback", 10, 24, 8, 34, True),
+)
+# realtime_bound of the fallback case: a box in a corner of `bound` that no ray of make_rays reaches, so the reference
+# forces pts_mask[:100] = True — 4 whole rays and 4 samples of the fifth at S = 24
+NEUS_FALLBACK_RT = [[1.9, 1.99], [1.9, 1.99], [1.9, 1.99]]
+
+
+def gen_neus_grad_cases():
+    """Renderer backward golden at the sample counts the configs produce (S = 24, 48, 72) and for a batch with no
+    sample inside realtime_bound: like gen_neus_grad, the REFERENCE's InstantNeuS.forward under enable_grad with the tcnn
+    modules replaced by oracle/neus_grad_oracle.py, the same loss and .backward().  Per case: inputs, forward outputs,
+    loss and every parameter gradient.  The hash-grid gradient is stored as its non-zero entries: int32 index deltas
+    and float32 values with the 8 low mantissa bits cleared (relative error <= 2^-16, compresses)."""
+    neus_mod = ref_import("src.InstantNeuS")
+    import tinycudann
+    from oracle import neus_grad_oracle as ngo
+    from goslam_b200 import synthetic
+    old = tinycudann.Encoding, tinycudann.Network
+    tinycudann.Encoding, tinycudann.Network = ngo.TorchHashGrid, ngo.TorchMLP
+    store = {}
+    try:
+        metas, total_entries = neus_oracle.hashgrid_meta()
+        offs = [m["offset"] * 2 for m in metas] + [total_entries * 2]
+        ress = [m["res"] for m in metas]
+        w = synthetic.make_neus_weights(seed=9, total_grid_params=total_entries * 2, layout=(offs, ress))
+        bound = [[-2.0, 2.0], [-2.0, 2.0], [-2.0, 2.0]]
+        for tag, R, S, n_uniform, seed, fallback in NEUS_GRAD_CASES:
+            net = neus_mod.InstantNeuS(synthetic.NEUS_CFG, bound, device="cpu")
+            with torch.no_grad():
+                net.sdf_network.encoding.encoding.params.copy_(w["grid"])
+                net.sdf_network.sdf_layer.weight.copy_(w["sdf_w"])
+                net.sdf_network.sdf_layer.bias.copy_(w["sdf_b"])
+                net.color_network._B.copy_(w["color_B"])
+                net.color_network.network.params.copy_(w["mlp"])
+            rt = torch.tensor(NEUS_FALLBACK_RT if fallback else [[-1.8, 1.9], [-2.0, 2.0], [-1.5, 2.0]])
+            net.update_bound(rt)
+            ro, rd, zv, ds = synthetic.make_rays(R, S=S, seed=seed, n_uniform=n_uniform)
+            pts = (ro[:, None] + rd[:, None] * (zv + ds / 2.0)[..., None]).reshape(-1, 3)
+            n_inb = int(net.in_bound(pts, rt).sum())
+            assert (n_inb == 0) == fallback, (tag, n_inb)
+            g = torch.Generator().manual_seed(seed)
+            rays_color = torch.rand(R, 3, generator=g)
+            rays_depth = 0.5 + 2.5 * torch.rand(R, generator=g)
+            rays_depth[::7] = 0.0
+            with torch.enable_grad():
+                out = net(ro, rd, zv, ds)
+                depth = rays_depth.reshape(-1, 1)
+                valid = (depth > 0).reshape(-1)
+                unc = 1.0 / torch.sqrt(out["depth_variance"][valid].detach() + 1e-10)
+                color_loss = torch.abs(out["color"][valid] - rays_color[valid]).mean()
+                depth_loss = (torch.abs(out["depth"][valid] - depth[valid]) * unc).mean()
+                sdf_loss, sparse_loss = net.compute_sdf_error(sdf=out["sdf"][valid], z_vals=out["z_vals"][valid], gt_depth=depth[valid])
+                total = color_loss * 2.0 + depth_loss * 1.0 + (sdf_loss + sparse_loss) * 2.0 + 0.1 * out["gradient_error"].mean()
+                total.backward()
+            gg = net.sdf_network.encoding.encoding.params.grad.numpy().astype(np.float32)
+            nz = np.nonzero(gg)[0]
+            val = (gg[nz].view(np.uint32) & np.uint32(0xFFFFFF00)).view(np.float32)
+            case = dict(rays_o=ro.numpy(), rays_d=rd.numpy(), z_vals_in=zv.numpy(), dists=ds.numpy(), rt_bound=rt.numpy(),
+                        rays_color=rays_color.numpy(), rays_depth=rays_depth.numpy(), loss=np.float32(total.item()),
+                        grid_grad_didx=np.diff(nz, prepend=0).astype(np.int32), grid_grad_val=val,
+                        g_sdf_w=net.sdf_network.sdf_layer.weight.grad.numpy(), g_sdf_b=net.sdf_network.sdf_layer.bias.grad.numpy(),
+                        g_color_B=net.color_network._B.grad.numpy(), g_mlp=net.color_network.network.params.grad.numpy(),
+                        g_variance=net.variance_network.variance.grad.numpy(),
+                        **{"out_" + k: v.detach().float().numpy() for k, v in out.items()})
+            store.update({tag + "_" + k: v for k, v in case.items()})
+            print("neus_grad_cases %-8s R=%d S=%d in-bound %d: loss %.6f, %d non-zero grid gradients, |g_sdf_w| %.4e g_var %.4e" % (
+                tag, R, S, n_inb, total.item(), nz.size, np.linalg.norm(case["g_sdf_w"]), float(case["g_variance"])))
+    finally:
+        tinycudann.Encoding, tinycudann.Network = old
+    np.savez_compressed(os.path.join(HERE, "neus_grad_cases.npz"), tags=np.array([c[0] for c in NEUS_GRAD_CASES]),
+                        bound=np.array(bound, np.float32), weights_seed=9, **store)
+
+
 def gen_neus_adamw():
     """Mapping-step trajectory golden: 8 iterations of Mapper.optimize_map's loop body (src/mapping.py:84-131: forward
     under enable_grad, loss, backward, clip_grad_norm_(35), AdamW step with the two parameter groups of :55-58) run by the

@@ -201,3 +201,63 @@ def test_backward_is_independent_of_ray_chunking(monkeypatch):
         # different loss scales per chunk and a different summation order (fp16 operands on the colour network, fp32
         # reductions in scheduling order): a chunking bug (a wrong 1/(R*S), a dropped chunk) is an O(1) error, 1e-2 is ample
         assert float((a - b).abs().max()) <= 1e-2 * scale, (a.shape, float((a - b).abs().max()), scale)
+
+
+GRAD_CASES = ["s24", "s48", "s72", "fallback"]
+
+
+@pytest.mark.parametrize("tag", GRAD_CASES)
+def test_backward_matches_reference_autograd_cases(tag):
+    """tests/golden/neus_grad_cases.npz (make_golden.py neus_grad_cases): the reference's forward + loss + autograd at
+    S = 24, 48, 72 and on a batch with no sample inside realtime_bound, where the reference forces its first 100 samples
+    into the network and gradients flow through them.  Every parameter gradient: relative L2 <= 2e-2, cosine >= 0.9995."""
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "neus_grad_cases.npz"))
+    c = {k[len(tag) + 1:]: g[k] for k in g.files if k.startswith(tag + "_")}
+    net = _net(int(g["weights_seed"]), g["bound"].tolist(), c["rt_bound"])
+    args = [torch.from_numpy(c[k]).to(dev()) for k in ("rays_o", "rays_d", "z_vals_in", "dists")]
+    with torch.enable_grad():
+        out = net(*args)
+        total, _ = _mapping_loss(net, out, torch.from_numpy(c["rays_color"]).to(dev()), torch.from_numpy(c["rays_depth"]).to(dev()))
+    for k in ("color", "depth", "weight_sum", "z_vals"):
+        want = c["out_" + k]
+        assert np.abs(out[k].detach().cpu().numpy().reshape(want.shape) - want).max() <= 2e-3 * max(1.0, np.abs(want).max()), k
+    total.backward()
+    grid_grad = net.sdf_network.encoding.encoding.params.grad.cpu().numpy()
+    idx = np.cumsum(c["grid_grad_didx"].astype(np.int64))
+    want_grid = np.zeros_like(grid_grad)
+    want_grid[idx] = c["grid_grad_val"]
+    _cmp("grid", grid_grad, want_grid)
+    touched = np.nonzero(grid_grad)[0]
+    assert np.setdiff1d(touched, idx).size <= 0.01 * touched.size
+    _cmp("sdf_w", net.sdf_network.sdf_layer.weight.grad.cpu().numpy(), c["g_sdf_w"])
+    _cmp("sdf_w[0]", net.sdf_network.sdf_layer.weight.grad.cpu().numpy()[0], c["g_sdf_w"][0])
+    _cmp("sdf_b", net.sdf_network.sdf_layer.bias.grad.cpu().numpy(), c["g_sdf_b"])
+    _cmp("color_B", net.color_network._B.grad.cpu().numpy(), c["g_color_B"])
+    _cmp("mlp", net.color_network.network.params.grad.cpu().numpy(), c["g_mlp"])
+    gv, wv = float(net.variance_network.variance.grad), float(c["g_variance"])
+    print("variance   got %.6e want %.6e" % (gv, wv))
+    assert abs(gv - wv) <= 2e-2 * abs(wv)
+
+
+def test_fallback_backward_is_independent_of_ray_chunking(monkeypatch):
+    """nothing in bound at S = 24 with CHUNK_RAYS = 2: the 100 forced samples span three backward chunks (48 samples
+    each), so each chunk must place itself in the call (sample0) and read the forward's fallback flag"""
+    from goslam_b200 import neus, synthetic
+    ro, rd, zv, ds = [t.to(dev()) for t in synthetic.make_rays(11, S=24, seed=34, n_uniform=8)]
+    rt = [[1.9, 1.99], [1.9, 1.99], [1.9, 1.99]]
+    gen = torch.Generator().manual_seed(8)
+    cc, cd = torch.randn(11, 3, generator=gen).to(dev()), torch.randn(11, 1, generator=gen).to(dev())
+    grads = []
+    for chunk in (1 << 16, 2):
+        monkeypatch.setattr(neus._NeusFunction, "CHUNK_RAYS", chunk)
+        net = _net(5, [[-2.0, 2.0]] * 3, rt)
+        with torch.enable_grad():
+            o = net(ro, rd, zv, ds)
+            assert int((o["sdf"] != 100.0).sum()) == 100
+            ((o["color"] * cc).sum() + (o["depth"] * cd).sum() + 0.01 * o["sdf"][o["sdf"] != 100.0].sum() + 30.0 * o["gradient_error"].sum()).backward()
+        grads.append([p.grad.clone() for p in net.trainable_tensors()])
+    for a, b in zip(*grads):
+        scale = float(a.abs().max())
+        assert scale > 0
+        # as in test_backward_is_independent_of_ray_chunking: a chunk that misses its forced samples is an O(1) error
+        assert float((a - b).abs().max()) <= 1e-2 * scale, (a.shape, float((a - b).abs().max()), scale)

@@ -110,3 +110,43 @@ def test_grid_backward_closed_form_matches_double_backward_autograd():
     assert np.abs(g_tab - want_tab).max() <= 2e-4 * np.abs(want_tab).max()               # the autograd side runs in float32
     # dL/dgy has the first-order part sum_n enc * 0 (none: d_enc does not multiply gy) and the second-order part only
     assert np.abs(g_gy - gy.grad.numpy()).max() <= 2e-4 * np.abs(gy.grad.numpy()).max()
+
+
+def test_closed_form_options_for_the_kernel_tests():
+    """the options the per-kernel GPU tests use: a ray slice of a larger call (total_samples), upstream gradients passed
+    as None, and the per-entry sum of |contribution| of the grid scatter"""
+    rng = np.random.default_rng(4)
+    R, S = 9, 20
+    alpha = rng.uniform(0, 0.4, (R, S))
+    rgb = rng.uniform(0.05, 0.95, (R, S, 3))
+    sdf, grad = rng.normal(0, 0.3, (R, S)), rng.normal(0, 0.8, (R, S, 3))
+    z = np.sort(rng.uniform(0.2, 3, (R, S)), axis=1)
+    dists, dirs = rng.uniform(0.01, 0.1, (R, S)), rng.normal(0, 1, (R, 3))
+    inb = rng.uniform(size=(R, S)) > 0.2
+    dc, dd, ds = rng.normal(size=(R, 3)), rng.normal(size=(R, 1)), rng.normal(size=(R, S))
+    full = ngo.composite_backward_closed_form(alpha, rgb, sdf, grad, z, dists, dirs, inb, 7.0, dc, dd, ds, 2.5)
+    sl = slice(3, 7)
+    part = ngo.composite_backward_closed_form(alpha[sl], rgb[sl], sdf[sl], grad[sl], z[sl], dists[sl], dirs[sl], inb[sl], 7.0,
+                                              dc[sl], dd[sl], ds[sl], 2.5, total_samples=R * S)
+    for a, b in zip(part[:3], full[:3]):
+        np.testing.assert_allclose(a, b[sl], rtol=1e-12, atol=1e-15)
+    none = ngo.composite_backward_closed_form(alpha, rgb, sdf, grad, z, dists, dirs, inb, 7.0, None, None, None, None)
+    zero = ngo.composite_backward_closed_form(alpha, rgb, sdf, grad, z, dists, dirs, inb, 7.0, np.zeros((R, 3)),
+                                              np.zeros((R, 1)), None, 0.0)
+    for a, b in zip(none, zero):
+        np.testing.assert_array_equal(a, b)
+    assert not np.any(none[0]) and not np.any(none[2]) and none[3] == 0.0
+
+    table = (rng.normal(0, 0.05, (no.hashgrid_meta()[1], 2))).astype(np.float16)
+    x01 = rng.uniform(0, 1, (40, 3)).astype(np.float32)
+    x01[:10] = x01[0]                                        # ten samples on the same point: shared entries
+    d_enc, q, gy = rng.normal(size=(40, 32)), rng.normal(size=(40, 3)), rng.normal(size=32)
+    g_tab, g_gy = ngo.grid_backward_closed_form(x01, table, d_enc, q, gy)
+    g2, gy2, a_tab, a_gy = ngo.grid_backward_closed_form(x01, table, d_enc, q, gy, with_abs=True)
+    np.testing.assert_array_equal(g_tab, g2)
+    np.testing.assert_array_equal(g_gy, gy2)
+    assert np.all(a_tab >= np.abs(g_tab)) and np.all(a_gy >= np.abs(g_gy))
+    assert np.array_equal(a_tab != 0, g_tab != 0)            # touched entries (a zero sum of non-zero terms is measure-zero)
+    # with no normal term and non-negative d_enc every contribution is non-negative: the two sums coincide
+    g3, _, a3, _ = ngo.grid_backward_closed_form(x01, table, np.abs(d_enc), np.zeros_like(q), gy, with_abs=True)
+    np.testing.assert_allclose(a3, g3, rtol=1e-12, atol=0)
