@@ -169,6 +169,8 @@ SIGNATURES = {
     "goslam_encoder_workspace_bytes": (c_size_t, [c_int] * 4),
     "goslam_basic_encoder": (c_int, [ctypes.POINTER(EncoderWeights), c_int, c_int, c_void_p, c_int, c_void_p, c_void_p] +
                              [c_int] * 3 + [c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
+    "goslam_fill_interpolate": (c_int, [c_void_p] * 5 + [c_int, c_int] + [c_void_p] * 3 + [c_int, c_int] +
+                                [c_void_p] * 3),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

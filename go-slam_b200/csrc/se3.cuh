@@ -104,6 +104,35 @@ __device__ __forceinline__ void gs_exp(const float* xi, float* t, float* q) {
   }
 }
 
+// log: SE3 -> se3, the inverse of gs_exp with lietorch.SE3.log's closed form and switches (go-slam_b200/lietorch.py):
+// the rotation vector from the quaternion in the atan2 form that stays continuous for qw < 0 (series below
+// |qv|^2 = 1e-12), then tau = V(phi)^-1 t, left as t at or below theta = 1e-4 where gs_exp leaves t = tau.
+__device__ __forceinline__ void gs_log(const float* t, const float* q, float* xi) {
+  const float n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2];
+  const float w = q[3];
+  float two_atan;
+  if (n2 < 1e-12f) {
+    two_atan = 2.0f / w - (2.0f / 3.0f) * n2 / (w * w * w);
+  } else {
+    const float n = sqrtf(n2);
+    const float sgn = w < 0.0f ? -1.0f : 1.0f;
+    two_atan = 2.0f * sgn * atan2f(n, w * sgn) / n;
+  }
+  float* phi = xi + 3;
+  phi[0] = two_atan * q[0]; phi[1] = two_atan * q[1]; phi[2] = two_atan * q[2];
+  const float th = sqrtf(phi[0] * phi[0] + phi[1] * phi[1] + phi[2] * phi[2]);
+  xi[0] = t[0]; xi[1] = t[1]; xi[2] = t[2];
+  if (th > 1e-4f) {
+    const float half = 0.5f * th;
+    const float coef = (1.0f - th * cosf(half) / (2.0f * sinf(half))) / (th * th);
+    float c[3] = {t[0], t[1], t[2]};
+    gs_cross_inplace(phi, c);                       // c1 = phi x t
+    xi[0] -= 0.5f * c[0]; xi[1] -= 0.5f * c[1]; xi[2] -= 0.5f * c[2];
+    gs_cross_inplace(phi, c);                       // c2 = phi x c1
+    xi[0] += coef * c[0]; xi[1] += coef * c[1]; xi[2] += coef * c[2];
+  }
+}
+
 // T1 = exp(xi) * T   (src/lib/droid_kernels.cu:877-895)
 __device__ __forceinline__ void gs_retr(const float* xi, const float* t, const float* q,
                                         float* t1, float* q1) {

@@ -678,6 +678,26 @@ int goslam_basic_encoder(const goslam_encoder_weights* weights, int norm, int ou
                          const float* mean, const float* stdv, int B, int H, int W, void* out, void* out2, int split,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Non-keyframe trajectory fill: PoseTrajectoryFiller.__fill's bracketing and linear SE3 interpolation
+ * (src/trajectory_filler.py:38-55) and the video hand-over `video[N:N+M] = (tt, ..., Gs, 1, depths, intrinsics / 8,
+ * ...)` (:62-63, src/depth_video.py:85-120), one launch on `stream` with no host synchronisation.  Device pointers.
+ *
+ * goslam_fill_interpolate — the video's live buffers timestamp [buffer], poses [buffer,7], intrinsics [buffer,4],
+ *   disps and disps_sens [buffer,H/8,W/8] (f32), N keyframes in rows 0..N-1; the chunk's M frames: tt [M] (f32
+ *   timestamps), intr_full [M,4] (full-resolution intrinsics), depth [M,H,W] (f32) or NULL.  Per frame k:
+ *     t0 = (number of ts[0:N] <= tt[k]) - 1,  t1 = t0 < N-1 ? t0+1 : t0             (int64, into t0[k], t1[k])
+ *     dt = ts[t1] - ts[t0] + 1e-3,  dP = P[t1] * P[t0]^-1,  v = log(dP) / dt,  w = v * (tt[k] - ts[t0]),
+ *     G = exp(w) * P[t0]                                                            (f32, in this order)
+ *   and row N+k receives timestamp = tt[k], poses = G, intrinsics = intr_full[k] / 8, disps = 1, and with depth
+ *   disps_sens = where(d > 0, 1 / d, d) of depth[k][3::8, 3::8] and disps = disps_sens (without depth disps_sens is
+ *   not written).  A frame before every keyframe (count 0) is bracketed as t0 = 0; callers reject it first.
+ *   N >= 1, 0 <= M <= 65535, H and W multiples of 8; otherwise GOSLAM_EINVAL.  The caller keeps N + M <= buffer.
+ * ---------------------------------------------------------------------------------- */
+int goslam_fill_interpolate(float* timestamp, float* poses, float* intrinsics, float* disps, float* disps_sens, int N,
+                            int M, const float* tt, const float* intr_full, const float* depth, int H, int W,
+                            int64_t* t0, int64_t* t1, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
