@@ -77,14 +77,11 @@ SIGNATURES = {
     "goslam_last_cuda_error": (ctypes.c_char_p, []),
     "goslam_corr_index_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     "goslam_corr_pyramid_lookup": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
-    "goslam_corr_build_workspace_bytes": (c_size_t, [c_int] * 4),
-    "goslam_corr_build": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_size_t, c_void_p]),
+    "goslam_corr_build": (c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_fmaps_to_kmajor": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
-    "goslam_corr_build_indexed": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_corr_level_plane_elems": (c_size_t, [c_int] * 4),
-    "goslam_corr_pool_build": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 5 + [c_void_p]),
+    "goslam_corr_pool_build": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_corr_pool_lookup": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
-    "goslam_corr_build_f32": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_altcorr_forward": (c_int, [c_void_p] * 4 + [c_int] * 8 + [c_void_p]),
     "goslam_altcorr_pyramid": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_frame_distance": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float, c_void_p]),

@@ -2,9 +2,9 @@
 //
 // Reference: CorrBlock.corr / CorrBlock.__init__ (src/modules/corr.py:25-41,67-76):
 //   corr[n] = (fmap1[n]/4)^T (fmap2[n]/4); level i+1 = F.avg_pool2d(level i, 2, 2).
-// This file is (a) the fp32 path of the CPU-shaped config and (b) the validation twin of
-// the wgmma kernel in corr_build_tc.cu (impl=2 in goslam_corr_build): same numerics
-// contract — fp32 accumulate over the 128 channels, x 1/16, one rounding to the volume
+// goslam_corr_build: the row-major build for f32 feature maps and for f16 ones outside the tensor-core
+// kernel's envelope (D != 128 or w > 128), and the validation twin of that kernel (corr_build_tc.cu):
+// same numerics contract — fp32 accumulate over the channels, x 1/16, one rounding to the volume
 // dtype; each pooled level is the mean of the *rounded* finer level (fp32 sum of 4 in
 // row-major window order, x 0.25, one rounding), exactly what avg_pool2d does.
 #include "common.cuh"
@@ -107,25 +107,16 @@ int build_simt(const TIn* f1, const TIn* f2, TOut* const* levels, int num_levels
 
 }  // namespace
 
-// exported to corr_build_tc.cu (same library, C++ linkage)
-int gs_corr_build_simt_f16(const __half* f1, const __half* f2, __half* const* levels,
-                           int num_levels, int N, int D, int h, int w, cudaStream_t st) {
-  return build_simt<__half, __half>(f1, f2, levels, num_levels, N, D, h, w, st);
-}
-int gs_corr_pool_f16(const __half* in, __half* out, long long planes, int h2, int w2,
-                     cudaStream_t st) {
-  const long long total = planes * (h2 >> 1) * (w2 >> 1);
-  if (total <= 0) return GOSLAM_EINVAL;
-  const int blocks = (int)((total + 255) / 256 > kNumSms * 32 ? kNumSms * 32 : (total + 255) / 256);
-  pool2x2_kernel<__half><<<blocks, 256, 0, st>>>(in, out, planes, h2, w2);
-  GS_CHECK_LAUNCH();
-  return GOSLAM_OK;
-}
-
-extern "C" int goslam_corr_build_f32(const float* fmap1, const float* fmap2, float* const* levels,
-                                     int num_levels, int N, int D, int h, int w, void* stream) {
+extern "C" int goslam_corr_build(const void* fmap1, const void* fmap2, int dtype, void* const* levels,
+                                 int num_levels, int N, int D, int h, int w, void* stream) {
   if (N < 0 || D <= 0 || h <= 0 || w <= 0 || num_levels < 1 || num_levels > 4) return GOSLAM_EINVAL;
+  if ((h >> (num_levels - 1)) <= 0 || (w >> (num_levels - 1)) <= 0) return GOSLAM_EINVAL;
+  if (dtype != GOSLAM_F16 && dtype != GOSLAM_F32) return GOSLAM_EINVAL;
   if (N == 0) return GOSLAM_OK;
-  return build_simt<float, float>(fmap1, fmap2, levels, num_levels, N, D, h, w,
-                                  (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == GOSLAM_F16)
+    return build_simt<__half, __half>(static_cast<const __half*>(fmap1), static_cast<const __half*>(fmap2),
+                                      reinterpret_cast<__half* const*>(levels), num_levels, N, D, h, w, st);
+  return build_simt<float, float>(static_cast<const float*>(fmap1), static_cast<const float*>(fmap2),
+                                  reinterpret_cast<float* const*>(levels), num_levels, N, D, h, w, st);
 }

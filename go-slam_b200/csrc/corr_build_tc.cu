@@ -13,25 +13,22 @@
 //               the device (slot1 = rig*ii, slot2 = rig*jj + (ii==jj)), so no gathered copies exist.
 //               A is released as soon as the item's last MMAs retire, so the next item's A and B tiles
 //               load under the current epilogue and band write-out.
-//               Tiled layout: warps 9-11 of this warpgroup are the store warps.  Per band they pool level 3
-//               from the staged level 2 and write both with one TMA tensor store each, out of a double-
-//               buffered band pool handed over by mbarriers ("staged": the 8 consumer warps, "freed": the
-//               store thread after cp.async.bulk.wait_group.read).  The consumer warpgroups never join.
+//               Warps 9-11 of this warpgroup are the store warps.  Per band they pool level 3 from the
+//               staged level 2 and write both with one TMA tensor store each, out of a double-buffered band
+//               pool handed over by mbarriers ("staged": the 8 consumer warps, "freed": the store thread
+//               after cp.async.bulk.wait_group.read).  The consumer warpgroups never join.
 //   warpgroups 0-1  consumers (232 registers each: the 128 fp32 accumulators and the epilogue stay in
 //               registers, no local memory); warpgroup g takes the x-tiles of parity g (B stage g), so
 //               one warpgroup's MMAs overlap the other's epilogue.  A warpgroup issues 32 wgmma m64n64k16
 //               (fp16 in, fp32 accumulate) for the whole 128x128 tile, then per m64 half rounds to fp16.
-//               Tiled layout: level 0 goes into swizzled staging with stmatrix, level 1 is pooled in
-//               registers from the rounded fragment and staged beside it; lane 0 of each warp writes its own
-//               16 source pixels of both with TMA tensor stores, level 0 as soon as it is staged
-//               (tiled_half_epilogue), so the warps of a warpgroup never wait for each other; the
-//               consumers issue no global stores.  Row-major layout: the fragment is transposed through a small per-warp buffer,
-//               each thread then owns 4 rows x 16 columns of its source pixel's patch (level 0 as
-//               full-sector 32-byte stores) and pools level 1 in registers.  Both pool FROM THE ROUNDED
-//               finer level (the avg_pool2d numerics) and stage level 2 (row-major: also level 1) per band;
-//               when the band's x-tiles are done those rows (and level 3, pooled from the staged level 2)
-//               leave as contiguous runs (tiled: through the store warps; row-major: both consumer
-//               warpgroups join and write them out).  The volume is never re-read.
+//               Level 0 goes into swizzled staging with stmatrix, level 1 is pooled in registers from the
+//               rounded fragment and staged beside it; lane 0 of each warp writes its own 16 source pixels
+//               of both with TMA tensor stores, level 0 as soon as it is staged (tiled_half_epilogue), so
+//               the warps of a warpgroup never wait for each other; the consumers issue no global stores.
+//               Every level is pooled FROM THE ROUNDED finer level (the avg_pool2d numerics); level 2 is
+//               staged per band and leaves with level 3 through the store warps.  The volume is never re-read.
+// Output layout (GOSLAM_LAYOUT_TILED): levels 0 and 1 as 4x4-element (32-byte) tiles, levels 2 and 3 as one
+// padded piece per 8-row band, so every store is whole sectors for any h x w.
 // Why the band staging: partial 32-byte-sector writes cost an ECC read-modify-write in L2.
 // The 1/4 feature scaling of the reference (`fmap / 4.0` in half) is applied by the K-major
 // re-layout prepass, exactly as the reference does it, so the accumulator needs no scaling.
@@ -42,9 +39,6 @@
 #include <cuda.h>
 #include <cstdlib>
 #include <cstring>
-
-int gs_corr_build_simt_f16(const __half* f1, const __half* f2, __half* const* levels,
-                           int num_levels, int N, int D, int h, int w, cudaStream_t st);
 
 namespace {
 
@@ -61,47 +55,33 @@ constexpr int kThreadsTC = kEpiThreads + 128;     // + the TMA producer warpgrou
 // register reallocation: 128 x 40 + 256 x 232 <= 65,536 (the producer needs few, the accumulators many)
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr int kMaxXB = 8;                                // x-tiles per band (w <= 128)
-constexpr int kStoreWarps = 3;                           // tiled: producer-warpgroup warps 9-11 write levels 2, 3
+constexpr int kStoreWarps = 3;                           // producer-warpgroup warps 9-11 write levels 2, 3
 // Shared memory, sized per launch from n_xb (the x-tiles of a band); offsets from a 1024-byte aligned base:
-//   item                                        tiled                           row-major
-//   mbarriers                                   1 KB                            1 KB
-//   A tile (128 source px x 128 ch)             32 KB                           32 KB
-//   B stages (2 x 128 target px x 128 ch)       64 KB                           64 KB
-//   level-0 staging (2 per warpgroup, m64)      4 x 16 KB                       -
-//   level-1 staging (2 per warpgroup, m64)      4 x 4 KB                        128 x (64 n_xb + 16) B   (band pool)
-//   level-2/3 band pool                         2 x 128 x (pitch2 + 32) B       128 x (16 n_xb + 8) B
-//   per-warp transpose buffers                  -                               8 x 2,176 B
-//   + 1 KB of alignment slack.  w = 80 (n_xb = 5): tiled 210 KB, row-major 168 KB; w = 128 (n_xb = 8): tiled
-//   218 KB, row-major 198 KB (<= 227 KB).
+//   mbarriers                                   1 KB
+//   A tile (128 source px x 128 ch)             32 KB
+//   B stages (2 x 128 target px x 128 ch)       64 KB
+//   level-0 staging (2 per warpgroup, m64)      4 x 16 KB
+//   level-1 staging (2 per warpgroup, m64)      4 x 4 KB
+//   level-2/3 band pool                         2 x 128 x (pitch2 + 32) B
+//   + 1 KB of alignment slack.  w = 80 (n_xb = 5): 210 KB; w = 128 (n_xb = 8): 218 KB (<= 227 KB).
 constexpr int kBarBytes = 1024;
 constexpr int kL0HalfBytes = 64 * 2 * 128;        // m64 half of a tile's level 0: 64 source px x 2 tile rows x 128 B
 constexpr int kL1HalfBytes = 64 * 64;             // ... of its level 1: 64 source px x one tile row of 2 tiles (64 B)
 constexpr int kL0WarpBytes = kL0HalfBytes / kGroupWarps, kL1WarpBytes = kL1HalfBytes / kGroupWarps;  // 16 source px
-constexpr int kL3BandBytes = kBM * 32;            // tiled: a band's level-3 pieces, 32 B per source pixel
-// per-warp transpose of the accumulator fragment: 8 tile rows x 128 fp16 columns, rows padded to 68 words
-constexpr int kXpRowWords = 68;
-constexpr int kXpWarpBytes = 8 * kXpRowWords * 4;                                 // 2,176 B
+constexpr int kL3BandBytes = kBM * 32;            // a band's level-3 pieces, 32 B per source pixel
 constexpr int kFixedBytes = 1024 + kBarBytes + (1 + kBStages) * kTileBytes;
+// the level-2 staging is dense: one piece of pitch2 bytes per source pixel, the box of the level-2 tensor map
 __host__ __device__ constexpr int pitch2_of(int n_xb) { return (n_xb * 16 + 31) / 32 * 32; }
-// tiled: the level-2 staging is dense (the box of the level-2 tensor map); row-major: padded against bank conflicts
-__host__ __device__ constexpr int pool2_src_bytes(bool tiled, int n_xb) {
-  return tiled ? pitch2_of(n_xb) : 2 * n_xb * 8 + 8;
+// one of the two band buffers, level 2 then level 3
+__host__ __device__ constexpr int band_bytes(int n_xb) { return kBM * pitch2_of(n_xb) + kL3BandBytes; }
+__host__ __device__ constexpr int smem_bytes(int n_xb) {
+  return kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + 2 * band_bytes(n_xb);
 }
-// tiled: one of the two band buffers, level 2 then level 3
-__host__ __device__ constexpr int band_bytes(int n_xb) { return kBM * pool2_src_bytes(true, n_xb) + kL3BandBytes; }
-__host__ __device__ constexpr int pool1_src_bytes(int n_xb) { return 4 * n_xb * 16 + 16; }
-__host__ __device__ constexpr int smem_bytes(bool tiled, int n_xb) {
-  return tiled ? kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + 2 * band_bytes(n_xb)
-               : kFixedBytes + kBM * (pool1_src_bytes(n_xb) + pool2_src_bytes(false, n_xb)) +
-                     kEpiThreads / 32 * kXpWarpBytes;
-}
-static_assert(smem_bytes(true, kMaxXB) <= 227 * 1024 && smem_bytes(false, kMaxXB) <= 227 * 1024,
-              "corr_build_tc_kernel exceeds the 227 KB of shared memory of a block");
+static_assert(smem_bytes(kMaxXB) <= 227 * 1024, "corr_build_tc_kernel exceeds the 227 KB of shared memory of a block");
 
 using namespace gs_tc;
 
 struct TcParams {
-  __half* lvl[4];
   int num_levels, N, h, w, hw;
   int n_mt, n_yb, n_xb;       // m-tiles, y-blocks, x-blocks
   int n_items;                // N * n_mt * n_yb
@@ -109,11 +89,10 @@ struct TcParams {
   // slot1 = rig*ii[e], slot2 = rig*jj[e] + (ii[e]==jj[e])   (src/factor_graph.py:108-113,290)
   const int64_t* ii; const int64_t* jj; int rig;
   const int* out_slot;        // optional edge -> output slot of the level buffers (CorrPool)
-  // tiled: levels 0 and 1 are stored as 4x4-element (32-byte) tiles, tile-row-major inside each
+  // levels 0 and 1 are stored as 4x4-element (32-byte) tiles, tile-row-major inside each
   // source pixel's plane (plane = H4*W4 tiles, padded with zeros); levels 2, 3 stay row-major.
   int w4_0, h4_0, w4_1, h4_1;
-  int pitch2, pitch3;         // tiled: bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
-  int aligned;                // row-major: w % 16 == 0 && h % 8 == 0: every store is a whole aligned sector run
+  int pitch2, pitch3;         // bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
 };
 
 // Build-time switch for profiling builds only (tools/build_variant.py -DGOSLAM_TC_EXPERIMENT=N); the shipped
@@ -142,39 +121,6 @@ __device__ __forceinline__ float pool_pair(uint32_t top, uint32_t bot) {
   s += lo_f(bot);
   s += hi_f(bot);
   return s * 0.25f;
-}
-// store NW packed words (2*NW halves) to dst, honouring alignment and the valid count
-template <int NW>
-__device__ __forceinline__ void store_row(__half* dst, const uint32_t (&r)[NW], int nvalid) {
-  const uintptr_t a = reinterpret_cast<uintptr_t>(dst);
-  if (nvalid >= 2 * NW) {
-    if (NW == 8 && (a & 31) == 0) {     // one full 32-byte sector per lane (2 x STG.128)
-      asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(dst), "r"(r[0]),
-                   "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                   : "memory");
-      return;
-    }
-    if (NW >= 4 && (a & 15) == 0) {
-#pragma unroll
-      for (int i = 0; i < NW; i += 4)
-        *reinterpret_cast<uint4*>(dst + 2 * i) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
-      return;
-    }
-    if (NW == 2 && (a & 7) == 0) {
-      *reinterpret_cast<uint2*>(dst) = make_uint2(r[0], r[1]);
-      return;
-    }
-    if ((a & 3) == 0) {
-#pragma unroll
-      for (int i = 0; i < NW; ++i) *reinterpret_cast<uint32_t*>(dst + 2 * i) = r[i];
-      return;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < NW; ++i) {
-    if (2 * i < nvalid) dst[2 * i] = __ushort_as_half((unsigned short)(r[i] & 0xffffu));
-    if (2 * i + 1 < nvalid) dst[2 * i + 1] = __ushort_as_half((unsigned short)(r[i] >> 16));
-  }
 }
 
 // Tiled epilogue of one m64 half of a 128x128 tile (this warp: 16 source rows x 128 target pixels, the
@@ -270,7 +216,6 @@ __device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], u
   }
 }
 
-template <bool kTiled>
 __global__ void __launch_bounds__(kThreadsTC, 1)
 corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                      const __grid_constant__ CUtensorMap mapL0, const __grid_constant__ CUtensorMap mapL1,
@@ -282,15 +227,14 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(base);
   unsigned char* smA = base + kBarBytes;                       // ONE A stage, reloaded once per band item
   unsigned char* smB = smA + kTileBytes;                       // [kBStages]
-  unsigned char* smEpi = smB + kBStages * kTileBytes;
   uint64_t* full_a = bars;
   uint64_t* empty_a = bars + 1;
   uint64_t* full_b = bars + 2;                   // [kBStages]
   uint64_t* empty_b = full_b + kBStages;
-  uint64_t* staged = empty_b + kBStages;         // tiled: [2] band buffers, written by all consumer warps
-  uint64_t* freed = staged + 2;                  // tiled: [2] ... and read out by the store warps' TMA stores
-  // tiled: level-0 / level-1 staging, two m64 halves per warpgroup, then the two band buffers (levels 2, 3)
-  unsigned char* smL0 = smEpi;
+  uint64_t* staged = empty_b + kBStages;         // [2] band buffers, written by all consumer warps
+  uint64_t* freed = staged + 2;                  // [2] ... and read out by the store warps' TMA stores
+  // level-0 / level-1 staging, two m64 halves per warpgroup, then the two band buffers (levels 2, 3)
+  unsigned char* smL0 = smB + kBStages * kTileBytes;
   unsigned char* smL1 = smL0 + 2 * kBStages * kL0HalfBytes;
   constexpr bool wr = kExperiment != 1;
 
@@ -344,8 +288,8 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           if (++bs == kBStages) { bs = 0; bph ^= 1; }
         }
       }
-    } else if (kTiled && warp > kEpiThreads / 32) {
-      // ===================== store warps (tiled): levels 2 and 3 of each band =====================
+    } else if (warp > kEpiThreads / 32) {
+      // ===================== store warps: levels 2 and 3 of each band =====================
       const int sid = threadIdx.x - (kEpiThreads + 32);          // 0 .. 95
       const int p2src = p.pitch2, p2row = p.n_xb * 8;
       unsigned char* pool2 = smL1 + 2 * kBStages * kL1HalfBytes;
@@ -390,19 +334,13 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     // ===================== consumers (warps 0..7): wgmma + epilogue, two warpgroups =====================
     setmaxnreg_inc<kConsumerRegs>();
     const int group = warp >> 2;                  // takes the tiles of parity `group`, held in B stage `group`
-    const int half = lane >> 4;                   // row-major: patch rows 4*half .. 4*half+3 (columns 64*half..)
     const int etid = threadIdx.x;                 // 0..255
     const int ts = group;
-    // band staging strides (bytes); row-major: the +16 / +8 pads make the per-source-pixel stride conflict-free
-    const int p1row = p.n_xb * 16, p1src = pool1_src_bytes(p.n_xb);
+    // band staging strides (bytes)
     const int p2row = p.n_xb * 8;
-    const int p2src = pool2_src_bytes(kTiled, p.n_xb);
-    unsigned char* pool1 = smEpi;                 // row-major only
-    unsigned char* pool2 = kTiled ? smL1 + 2 * kBStages * kL1HalfBytes : pool1 + kBM * p1src;
-    unsigned char* smXp = pool2 + kBM * p2src;    // row-major only: [8 consumer warps][kXpWarpBytes]
-    uint32_t* xp = reinterpret_cast<uint32_t*>(smXp + warp * kXpWarpBytes);
-    const int h1 = p.h >> 1, w1 = p.w >> 1, h2 = p.h >> 2, w2 = p.w >> 2, h3 = p.h >> 3, w3 = p.w >> 3;
-    if (kTiled && etid < 2 * kBM) {
+    const int p2src = pitch2_of(p.n_xb);
+    unsigned char* pool2 = smL1 + 2 * kBStages * kL1HalfBytes;
+    if (etid < 2 * kBM) {
       // the level-2 piece's padding to pitch2 is written out with it: zeros, once per band buffer
       unsigned char* piece = pool2 + (etid >> 7) * band_bytes(p.n_xb) + (etid & (kBM - 1)) * p2src;
       for (int b = 2 * p2row; b < p2src; b += 4) st_shared_u32(smem_u32(piece + b), 0u);
@@ -414,19 +352,14 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
       const int mt = (item / p.n_yb) % p.n_mt;
       const int n = item / (p.n_yb * p.n_mt);
       const int n_out = p.out_slot ? __ldg(p.out_slot + n) : n;
-      const int y0 = yb * kPY;
       mbar_wait(full_a, aph);
       aph ^= 1;
       bool a_held = true;
-      unsigned char* band = pool2;
-      if constexpr (kTiled) {
-        // tiled: band buffer it % 2, free once the store warps' TMA has read out the band staged there before
-        band += (it & 1) * band_bytes(p.n_xb);
-        mbar_wait(&freed[it & 1], ((it >> 1) & 1) ^ 1);
-      }
+      // band buffer it % 2, free once the store warps' TMA has read out the band staged there before
+      unsigned char* band = pool2 + (it & 1) * band_bytes(p.n_xb);
+      mbar_wait(&freed[it & 1], ((it >> 1) & 1) ^ 1);
       for (int xb = 0; xb < p.n_xb; ++xb, ++tile) {
         if ((tile & (kBStages - 1)) != ts) continue;
-        const int x0 = xb * kPX;
         mbar_wait(&full_b[ts], bph);
         bph ^= 1;
         // 128 x 128 x 128 tile: two m64 row halves, N = 128 as two m64n64 halves (columns 0-63 | 64-127)
@@ -468,7 +401,6 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
         if (xb + kBStages >= p.n_xb) a_held = false;
 #pragma unroll
         for (int mh = 0; mh < 2; ++mh) {
-        if constexpr (kTiled) {
           unsigned char* st0 = smL0 + (group * 2 + mh) * kL0HalfBytes;
           unsigned char* st1 = smL1 + (group * 2 + mh) * kL1HalfBytes;
           // Each warp writes its own 16 source pixels: one bulk group for level 0, issued as soon as its stmatrix
@@ -496,143 +428,16 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
               tma_store_4d_hint(&mapL1, st1 + wq * kL1WarpBytes, xb * 32, yb, s0, n_out, stream);
             bulk_commit();
           }
-        } else {
-        const int row = mh * 64 + (warp & 3) * 16 + (lane & 15);  // tile row = source pixel (after the transpose)
-        const int src = mt * kBM + row;
-        const bool src_ok = src < p.hw && wr;
-        const long long plane_id = (long long)n_out * p.hw + src;
-        // fp16 rounding, then fragment -> (row, half) through the warp's transpose buffer, 8 rows per pass:
-        // hr[R][x] = columns 64*half + 16R + 2x, 2x+1 of the thread's row (patch row 4*half + R)
-        uint32_t hr[4][8];
-#pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-#pragma unroll
-          for (int sub = 0; sub < 2; ++sub)
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              xp[(lane >> 2) * kXpRowWords + sub * 32 + 4 * j + (lane & 3)] =
-                  pack2(acc[mh][sub][4 * j + 2 * pass], acc[mh][sub][4 * j + 2 * pass + 1]);
-          __syncwarp();
-          if (((lane >> 3) & 1) == pass) {
-            const uint4* sp = reinterpret_cast<const uint4*>(xp + (lane & 7) * kXpRowWords + half * 32);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const uint4 v = sp[i];
-              hr[i >> 1][4 * (i & 1)] = v.x; hr[i >> 1][4 * (i & 1) + 1] = v.y;
-              hr[i >> 1][4 * (i & 1) + 2] = v.z; hr[i >> 1][4 * (i & 1) + 3] = v.w;
-            }
-          }
-          __syncwarp();
-        }
-        uint32_t l1[2][4];     // the two level-1 rows this thread produces (8 halves each)
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          const int c = 2 * half + cc;           // 32-column chunk = patch rows 2c, 2c+1
-          if (src_ok) {
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-              const int y = y0 + 2 * c + r;
-              if (y < p.h) store_row<8>(p.lvl[0] + (plane_id * p.h + y) * p.w + x0, hr[2 * cc + r], p.w - x0);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            l1[cc][j] = pack2(pool_pair(hr[2 * cc][2 * j], hr[2 * cc + 1][2 * j]),
-                              pool_pair(hr[2 * cc][2 * j + 1], hr[2 * cc + 1][2 * j + 1]));
-          *reinterpret_cast<uint4*>(pool1 + row * p1src + c * p1row + xb * 16) =
-              make_uint4(l1[cc][0], l1[cc][1], l1[cc][2], l1[cc][3]);
-        }
-        // level-2 row `half` of the band, from the two level-1 rows
-        {
-          const uint32_t a0 = pack2(pool_pair(l1[0][0], l1[1][0]), pool_pair(l1[0][1], l1[1][1]));
-          const uint32_t a1 = pack2(pool_pair(l1[0][2], l1[1][2]), pool_pair(l1[0][3], l1[1][3]));
-          *reinterpret_cast<uint2*>(pool2 + row * p2src + half * p2row + xb * 8) = make_uint2(a0, a1);
-        }
-        }
         }
       }
       // a warp that had no tile in this item releases A here
       if (a_held && lane == 0) mbar_arrive(empty_a);
-      if constexpr (kTiled) {
-        // hand the band to the store warps; the two consumer warpgroups go on without joining
-        fence_async_smem();                      // staged rows become visible to the async (TMA) proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&staged[it & 1]);
-        continue;
-      }
-      // ---- row-major band write-out: both consumer warpgroups have staged every x-tile of this 8-row band ----
-      named_bar_sync(3, kEpiThreads);
-      if (wr && p.num_levels > 1)
-      for (int s_loc = etid >> 2; s_loc < kBM; s_loc += kEpiThreads / 4) {
-        const int part = etid & 3;                             // four threads per source pixel
-        const int s_glb = mt * kBM + s_loc;
-        if (s_glb < p.hw) {
-          const long long pl = (long long)n_out * p.hw + s_glb;
-          const unsigned char* sp1 = pool1 + s_loc * p1src;
-          const unsigned char* sp2 = pool2 + s_loc * p2src;
-          if (p.aligned) {
-            // level 1: 4 full rows, contiguous in memory, 32-byte aligned: whole sectors
-            unsigned char* g1 = reinterpret_cast<unsigned char*>(p.lvl[1]) +
-                                (pl * h1 + (y0 >> 1)) * (long long)p1row;
-            for (int off = part * 32; off < 4 * p1row; off += 128) {
-              uint32_t rr[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) rr[k] = *reinterpret_cast<const uint32_t*>(sp1 + off + 4 * k);
-              asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4}; st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(g1 + off), "r"(rr[0]),
-                           "r"(rr[1]), "r"(rr[2]), "r"(rr[3]), "r"(rr[4]), "r"(rr[5]), "r"(rr[6]), "r"(rr[7])
-                           : "memory");
-            }
-            if (part == 1 && p.num_levels > 2) {                // level 2: 2 rows, 16-byte chunks
-              unsigned char* g2 = reinterpret_cast<unsigned char*>(p.lvl[2]) +
-                                  (pl * h2 + (y0 >> 2)) * (long long)p2row;
-              for (int off = 0; off < 2 * p2row; off += 16)
-                *reinterpret_cast<uint4*>(g2 + off) = make_uint4(
-                    *reinterpret_cast<const uint32_t*>(sp2 + off), *reinterpret_cast<const uint32_t*>(sp2 + off + 4),
-                    *reinterpret_cast<const uint32_t*>(sp2 + off + 8), *reinterpret_cast<const uint32_t*>(sp2 + off + 12));
-            }
-            if (part == 2 && p.num_levels > 3) {                // level 3: 1 row pooled from level 2
-              __half* g3 = p.lvl[3] + (pl * h3 + (y0 >> 3)) * w3;
-              for (int x = 0; x < w3; x += 2) {
-                const uint32_t t = *reinterpret_cast<const uint32_t*>(sp2 + 4 * x);        // row 0: cols 2x, 2x+1
-                const uint32_t t2 = *reinterpret_cast<const uint32_t*>(sp2 + 4 * x + 4);   //        cols 2x+2, 2x+3
-                const uint32_t b = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 4 * x);
-                const uint32_t b2 = *reinterpret_cast<const uint32_t*>(sp2 + p2row + 4 * x + 4);
-                *reinterpret_cast<uint32_t*>(g3 + x) = pack2(pool_pair(t, b), pool_pair(t2, b2));
-              }
-            }
-          } else {
-            // ragged shapes: element-wise with bounds (staging rows are n_xb*8 / n_xb*4 halves wide)
-            const __half* s1 = reinterpret_cast<const __half*>(sp1);
-            const __half* s2 = reinterpret_cast<const __half*>(sp2);
-            for (int r = 0; r < 4; ++r) {
-              const int y = (y0 >> 1) + r;
-              if (y >= h1) break;
-              __half* g = p.lvl[1] + (pl * h1 + y) * w1;
-              for (int x = part; x < w1; x += 4) g[x] = s1[r * (p1row / 2) + x];
-            }
-            if (p.num_levels > 2)
-              for (int r = 0; r < 2; ++r) {
-                const int y = (y0 >> 2) + r;
-                if (y >= h2) break;
-                __half* g = p.lvl[2] + (pl * h2 + y) * w2;
-                for (int x = part; x < w2; x += 4) g[x] = s2[r * (p2row / 2) + x];
-              }
-            if (p.num_levels > 3 && (y0 >> 3) < h3) {
-              __half* g = p.lvl[3] + (pl * h3 + (y0 >> 3)) * w3;
-              for (int x = part; x < w3; x += 4) {
-                float sum = __half2float(s2[2 * x]);
-                sum += __half2float(s2[2 * x + 1]);
-                sum += __half2float(s2[(p2row / 2) + 2 * x]);
-                sum += __half2float(s2[(p2row / 2) + 2 * x + 1]);
-                g[x] = __float2half_rn(sum * 0.25f);
-              }
-            }
-          }
-        }
-      }
-      named_bar_sync(3, kEpiThreads);
+      // hand the band to the store warps; the two consumer warpgroups go on without joining
+      fence_async_smem();                        // staged rows become visible to the async (TMA) proxy
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&staged[it & 1]);
     }
-    if (kTiled) bulk_wait_all();
+    bulk_wait_all();
   }
 }
 
@@ -787,27 +592,23 @@ bool cached_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
   return true;
 }
 
-// launch the tensor-core kernel on K-major (pre-scaled) operands: f1t/f2t = [F1|F2, hw, 128]
-int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_t* ii,
-              const int64_t* jj, int rig, const int* out_slot, int tiled, __half* const* levels,
-              int num_levels, int N, int h, int w, cudaStream_t st) {
+// launch the tensor-core kernel on the video-level K-major (pre-scaled) feature maps f = [F, hw, 128]
+int launch_tc(const __half* f, int F, const int64_t* ii, const int64_t* jj, int rig, const int* out_slot,
+              __half* const* levels, int num_levels, int N, int h, int w, cudaStream_t st) {
   const int hw = h * w;
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return GOSLAM_ELAUNCH;
+  // the tensor stores need 16-byte aligned level buffers
+  for (int i = 0; i < num_levels; ++i)
+    if (reinterpret_cast<uintptr_t>(levels[i]) & 15) return GOSLAM_EINVAL;
   CUtensorMap mapA, mapB, mapL0, mapL1, mapL2, mapL3;
-  if (!cached_map(enc, MapKey{f1t, F1, h, w, 0}, &mapA) || !cached_map(enc, MapKey{f2t, F2, h, w, 1}, &mapB))
+  if (!cached_map(enc, MapKey{f, F, h, w, 0}, &mapA) || !cached_map(enc, MapKey{f, F, h, w, 1}, &mapB))
     return GOSLAM_ELAUNCH;
-  mapL0 = mapL1 = mapL2 = mapL3 = mapA;      // row-major: unused
-  if (tiled) {
-    // the tensor stores need 16-byte aligned level buffers
-    for (int i = 0; i < num_levels; ++i)
-      if (reinterpret_cast<uintptr_t>(levels[i]) & 15) return GOSLAM_EINVAL;
-    CUtensorMap* maps[4] = {&mapL0, &mapL1, &mapL2, &mapL3};
-    for (int i = 0; i < num_levels; ++i)
-      if (!cached_map(enc, MapKey{levels[i], 0, h, w, 2 + i}, maps[i])) return GOSLAM_ELAUNCH;
-  }
+  mapL0 = mapL1 = mapL2 = mapL3 = mapA;      // the maps of levels >= num_levels are unused
+  CUtensorMap* maps[4] = {&mapL0, &mapL1, &mapL2, &mapL3};
+  for (int i = 0; i < num_levels; ++i)
+    if (!cached_map(enc, MapKey{levels[i], 0, h, w, 2 + i}, maps[i])) return GOSLAM_ELAUNCH;
   TcParams p{};
-  for (int i = 0; i < 4; ++i) p.lvl[i] = i < num_levels ? levels[i] : nullptr;
   p.num_levels = num_levels; p.N = N; p.h = h; p.w = w; p.hw = hw;
   p.n_mt = gs_cdiv(hw, kBM); p.n_yb = gs_cdiv(h, kPY); p.n_xb = gs_cdiv(w, kPX);
   p.n_items = N * p.n_mt * p.n_yb;
@@ -815,7 +616,6 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   p.w4_0 = gs_cdiv(w, 4); p.h4_0 = gs_cdiv(h, 4);
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
   p.pitch2 = pitch2_of(p.n_xb); p.pitch3 = 32;
-  p.aligned = (w % 16 == 0 && h % 8 == 0) ? 1 : 0;
   // per-device: opt-in shared memory + SM count, looked up once per device
   static int sm_count[64];
   static std::mutex dev_mu;
@@ -826,10 +626,8 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
   {
     std::lock_guard<std::mutex> lock(dev_mu);
     if (sm_count[dev] == 0) {
-      if (cudaFuncSetAttribute(corr_build_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               smem_bytes(true, kMaxXB)) != cudaSuccess ||
-          cudaFuncSetAttribute(corr_build_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               smem_bytes(false, kMaxXB)) != cudaSuccess)
+      if (cudaFuncSetAttribute(corr_build_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               smem_bytes(kMaxXB)) != cudaSuccess)
         return GOSLAM_ELAUNCH;
       int n = kNumSms;
       cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
@@ -838,37 +636,14 @@ int launch_tc(const __half* f1t, int F1, const __half* f2t, int F2, const int64_
     sms = sm_count[dev];
   }
   const int grid = p.n_items < sms ? p.n_items : sms;
-  const int smem = smem_bytes(tiled != 0, p.n_xb);
-  if (tiled)
-    corr_build_tc_kernel<true><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
-  else
-    corr_build_tc_kernel<false><<<grid, kThreadsTC, smem, st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
+  corr_build_tc_kernel<<<grid, kThreadsTC, smem_bytes(p.n_xb), st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
-}
-
-int build_tc(const __half* f1, const __half* f2, __half* const* levels, int num_levels, int N,
-             int h, int w, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  const int hw = h * w;
-  const size_t per = (size_t)N * hw * kD * sizeof(__half);
-  if (workspace == nullptr || workspace_bytes < 2 * gs_align(per)) return GOSLAM_EWORKSPACE;
-  __half* f1t = reinterpret_cast<__half*>(workspace);
-  __half* f2t = reinterpret_cast<__half*>(reinterpret_cast<char*>(workspace) + gs_align(per));
-  dim3 tg(gs_cdiv(hw, 64), N);
-  to_kmajor_kernel<<<tg, 256, 0, st>>>(f1, f1t, hw);
-  to_kmajor_kernel<<<tg, 256, 0, st>>>(f2, f2t, hw);
-  GS_CHECK_LAUNCH();
-  return launch_tc(f1t, N, f2t, N, nullptr, nullptr, 1, nullptr, 0, levels, num_levels, N, h, w, st);
 }
 
 }  // namespace
 
 extern "C" {
-
-size_t goslam_corr_build_workspace_bytes(int N, int D, int h, int w) {
-  if (N <= 0 || D != kD) return 256;
-  return 2 * gs_align((size_t)N * h * w * kD * sizeof(__half)) + 256;
-}
 
 int goslam_fmaps_to_kmajor(const void* fmaps, void* out, int F, int D, int h, int w, void* stream) {
   if (F < 0 || D != kD || h <= 0 || w <= 0) return GOSLAM_EINVAL;
@@ -878,13 +653,6 @@ int goslam_fmaps_to_kmajor(const void* fmaps, void* out, int F, int D, int h, in
                                                          reinterpret_cast<__half*>(out), h * w);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
-}
-
-int goslam_corr_build_indexed(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
-                              const int64_t* jj, void* const* levels, int num_levels, int N, int D,
-                              int h, int w, void* stream) {
-  return goslam_corr_pool_build(fmaps_kmajor, F, rig, ii, jj, nullptr, GOSLAM_LAYOUT_ROWMAJOR, levels,
-                                num_levels, N, D, h, w, stream);
 }
 
 size_t goslam_corr_level_plane_elems(int level, int layout, int h, int w) {
@@ -901,36 +669,15 @@ size_t goslam_corr_level_plane_elems(int level, int layout, int h, int w) {
 }
 
 int goslam_corr_pool_build(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
-                           const int64_t* jj, const int* slots, int layout, void* const* levels,
+                           const int64_t* jj, const int* slots, void* const* levels,
                            int num_levels, int N, int D, int h, int w, void* stream) {
-  if (layout != GOSLAM_LAYOUT_ROWMAJOR && layout != GOSLAM_LAYOUT_TILED) return GOSLAM_EINVAL;
   if (N < 0 || F <= 0 || rig < 1 || D != kD || h <= 0 || w <= 0 || num_levels < 1 || num_levels > 4)
     return GOSLAM_EINVAL;
   if ((h >> (num_levels - 1)) <= 0 || (w >> (num_levels - 1)) <= 0) return GOSLAM_EINVAL;
   if (w > kMaxXB * kPX) return GOSLAM_EINVAL;
   if (N == 0) return GOSLAM_OK;
-  const __half* f = reinterpret_cast<const __half*>(fmaps_kmajor);
-  return launch_tc(f, F, f, F, ii, jj, rig, slots, layout == GOSLAM_LAYOUT_TILED,
+  return launch_tc(reinterpret_cast<const __half*>(fmaps_kmajor), F, ii, jj, rig, slots,
                    reinterpret_cast<__half* const*>(levels), num_levels, N, h, w, (cudaStream_t)stream);
-}
-
-int goslam_corr_build(const void* fmap1, const void* fmap2, void* const* levels, int num_levels,
-                      int N, int D, int h, int w, int impl, void* workspace,
-                      size_t workspace_bytes, void* stream) {
-  if (N < 0 || D <= 0 || h <= 0 || w <= 0 || num_levels < 1 || num_levels > 4) return GOSLAM_EINVAL;
-  if ((h >> (num_levels - 1)) <= 0 || (w >> (num_levels - 1)) <= 0) return GOSLAM_EINVAL;
-  if (N == 0) return GOSLAM_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  const __half* f1 = reinterpret_cast<const __half*>(fmap1);
-  const __half* f2 = reinterpret_cast<const __half*>(fmap2);
-  __half* const* lv = reinterpret_cast<__half* const*>(levels);
-  if (impl == 0) impl = (D == kD && w <= kMaxXB * kPX) ? 1 : 2;
-  if (impl == 1) {
-    if (D != kD || w > kMaxXB * kPX) return GOSLAM_EINVAL;
-    return build_tc(f1, f2, lv, num_levels, N, h, w, workspace, workspace_bytes, st);
-  }
-  if (impl == 2) return gs_corr_build_simt_f16(f1, f2, lv, num_levels, N, D, h, w, st);
-  return GOSLAM_EINVAL;
 }
 
 }  // extern "C"

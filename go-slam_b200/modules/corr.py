@@ -1,11 +1,16 @@
 """CorrBlock / AltCorrBlock with the reference's constructor and call signatures
 (src/modules/corr.py:25-65,97-145), backed by the sm_90a kernels.
 
-CorrBlock(fmap1, fmap2)      -> wgmma all-pairs build + in-epilogue 4-level pyramid
-                                (goslam_corr_build; reference: torch.matmul + 3x avg_pool2d)
-CorrBlock.__call__(coords)   -> ONE fused 4-level radius-3 lookup (goslam_corr_pyramid_lookup;
-                                reference: 4 x corr_index_forward + torch.cat)
+CorrBlock(fmap1, fmap2)      -> half inputs with D == 128, w <= 128: the wgmma all-pairs build with the
+                                4-level pyramid in its epilogue, into a private CorrPool (goslam_corr_pool_build);
+                                anything else (float32, other shapes): the CUDA-core build, row-major
+                                (goslam_corr_build).  Reference: torch.matmul + 3x avg_pool2d.
+CorrBlock.__call__(coords)   -> ONE fused 4-level radius-3 lookup (goslam_corr_pool_lookup /
+                                goslam_corr_pyramid_lookup; reference: 4 x corr_index_forward + torch.cat)
 AltCorrBlock(fmaps)(coords, ii, jj) -> windowed correlation, all levels in one launch (goslam_altcorr_pyramid)
+
+A pooled pyramid is in the tiled layout, private to the build and lookup kernels; `corr_pyramid` /
+`gather_pyramid()` give the reference's [N, h, w, h>>i, w>>i] levels as a de-tiled copy.
 """
 import ctypes
 
@@ -13,7 +18,6 @@ import torch
 import torch.nn.functional as F
 
 from .. import _lib
-from ..droid_backends import _workspace
 
 
 def _ptr_array(tensors):
@@ -34,14 +38,15 @@ class CorrPool:
     one.  The build and lookup kernels follow the table on the device
     (goslam_corr_pool_build / goslam_corr_pool_lookup)."""
 
-    ROWMAJOR, TILED = 0, 1
+    TILED = 1                                                    # == GOSLAM_LAYOUT_TILED
 
     def __init__(self, capacity, ht, wd, num_levels=4, device="cuda", layout="tiled"):
-        """layout "tiled" (default): levels 0/1 as 4x4-element tiles (one 32-byte sector each),
+        """levels 0/1 as 4x4-element tiles (one 32-byte sector each), levels 2/3 as padded band pieces,
         private to the build and lookup kernels — nothing else in GO-SLAM reads the pyramid
-        (include/goslam_b200.h, GOSLAM_LAYOUT_TILED); "rowmajor": the reference's layout."""
+        (include/goslam_b200.h, GOSLAM_LAYOUT_TILED).  "tiled" is the only layout."""
+        if layout != "tiled":
+            raise ValueError("CorrPool: layout must be \"tiled\", got %r" % (layout,))
         self.capacity, self.ht, self.wd, self.num_levels = int(capacity), ht, wd, num_levels
-        self.layout = {"tiled": self.TILED, "rowmajor": self.ROWMAJOR}[layout]
         self.plane_elems = [self._plane_elems(i) for i in range(num_levels)]
         self.levels = [torch.empty((self.capacity, ht * wd, self.plane_elems[i]), dtype=torch.float16, device=device)
                        for i in range(num_levels)]
@@ -56,31 +61,27 @@ class CorrPool:
             return self._iota[slots[0]:slots[0] + n]
         return torch.tensor(slots, dtype=torch.int32, device=self._iota.device)
 
-    def _plane_elems(self, i):
+    def _plane_elems(self, i):                                   # == goslam_corr_level_plane_elems
         hl, wl = self.ht >> i, self.wd >> i
-        if self.layout == self.TILED:                             # == goslam_corr_level_plane_elems
-            if i < 2:
-                return ((hl + 3) // 4) * ((wl + 3) // 4) * 16
-            n_yb, n_xb = (self.ht + 7) // 8, (self.wd + 15) // 16
-            return n_yb * ((n_xb * 8 + 15) // 16 * 16) if i == 2 else n_yb * 16
-        return hl * wl
+        if i < 2:
+            return ((hl + 3) // 4) * ((wl + 3) // 4) * 16
+        n_yb, n_xb = (self.ht + 7) // 8, (self.wd + 15) // 16
+        return n_yb * ((n_xb * 8 + 15) // 16 * 16) if i == 2 else n_yb * 16
 
     def level_rowmajor(self, i, slots=None):
         """level i as [n, ht, wd, ht>>i, wd>>i] (a gathered, de-tiled copy; tests / debugging)."""
         lvl = self.levels[i] if slots is None else self.levels[i][slots]
         hl, wl = self.ht >> i, self.wd >> i
         n = lvl.shape[0]
-        if self.layout == self.TILED and i < 2:
+        if i < 2:
             h4, w4 = (hl + 3) // 4, (wl + 3) // 4
             lvl = lvl.view(n, self.ht, self.wd, h4, w4, 4, 4).permute(0, 1, 2, 3, 5, 4, 6)
             return lvl.reshape(n, self.ht, self.wd, 4 * h4, 4 * w4)[..., :hl, :wl].contiguous()
-        if self.layout == self.TILED:
-            n_yb, n_xb = (self.ht + 7) // 8, (self.wd + 15) // 16
-            if i == 2:          # per band: 2 rows of n_xb*4 columns, padded to a multiple of 16 elements
-                lvl = lvl.view(n, self.ht, self.wd, n_yb, -1)[..., :2 * n_xb * 4]
-                return lvl.reshape(n, self.ht, self.wd, 2 * n_yb, n_xb * 4)[..., :hl, :wl].contiguous()
-            return lvl.view(n, self.ht, self.wd, n_yb, 16)[..., :hl, :wl].contiguous()
-        return lvl.view(n, self.ht, self.wd, hl, wl)
+        n_yb, n_xb = (self.ht + 7) // 8, (self.wd + 15) // 16
+        if i == 2:              # per band: 2 rows of n_xb*4 columns, padded to a multiple of 16 elements
+            lvl = lvl.view(n, self.ht, self.wd, n_yb, -1)[..., :2 * n_xb * 4]
+            return lvl.reshape(n, self.ht, self.wd, 2 * n_yb, n_xb * 4)[..., :hl, :wl].contiguous()
+        return lvl.view(n, self.ht, self.wd, n_yb, 16)[..., :hl, :wl].contiguous()
 
     @property
     def free_slots(self):
@@ -114,9 +115,12 @@ class CorrPool:
 
 
 class CorrBlock:
-    pool = None          # set for slot-pool blocks (see CorrPool); then `slots`/`_slots_host` exist
+    """A half-precision block inside the tensor-core envelope lives in a CorrPool (`pool`, `slots`,
+    `_slots_host`): the factor graph's, or a private one.  Any other block holds the reference's
+    row-major list of levels (`_levels`) from the CUDA-core build."""
+    pool = None
 
-    def __init__(self, fmap1, fmap2, num_levels=4, radius=3, impl=0):
+    def __init__(self, fmap1, fmap2, num_levels=4, radius=3):
         self.num_levels = num_levels
         self.radius = radius
         if not fmap1.is_cuda:
@@ -125,73 +129,63 @@ class CorrBlock:
         N = batch * num
         self.ht, self.wd = ht, wd
         dev = fmap1.device
-        f1 = fmap1.reshape(N, dim, ht, wd).contiguous()
-        f2 = fmap2.reshape(N, dim, ht, wd).contiguous()
-        lib = _lib.load()
-        if f1.dtype == torch.float16:
-            f2 = f2.half()             # named: a converted copy must outlive the launch
-            levels = [torch.empty((N, ht, wd, ht >> i, wd >> i), dtype=torch.float16, device=dev)
-                      for i in range(num_levels)]
-            with torch.cuda.device(dev):
-                nbytes = lib.goslam_corr_build_workspace_bytes(N, dim, ht, wd)
-                ws = _workspace(nbytes, dev)
-                rc = lib.goslam_corr_build(
-                    _lib.ptr(f1), _lib.ptr(f2), _ptr_array(levels), num_levels, N, dim, ht, wd,
-                    int(impl), _lib.ptr(ws), ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-            _lib.check(rc, "corr_build")
-        else:
-            f1, f2 = f1.float(), f2.float()
-            levels = [torch.empty((N, ht, wd, ht >> i, wd >> i), dtype=torch.float32, device=dev)
-                      for i in range(num_levels)]
-            with torch.cuda.device(dev):
-                rc = lib.goslam_corr_build_f32(_lib.ptr(f1), _lib.ptr(f2), _ptr_array(levels),
-                                               num_levels, N, dim, ht, wd, _lib.stream_ptr())
-            _lib.check(rc, "corr_build_f32")
-        self.corr_pyramid = levels
+        if fmap1.dtype == torch.float16 and dim == 128 and wd <= 128:
+            # both maps K-major in one [2N, hw, 128] buffer; edge e pairs frame e with frame N + e
+            km = torch.empty((2 * N, ht * wd, 128), dtype=torch.float16, device=dev)
+            fmaps_to_kmajor(fmap1.reshape(N, dim, ht, wd), out=km[:N])
+            fmaps_to_kmajor(fmap2.reshape(N, dim, ht, wd).half(), out=km[N:])
+            ii = torch.arange(N, device=dev)
+            self._build_pooled(km, ii, ii + N, 1, None)
+            return
+        dtype = torch.float16 if fmap1.dtype == torch.float16 else torch.float32
+        f1 = fmap1.reshape(N, dim, ht, wd).to(dtype).contiguous()
+        f2 = fmap2.reshape(N, dim, ht, wd).to(dtype).contiguous()   # named: a converted copy must outlive the launch
+        self._levels = [torch.empty((N, ht, wd, ht >> i, wd >> i), dtype=dtype, device=dev)
+                        for i in range(num_levels)]
+        with torch.cuda.device(dev):
+            rc = _lib.load().goslam_corr_build(
+                _lib.ptr(f1), _lib.ptr(f2), 1 if dtype == torch.float16 else 0, _ptr_array(self._levels),
+                num_levels, N, dim, ht, wd, _lib.stream_ptr())
+        _lib.check(rc, "corr_build")
 
     @classmethod
     def from_video(cls, fmaps_kmajor, ii, jj, ht, wd, rig=1, num_levels=4, radius=3, pool=None):
         """FactorGraph.add_factors' volume for edges (ii, jj) straight from video-level K-major
         feature maps [buffer*rig, ht*wd, 128] (see `fmaps_to_kmajor`): no gathered copies.
-        With `pool` the volumes are written into free slots of that CorrPool."""
+        The volumes are written into free slots of `pool`, or of a private CorrPool without one."""
         self = cls.__new__(cls)
         self.num_levels, self.radius, self.ht, self.wd = num_levels, radius, ht, wd
+        self._build_pooled(fmaps_kmajor, ii, jj, rig, pool)
+        return self
+
+    def _build_pooled(self, fmaps_kmajor, ii, jj, rig, pool):
         dev = fmaps_kmajor.device
         N = int(ii.shape[0])
-        F = int(fmaps_kmajor.shape[0])
-        if pool is not None:
-            if (pool.ht, pool.wd, pool.num_levels) != (ht, wd, num_levels):
-                raise RuntimeError("CorrBlock.from_video: pool shape mismatch")
-            self.pool = pool
-            self._slots_host = pool.alloc(N)
-            self.slots = pool.slot_table(self._slots_host)
-            with torch.cuda.device(dev):
-                rc = _lib.load().goslam_corr_pool_build(
-                    _lib.ptr(fmaps_kmajor), F, int(rig), _lib.ptr(ii), _lib.ptr(jj), _lib.ptr(self.slots),
-                    pool.layout, _ptr_array(pool.levels), num_levels, N, 128, ht, wd, _lib.stream_ptr())
-            _lib.check(rc, "corr_pool_build")
-            return self
-        levels = [torch.empty((N, ht, wd, ht >> i, wd >> i), dtype=torch.float16, device=dev)
-                  for i in range(num_levels)]
+        if pool is None:
+            pool = CorrPool(N, self.ht, self.wd, self.num_levels, device=dev)
+        elif (pool.ht, pool.wd, pool.num_levels) != (self.ht, self.wd, self.num_levels):
+            raise RuntimeError("CorrBlock.from_video: pool shape mismatch")
+        self.pool = pool
+        self._slots_host = pool.alloc(N)
+        self.slots = pool.slot_table(self._slots_host)
         with torch.cuda.device(dev):
-            rc = _lib.load().goslam_corr_build_indexed(
-                _lib.ptr(fmaps_kmajor), F, int(rig), _lib.ptr(ii), _lib.ptr(jj), _ptr_array(levels),
-                num_levels, N, 128, ht, wd, _lib.stream_ptr())
-        _lib.check(rc, "corr_build_indexed")
-        self.corr_pyramid = levels
-        return self
+            rc = _lib.load().goslam_corr_pool_build(
+                _lib.ptr(fmaps_kmajor), int(fmaps_kmajor.shape[0]), int(rig), _lib.ptr(ii), _lib.ptr(jj),
+                _lib.ptr(self.slots), _ptr_array(pool.levels), self.num_levels, N, 128, self.ht, self.wd,
+                _lib.stream_ptr())
+        _lib.check(rc, "corr_pool_build")
 
     def __call__(self, coords):
         batch, num, ht, wd, _ = coords.shape
         N = batch * num
         if self.pool is not None:
             return self._call_pooled(coords, batch, num, ht, wd)
-        vol0 = self.corr_pyramid[0]
+        vol0 = self._levels[0]
         rd = 2 * self.radius + 1
         coords = coords.reshape(N, ht, wd, 2).contiguous().float()
         out = torch.empty((batch, num, self.num_levels * rd * rd, ht, wd), dtype=vol0.dtype,
                           device=vol0.device)
-        pyr = [p.contiguous() for p in self.corr_pyramid]
+        pyr = [p.contiguous() for p in self._levels]
         with torch.cuda.device(vol0.device):
             rc = _lib.load().goslam_corr_pyramid_lookup(
                 _ptr_array(pyr), 1 if vol0.dtype == torch.float16 else 0, self.num_levels,
@@ -212,39 +206,50 @@ class CorrBlock:
         with torch.cuda.device(dev):
             rc = _lib.load().goslam_corr_pool_lookup(
                 _ptr_array(pool.levels), 1, self.num_levels, _lib.ptr(self.slots), pool.capacity,
-                pool.layout, _lib.ptr(coords), _lib.ptr(out), N, ht, wd, pool.ht, pool.wd, int(self.radius),
+                pool.TILED, _lib.ptr(coords), _lib.ptr(out), N, ht, wd, pool.ht, pool.wd, int(self.radius),
                 _lib.stream_ptr())
         _lib.check(rc, "corr_pool_lookup")
         return out
 
     def cat(self, other):
-        if self.pool is not None:
+        if self.pool is None:
+            for i in range(self.num_levels):
+                self._levels[i] = torch.cat([self._levels[i], other.corr_pyramid[i]], dim=0)
+            return self
+        if other.pool is self.pool:
             # O(edges): join the slot tables; `other` gives up its slots
-            if other.pool is not self.pool:
-                raise RuntimeError("CorrBlock.cat: blocks live in different pools")
             self._slots_host = self._slots_host + other._slots_host
             self.slots = torch.cat([self.slots, other.slots])
             other._slots_host, other.slots = [], other.slots[:0]
             return self
-        for i in range(self.num_levels):
-            self.corr_pyramid[i] = torch.cat([self.corr_pyramid[i], other.corr_pyramid[i]], dim=0)
+        if other.pool is None:
+            raise RuntimeError("CorrBlock.cat: a pooled block cannot take the edges of a row-major one")
+        # blocks in different pools (e.g. two CorrBlock(f1, f2)): both copied into a new private pool, the
+        # copy the reference's torch.cat makes
+        n = len(self._slots_host) + len(other._slots_host)
+        pool = CorrPool(n, self.ht, self.wd, self.num_levels, device=self.pool.levels[0].device)
+        for i, lvl in enumerate(pool.levels):
+            torch.cat([self.pool.levels[i][self.slots.long()], other.pool.levels[i][other.slots.long()]], out=lvl)
+        self.free()
+        self.pool, self._slots_host = pool, pool.alloc(n)
+        self.slots = pool.slot_table(self._slots_host)
         return self
 
     def __getitem__(self, index):
-        if self.pool is not None:
-            # O(edges): keep the selected slot ids, hand the others back to the pool.  Any index
-            # form torch accepts on dim 0 works (FactorGraph passes boolean masks).
-            ids = torch.arange(len(self._slots_host))[index.cpu() if torch.is_tensor(index) else index]
-            keep = [int(i) for i in ids.reshape(-1).tolist()]
-            kept = set(keep)
-            if len(kept) != len(keep):
-                raise RuntimeError("CorrBlock[index]: a pooled block cannot hold one slot twice")
-            self.pool.release(s for i, s in enumerate(self._slots_host) if i not in kept)
-            self._slots_host = [self._slots_host[i] for i in keep]
-            self.slots = self.pool.slot_table(self._slots_host)
+        if self.pool is None:
+            for i in range(self.num_levels):
+                self._levels[i] = self._levels[i][index]
             return self
-        for i in range(self.num_levels):
-            self.corr_pyramid[i] = self.corr_pyramid[i][index]
+        # O(edges): keep the selected slot ids, hand the others back to the pool.  Any index
+        # form torch accepts on dim 0 works (FactorGraph passes boolean masks).
+        ids = torch.arange(len(self._slots_host))[index.cpu() if torch.is_tensor(index) else index]
+        keep = [int(i) for i in ids.reshape(-1).tolist()]
+        kept = set(keep)
+        if len(kept) != len(keep):
+            raise RuntimeError("CorrBlock[index]: a pooled block cannot hold one slot twice")
+        self.pool.release(s for i, s in enumerate(self._slots_host) if i not in kept)
+        self._slots_host = [self._slots_host[i] for i in keep]
+        self.slots = self.pool.slot_table(self._slots_host)
         return self
 
     def free(self):
@@ -260,11 +265,14 @@ class CorrBlock:
             pass
 
     def gather_pyramid(self):
-        """materialise [N,h,w,h>>i,w>>i] per level (tests / code that reads .corr_pyramid)."""
+        """[N,h,w,h>>i,w>>i] per level: a de-tiled copy for a pooled block (tests / the smoke entry), the
+        block's own levels otherwise."""
         if self.pool is None:
-            return self.corr_pyramid
+            return self._levels
         idx = self.slots.long()
         return [self.pool.level_rowmajor(i, idx) for i in range(self.num_levels)]
+
+    corr_pyramid = property(gather_pyramid)
 
     @staticmethod
     def corr(fmap1, fmap2):

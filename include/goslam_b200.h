@@ -63,26 +63,21 @@ int goslam_corr_pyramid_lookup(const void* const* pyramid, int dtype, int num_le
  * Correlation volume — all-pairs build + 2x2 average-pool pyramid.
  * Replaces CorrBlock.__init__/CorrBlock.corr (src/modules/corr.py:25-41,67-76):
  *   corr[n] = (fmap1[n]/4)^T (fmap2[n]/4)  -> level0 [N,h,w,h,w]; level i+1 = avg_pool2d(level i,2,2).
- *   fmap1,fmap2 [N,D,h,w] f16 (channel-major, as DepthVideo.fmaps stores them),
- *   levels[L] output pointers, f16, level i dims [N,h,w,h>>i,w>>i].
- * impl: 0 = auto, 1 = wgmma/TMA tensor-core kernel, 2 = SIMT reference kernel.
- * workspace: goslam_corr_build_workspace_bytes(N,D,h,w) bytes (K-major staging). */
-size_t goslam_corr_build_workspace_bytes(int N, int D, int h, int w);
-int goslam_corr_build(const void* fmap1, const void* fmap2, void* const* levels,
-                      int num_levels, int N, int D, int h, int w, int impl,
-                      void* workspace, size_t workspace_bytes, void* stream);
+ * CUDA-core build in the reference's row-major layout:
+ *   fmap1,fmap2 [N,D,h,w] (channel-major, as DepthVideo.fmaps stores them), dtype GOSLAM_F16 | GOSLAM_F32;
+ *   levels[L] output pointers of the same dtype, level i dims [N,h,w,h>>i,w>>i].
+ * The tensor-core build is goslam_corr_pool_build below. */
+int goslam_corr_build(const void* fmap1, const void* fmap2, int dtype, void* const* levels,
+                      int num_levels, int N, int D, int h, int w, void* stream);
 /* Video-level form of FactorGraph.add_factors' correlation build (src/factor_graph.py:106-114):
  * the per-frame feature maps are kept K-major AND PRE-SCALED BY 1/4 in half — the reference's
  * `fmap / 4.0` (src/modules/corr.py:71-72) — as [F = buffer*rig, h*w, D] f16, converted ONCE when a
  * keyframe is inserted by goslam_fmaps_to_kmajor from DepthVideo.fmaps' [F, D, h, w], and the
  * kernel indexes them per edge on the device: slot1 = rig*ii[e], slot2 = rig*jj[e] + (ii[e]==jj[e])
- * — no gathered [N,D,h,w] copies, no per-edge re-layout.  Tensor-core kernel only (D == 128). */
+ * — no gathered [N,D,h,w] copies, no per-edge re-layout.  Tensor-core kernel only (D == 128, w <= 128). */
 int goslam_fmaps_to_kmajor(const void* fmaps, void* out, int F, int D, int h, int w, void* stream);
-int goslam_corr_build_indexed(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
-                              const int64_t* jj, void* const* levels, int num_levels, int N, int D,
-                              int h, int w, void* stream);
 
-/* Slot-pool variants: the edge dimension of the volume is a POOL of `capacity` slots that the
+/* Slot-pool build and lookup: the edge dimension of the volume is a POOL of `capacity` slots that the
  * factor graph allocates once; edge e of a block lives in slot slots[e] (int32, device).  Makes
  * CorrBlock.cat / CorrBlock.__getitem__ (src/modules/corr.py:55-65, hit on every add_factors /
  * rm_factors, src/factor_graph.py:114,149) an edit of the slot table instead of a copy of the
@@ -92,23 +87,23 @@ int goslam_corr_build_indexed(const void* fmaps_kmajor, int F, int rig, const in
  * layout: GOSLAM_LAYOUT_ROWMAJOR = the reference's [slot,h,w,h>>i,w>>i];
  *         GOSLAM_LAYOUT_TILED    = levels 0 and 1 stored as 4x4-element (32-byte = one DRAM sector)
  *         tiles, tile-row-major inside each source pixel's plane, planes padded with zeros to whole
- *         tiles; levels 2 and 3 row-major.  Nothing in the reference outside CorrBlock reads the
- *         pyramid, so its layout is private to build + lookup: the tiled form turns the build's
- *         per-thread output into one 128-byte run and cuts the sectors an 8x8 lookup window touches
- *         from ~11.5 to ~7.6.  goslam_corr_level_plane_elems gives the per-source-pixel plane size
- *         (f16 elements) of a level: buffer i holds capacity * h*w * plane_elems(i) elements. */
+ *         tiles; levels 2 and 3 as one padded piece per 8-row band of level 0.  Nothing in the
+ *         reference outside CorrBlock reads the pyramid, so its layout is private to build + lookup:
+ *         the tiled form turns the build's per-thread output into one 128-byte run and cuts the sectors
+ *         an 8x8 lookup window touches from ~11.5 to ~7.6.  goslam_corr_level_plane_elems gives the
+ *         per-source-pixel plane size (f16 elements) of a level: buffer i holds capacity * h*w *
+ *         plane_elems(i) elements.
+ * goslam_corr_pool_build always writes the tiled layout; goslam_corr_pool_lookup reads either (the
+ * row-major form serves caller-owned volumes and goslam_corr_build's output, f16 or f32). */
 #define GOSLAM_LAYOUT_ROWMAJOR 0
 #define GOSLAM_LAYOUT_TILED 1
 size_t goslam_corr_level_plane_elems(int level, int layout, int h, int w);
 int goslam_corr_pool_build(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
-                           const int64_t* jj, const int* slots, int layout, void* const* levels,
+                           const int64_t* jj, const int* slots, void* const* levels,
                            int num_levels, int N, int D, int h, int w, void* stream);
 int goslam_corr_pool_lookup(const void* const* pyramid, int dtype, int num_levels, const int* slots,
                             int capacity, int layout, const float* coords_hw2, void* out, int N,
                             int h1, int w1, int h2, int w2, int radius, void* stream);
-/* fp32 variant used by the CPU-shaped config (fmaps f32, volume f32); SIMT only. */
-int goslam_corr_build_f32(const float* fmap1, const float* fmap2, float* const* levels,
-                          int num_levels, int N, int D, int h, int w, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * On-the-fly windowed correlation (no volume).

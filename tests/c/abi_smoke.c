@@ -26,6 +26,8 @@ int main(void) {
   /* argument validation happens before any CUDA call */
   if (goslam_corr_index_forward(NULL, GOSLAM_F16, NULL, NULL, -1, 1, 1, 1, 1, 3, NULL) != GOSLAM_EINVAL) { printf("einval\n"); ++fails; }
   if (goslam_corr_index_backward() != GOSLAM_EUNSUPPORTED) { printf("unsupported\n"); ++fails; }
+  if (goslam_corr_build(NULL, NULL, GOSLAM_F16, NULL, 4, 1, 128, 4, 80, NULL) != GOSLAM_EINVAL) { printf("corr_build einval\n"); ++fails; }
+  if (goslam_corr_pool_build(NULL, 8, 1, NULL, NULL, NULL, NULL, 4, 1, 128, 40, 160, NULL) != GOSLAM_EINVAL) { printf("pool_build einval\n"); ++fails; }
   printf(fails ? "FAILED %d\n" : "abi smoke ok\n", fails);
   return fails;
 }

@@ -14,7 +14,7 @@ def test_corr_build_tc_kernel_uses_no_local_memory():
     out = subprocess.run(["cuobjdump", "-res-usage", _lib.lib_path()], capture_output=True, text=True).stdout
     lines = out.splitlines()
     idx = [i for i, l in enumerate(lines) if "Function" in l and "corr_build_tc_kernel" in l]
-    assert idx, "corr_build_tc_kernel not found in the library"
+    assert len(idx) == 1, "expected one corr_build_tc_kernel in the library, found %d" % len(idx)
     usage = lines[idx[0] + 1]
     assert re.search(r"\bSTACK:0\b", usage), usage
     assert re.search(r"\bLOCAL:0\b", usage), usage

@@ -97,19 +97,47 @@ def test_corr_block_build_and_lookup(dtype, hw):
         np.testing.assert_allclose(got, want, rtol=2e-7, atol=1e-7)
 
 
+def _simt_pyramid(f1, f2, num_levels=4):
+    """goslam_corr_build, the CUDA-core row-major build, called directly on half feature maps [N, D, h, w]."""
+    import ctypes
+    from goslam_b200 import _lib
+    N, D, h, w = f1.shape
+    levels = [torch.empty((N, h, w, h >> i, w >> i), dtype=torch.float16, device=f1.device) for i in range(num_levels)]
+    ptrs = (ctypes.c_void_p * num_levels)(*[t.data_ptr() for t in levels])
+    rc = _lib.load().goslam_corr_build(_lib.ptr(f1), _lib.ptr(f2), 1, ptrs, num_levels, N, D, h, w, _lib.stream_ptr())
+    _lib.check(rc, "corr_build")
+    return levels
+
+
+def _rowmajor_lookup(pyramid, coords):
+    """goslam_corr_pyramid_lookup on row-major f16 levels [N, h, w, h>>i, w>>i]; coords [1, N, h, w, 2]."""
+    import ctypes
+    from goslam_b200 import _lib
+    N, h, w = pyramid[0].shape[:3]
+    L = len(pyramid)
+    out = torch.empty((1, N, L * 49, h, w), dtype=torch.float16, device=coords.device)
+    c = coords.reshape(N, h, w, 2).float().contiguous()
+    ptrs = (ctypes.c_void_p * L)(*[t.data_ptr() for t in pyramid])
+    rc = _lib.load().goslam_corr_pyramid_lookup(ptrs, 1, L, _lib.ptr(c), _lib.ptr(out), N, h, w, h, w, 3,
+                                                _lib.stream_ptr())
+    _lib.check(rc, "corr_pyramid_lookup")
+    return out
+
+
 @pytest.mark.parametrize("hw", [(40, 80), (30, 40), (12, 20)])
-def test_corr_build_tcgen05_matches_simt(hw):
-    """the tensor-core kernel (impl=1) and its CUDA-core twin (impl=2) share one numerics
-    contract; they may differ only where fp32 summation order flips a half rounding."""
+def test_corr_build_tc_matches_simt(hw):
+    """the tensor-core kernel (CorrBlock on half inputs) and its CUDA-core twin (goslam_corr_build) share
+    one numerics contract; they may differ only where fp32 summation order flips a half rounding."""
     from goslam_b200.modules import CorrBlock
     h, w = hw
     g = torch.Generator().manual_seed(4)
     f1 = torch.randn(1, 3, 128, h, w, generator=g).half().to(dev())
     f2 = torch.randn(1, 3, 128, h, w, generator=g).half().to(dev())
-    a = CorrBlock(f1, f2, impl=1)
-    b = CorrBlock(f1, f2, impl=2)
+    a = CorrBlock(f1, f2)
+    assert a.pool is not None
+    b = _simt_pyramid(f1[0], f2[0])
     for i in range(4):
-        x, y = a.corr_pyramid[i].float(), b.corr_pyramid[i].float()
+        x, y = a.corr_pyramid[i].float(), b[i].float()
         assert x.shape == y.shape
         assert torch.isfinite(x).all()
         assert (x - y).abs().max().item() <= 2e-3 * max(1.0, y.abs().max().item())
@@ -141,19 +169,18 @@ def test_corr_block_from_video_matches_gathered_build():
             assert torch.equal(x, y)
 
 
-@pytest.mark.parametrize("layout", ["tiled", "rowmajor"])
-@pytest.mark.parametrize("hw", [(24, 32), (30, 40), (22, 26)])
-def test_corr_pool_add_remove_matches_cat_and_mask(layout, hw):
+@pytest.mark.parametrize("hw", [(24, 32), (30, 40), (22, 26), (8, 16), (37, 45), (20, 128)])
+def test_corr_pool_add_remove_matches_cat_and_mask(hw):
     """FactorGraph's add_factors / rm_factors sequence (src/factor_graph.py:114,149) on a slot pool:
-    cat() and [mask] edit the slot table only, and the pooled lookup equals the lookup on a
-    pyramid that was really concatenated / masked, bit for bit."""
+    cat() and [mask] edit the slot table only, and the pooled pyramid and lookup equal, bit for bit, the
+    reference's torch.cat / mask of the one-block pyramids and the row-major lookup on that."""
     from goslam_b200.modules import CorrBlock
     from goslam_b200.modules.corr import CorrPool, fmaps_to_kmajor
     g = torch.Generator().manual_seed(16)
     h, w = hw
     fmaps = torch.randn(6, 1, 128, h, w, generator=g).half().to(dev())
     km = fmaps_to_kmajor(fmaps)
-    pool = CorrPool(10, h, w, device=dev(), layout=layout)
+    pool = CorrPool(10, h, w, device=dev())
     ptrs = [lvl.data_ptr() for lvl in pool.levels]
 
     def edges(pairs):
@@ -172,29 +199,33 @@ def test_corr_pool_add_remove_matches_cat_and_mask(layout, hw):
     i1, j1 = edges([(0, 1), (1, 0), (1, 2), (2, 1)])
     i2, j2 = edges([(2, 3), (3, 2), (0, 3)])
     i3, j3 = edges([(4, 5), (5, 4), (3, 5), (5, 3), (4, 2)])
-    plain = CorrBlock.from_video(km, i1, j1, h, w)
+    def one_block(i, j):
+        return CorrBlock.from_video(km, i, j, h, w).gather_pyramid()
+
+    def check(plain, pooled, n):
+        for x, y in zip(plain, pooled.gather_pyramid()):
+            assert torch.equal(x, y)
+        c = coords_for(n)
+        assert torch.equal(_rowmajor_lookup(plain, c), pooled(c))
+
+    plain = one_block(i1, j1)                                # the reference's row-major pyramid, edited by copies
     pooled = CorrBlock.from_video(km, i1, j1, h, w, pool=pool)
     assert pool.free_slots == 6
     # add
-    plain = plain.cat(CorrBlock.from_video(km, i2, j2, h, w))
+    plain = [torch.cat([x, y]) for x, y in zip(plain, one_block(i2, j2))]
     pooled = pooled.cat(CorrBlock.from_video(km, i2, j2, h, w, pool=pool))
     assert pool.free_slots == 3 and len(pooled._slots_host) == 7
-    c = coords_for(7)
-    assert torch.equal(plain(c), pooled(c))
+    check(plain, pooled, 7)
     # remove (boolean keep-mask, as rm_factors passes ~mask)
     keep = torch.tensor([True, False, True, True, False, True, False], device=dev())
-    plain, pooled = plain[keep], pooled[keep]
+    plain, pooled = [x[keep] for x in plain], pooled[keep]
     assert pool.free_slots == 6
-    c = coords_for(4)
-    assert torch.equal(plain(c), pooled(c))
+    check(plain, pooled, 4)
     # add again: freed slots are reused, nothing was reallocated or moved
-    plain = plain.cat(CorrBlock.from_video(km, i3, j3, h, w))
+    plain = [torch.cat([x, y]) for x, y in zip(plain, one_block(i3, j3))]
     pooled = pooled.cat(CorrBlock.from_video(km, i3, j3, h, w, pool=pool))
     assert pool.free_slots == 1 and sorted(pooled._slots_host) == sorted(set(pooled._slots_host))
-    c = coords_for(9)
-    assert torch.equal(plain(c), pooled(c))
-    for x, y in zip(plain.corr_pyramid, pooled.gather_pyramid()):
-        assert torch.equal(x, y)
+    check(plain, pooled, 9)
     assert [lvl.data_ptr() for lvl in pool.levels] == ptrs
     with pytest.raises(RuntimeError):
         CorrBlock.from_video(km, i1, j1, h, w, pool=pool)      # 4 edges, 1 free slot

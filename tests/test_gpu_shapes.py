@@ -40,16 +40,16 @@ def _check_pyramid(got_levels, want_levels):
 
 
 @pytest.mark.parametrize("hw", SHAPES)
-def test_tcgen05_build_vs_oracle(hw):
-    """CorrBlock(fmap1, fmap2, impl=1) — the reference-layout tensor-core build — and the fused
-    lookup on it, against the oracle (bit-exact for the half-precision lookup)."""
+def test_corr_block_build_vs_oracle(hw):
+    """CorrBlock(fmap1, fmap2) — the tensor-core build into a private pool — and the fused lookup on
+    it, against the oracle (bit-exact for the half-precision lookup)."""
     from goslam_b200.modules import CorrBlock
     h, w = hw
     N = 2
     g = torch.Generator().manual_seed(100 + h)
     f1 = torch.randn(1, N, 128, h, w, generator=g).half()
     f2 = torch.randn(1, N, 128, h, w, generator=g).half()
-    blk = CorrBlock(f1.to(dev()), f2.to(dev()), impl=1)
+    blk = CorrBlock(f1.to(dev()), f2.to(dev()))
     _check_pyramid(blk.corr_pyramid, corr_oracle.corr_build(f1[0], f2[0], 4))
     coords = _coords(N, h, w, g)
     out = blk(coords.to(dev()))
@@ -57,11 +57,12 @@ def test_tcgen05_build_vs_oracle(hw):
     np.testing.assert_array_equal(out[0].cpu().numpy().astype(np.float32), want.astype(np.float32))
 
 
-@pytest.mark.parametrize("layout", ["tiled", "rowmajor"])
+@pytest.mark.parametrize("num_levels", [4, 1])
 @pytest.mark.parametrize("hw,rig", [((48, 64), 1), ((40, 80), 1), ((30, 40), 1), ((40, 60), 2), ((60, 80), 1)])
-def test_pool_build_and_lookup_vs_oracle(hw, rig, layout):
-    """FactorGraph's path: video-level K-major maps -> pooled (tiled / row-major) tensor-core build ->
-    pooled 4-level lookup; stereo rigs use the right image for self-edges (src/factor_graph.py:108-111)."""
+def test_pool_build_and_lookup_vs_oracle(hw, rig, num_levels):
+    """FactorGraph's path: video-level K-major maps -> pooled tensor-core build -> pooled lookup of every
+    level; stereo rigs use the right image for self-edges (src/factor_graph.py:108-111).  num_levels = 1
+    leaves the stores of levels 1-3 out of the build."""
     from goslam_b200.modules import CorrBlock
     from goslam_b200.modules.corr import CorrPool, fmaps_to_kmajor
     h, w = hw
@@ -75,14 +76,49 @@ def test_pool_build_and_lookup_vs_oracle(hw, rig, layout):
         jj = torch.tensor([1, 0, 2])
     N = ii.numel()
     c = (ii == jj).long() if rig == 2 else torch.zeros_like(ii)
-    want_pyr = corr_oracle.corr_build(fmaps[ii, 0], fmaps[jj, c], 4)
+    want_pyr = corr_oracle.corr_build(fmaps[ii, 0], fmaps[jj, c], num_levels)
     km = fmaps_to_kmajor(fmaps.to(dev()))
-    pool = CorrPool(N + 3, h, w, device=dev(), layout=layout)
+    pool = CorrPool(N + 3, h, w, num_levels, device=dev())
     pool.alloc(2)                                       # edges do not start at slot 0
-    blk = CorrBlock.from_video(km, ii.to(dev()), jj.to(dev()), h, w, rig=rig, pool=pool)
+    blk = CorrBlock.from_video(km, ii.to(dev()), jj.to(dev()), h, w, rig=rig, num_levels=num_levels, pool=pool)
     got_pyr = blk.gather_pyramid()
+    assert len(got_pyr) == num_levels
     _check_pyramid(got_pyr, want_pyr)
     coords = _coords(N, h, w, g)
     out = blk(coords.to(dev()))
     want = corr_oracle.corr_pyramid_lookup([p.cpu().numpy() for p in got_pyr], coords[0].numpy(), 3)
     np.testing.assert_array_equal(out[0].cpu().numpy().astype(np.float32), want.astype(np.float32))
+
+
+@pytest.mark.parametrize("hw", SHAPES)
+def test_corr_level0_vs_oracle(hw):
+    """CorrBlock.corr (level 0 only): the tensor-core build with one level."""
+    from goslam_b200.modules import CorrBlock
+    h, w = hw
+    g = torch.Generator().manual_seed(400 + h)
+    f1 = torch.randn(1, 2, 128, h, w, generator=g).half()
+    f2 = torch.randn(1, 2, 128, h, w, generator=g).half()
+    got = CorrBlock.corr(f1.to(dev()), f2.to(dev()))
+    assert got.shape == (1, 2, h, w, h, w)
+    _check_pyramid([got[0]], corr_oracle.corr_build(f1[0], f2[0], 1))
+
+
+def test_cat_of_two_private_pool_blocks():
+    """the reference's cat for any two blocks: two CorrBlock(f1, f2) live in different private pools, and
+    their cat holds both pyramids, edge order kept, and looks up like one block built from all edges."""
+    from goslam_b200.modules import CorrBlock
+    h, w = 40, 60
+    g = torch.Generator().manual_seed(500)
+    f1 = torch.randn(1, 5, 128, h, w, generator=g).half().to(dev())
+    f2 = torch.randn(1, 5, 128, h, w, generator=g).half().to(dev())
+    a = CorrBlock(f1[:, :2], f2[:, :2])
+    b = CorrBlock(f1[:, 2:], f2[:, 2:])
+    want = [torch.cat([x, y]) for x, y in zip(a.corr_pyramid, b.corr_pyramid)]
+    whole = CorrBlock(f1, f2)
+    ab = a.cat(b)
+    assert ab is a and a.pool is not b.pool and len(a._slots_host) == 5
+    for x, y, z in zip(ab.corr_pyramid, want, whole.corr_pyramid):
+        assert torch.equal(x, y) and torch.equal(x, z)
+    coords = _coords(5, h, w, g).to(dev())
+    assert torch.equal(ab(coords), whole(coords))
+    assert len(b._slots_host) == 3                      # `b` keeps its own edges

@@ -166,11 +166,13 @@ def test_synthetic_graph_matches_reference_neighbourhood_rule():
     assert abs(float(sc["poses"][:, 3:].norm(dim=-1).mean()) - 1.0) < 1e-5
 
 
-def test_corr_pool_slot_bookkeeping():
+def test_tiled_corr_pool_slot_bookkeeping():
     """CorrPool is host-side bookkeeping only: allocation order, release, exhaustion."""
     from goslam_b200.modules.corr import CorrPool
-    pool = CorrPool(5, 8, 8, num_levels=2, device="cpu", layout="rowmajor")
-    assert [tuple(l.shape) for l in pool.levels] == [(5, 64, 64), (5, 64, 16)]
+    pool = CorrPool(5, 8, 8, num_levels=2, device="cpu", layout="tiled")
+    assert [tuple(l.shape) for l in pool.levels] == [(5, 64, 2 * 2 * 16), (5, 64, 1 * 1 * 16)]
+    with pytest.raises(ValueError):
+        CorrPool(5, 8, 8, num_levels=2, device="cpu", layout="rowmajor")      # the build writes the tiled layout only
     # tiled planes are padded to whole 4x4 tiles on levels 0/1 (same formula as the C helper)
     tiled = CorrPool(2, 30, 40, num_levels=4, device="cpu")
     assert tiled.plane_elems == [8 * 10 * 16, 4 * 5 * 16, 4 * 32, 4 * 16]      # 4 bands, 3 x-blocks
