@@ -168,6 +168,17 @@ SIGNATURES = {
                              [c_int] * 3 + [c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
     "goslam_fill_interpolate": (c_int, [c_void_p] * 5 + [c_int, c_int] + [c_void_p] * 3 + [c_int, c_int] +
                                 [c_void_p] * 3),
+    "goslam_mesh_sample_workspace_bytes": (c_size_t, [c_int64]),
+    "goslam_mesh_sample_surface": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
+                                           c_void_p, c_size_t, c_void_p]),
+    "goslam_nn_index_workspace_bytes": (c_size_t, [c_int64]),
+    "goslam_nn_index_build": (c_int, [c_void_p, c_int64, ctypes.c_double, c_void_p, c_size_t, c_void_p]),
+    "goslam_nn_query": (c_int, [c_void_p, c_size_t, c_int64, c_void_p, c_int64, ctypes.c_double, c_void_p, c_void_p,
+                                c_void_p]),
+    "goslam_nn_distance_stats": (c_int, [c_void_p, c_int64, ctypes.c_double, c_void_p, c_void_p]),
+    "goslam_icp_workspace_bytes": (c_size_t, [c_int64]),
+    "goslam_icp_point_to_point": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, c_int64, ctypes.c_double, c_void_p, c_int,
+                                          ctypes.c_double, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

@@ -20,6 +20,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "mesh_geom.cuh"
 
 namespace {
 
@@ -315,19 +316,7 @@ __global__ void __launch_bounds__(256) edge_kernel(const double* verts, long lon
     efaces[3 * f + j] = (unsigned)f;
   }
   parent[f] = (unsigned)f;
-  double A = 0.0;
-  if (ok) {
-    const double* p0 = verts + 3 * v[0];
-    const double* p1 = verts + 3 * v[1];
-    const double* p2 = verts + 3 * v[2];
-    const double ax = dsub(p1[0], p0[0]), ay = dsub(p1[1], p0[1]), az = dsub(p1[2], p0[2]);
-    const double bx = dsub(p2[0], p0[0]), by = dsub(p2[1], p0[1]), bz = dsub(p2[2], p0[2]);
-    const double cx = dsub(dmul(ay, bz), dmul(az, by));
-    const double cy = dsub(dmul(az, bx), dmul(ax, bz));
-    const double cz = dsub(dmul(ax, by), dmul(ay, bx));
-    A = dmul(0.5, __dsqrt_rn(dadd(dadd(dmul(cx, cx), dmul(cy, cy)), dmul(cz, cz))));
-  }
-  area[f] = A;
+  area[f] = ok ? gs_face_area(verts + 3 * v[0], verts + 3 * v[1], verts + 3 * v[2]) : 0.0;
 }
 
 __device__ __forceinline__ unsigned find_root(const unsigned* parent, unsigned x) {

@@ -4,12 +4,20 @@ and the face-mask culls between them, in csrc/mesh_view.cu and csrc/mesh.cu.
 
     Mesher.cull_mesh = goslam_b200.mesher.cull_mesh      # drop-in method; `import pyrender` can go
 
+The evaluation step of Mesher.__call__(the_end=True) (align_mesh, eval_mesh, src/mesher.py:339-421) runs on the device
+too, in csrc/mesh_eval.cu: surface sampling, exact nearest-neighbour search on a uniform grid and point-to-point ICP.
+
+    import src.mesher as m, goslam_b200.mesher as gm
+    m.align_mesh, m.eval_mesh = gm.align_mesh, gm.eval_mesh
+
 Tensor-level functions take CUDA tensors: vertices [V,3] f64, faces [F,3] i64, colours [V,C] (any dtype) or None.  Every
 cull keeps faces and vertices in their input order (update_faces + remove_unreferenced_vertices) and carries the colours
 of the kept vertices along.
 """
 import ctypes
+import math
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -240,3 +248,194 @@ def cull_mesh(self, mesh, estimate_c2w_list, bound, mesh_out_file):
     cull.export(mesh_out_file)
     forecast.export(mesh_out_file.replace(".ply", "_forecast.ply"))
     return cull, forecast
+
+
+# ---- reconstruction evaluation (align_mesh / eval_mesh) -----------------------------------------------------------
+def _points(x, what):
+    x = torch.as_tensor(x)
+    if not x.is_cuda:
+        raise RuntimeError("%s: CUDA tensors required (no CPU fallback)" % what)
+    x = x.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    if x.shape[0] == 0:
+        raise ValueError("%s: no points" % what)
+    return x
+
+
+class NNIndex:
+    """A uniform-grid index over points [n,3] (CUDA, f64), built once and queried any number of times.  Cells are at
+    least `min_cell` wide (pass the radius of radius queries); results do not depend on it."""
+
+    def __init__(self, points, min_cell=0.0):
+        self.points = _points(points, "NNIndex")
+        n = self.points.shape[0]
+        lib = _lib.load()
+        with torch.cuda.device(self.points.device):
+            nbytes = lib.goslam_nn_index_workspace_bytes(n)
+            if nbytes == 0:
+                raise RuntimeError("NNIndex: cannot index %d points" % n)
+            self.buf = torch.empty(nbytes, dtype=torch.uint8, device=self.points.device)
+            _lib.check(lib.goslam_nn_index_build(_lib.ptr(self.points), n, float(min_cell), _lib.ptr(self.buf), nbytes,
+                                                 _lib.stream_ptr()), "nn_index_build")
+
+    def __len__(self):
+        return self.points.shape[0]
+
+    def query(self, query, max_dist=math.inf):
+        """(dist f64, idx i64) of the nearest indexed point to each query with distance < max_dist (inf / -1 where
+        there is none); the smallest index among equal distances"""
+        q = _points(query, "NNIndex.query") if torch.as_tensor(query).numel() else \
+            torch.empty((0, 3), dtype=torch.float64, device=self.points.device)
+        dist = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
+        idx = torch.empty(q.shape[0], dtype=torch.int64, device=q.device)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib.load().goslam_nn_query(_lib.ptr(self.buf), self.buf.numel(), len(self), _lib.ptr(q),
+                                                   q.shape[0], float(max_dist), _lib.ptr(dist), _lib.ptr(idx),
+                                                   _lib.stream_ptr()), "nn_query")
+        return dist, idx
+
+
+def nearest(query, points, max_dist=math.inf):
+    """(dist f64, idx i64): the nearest of points [M,3] to each of query [N,3] (cKDTree.query; with a finite max_dist
+    only distances < max_dist count, idx -1 where none does).  Exact."""
+    return NNIndex(points, 0.0 if math.isinf(max_dist) else max_dist).query(query, max_dist)
+
+
+def _uniforms(count, generator, dev):
+    """the draws of sample_surface: [count, 3] f64 (face pick, two lengths) from torch's CUDA generator"""
+    return torch.rand((count, 3), dtype=torch.float64, device=dev, generator=generator)
+
+
+def sample_surface_from(verts, faces, uniforms):
+    """trimesh.sample.sample_surface for given uniforms [count, 3] (u, l0, l1): area-weighted face choice
+    (searchsorted side='left' on the fp64 cumulative areas) and trimesh's point rule.  [count, 3] f64."""
+    verts, faces = _mesh_args(verts, faces)
+    if faces.shape[0] == 0 or verts.shape[0] == 0:
+        raise ValueError("sample_surface: the mesh has no faces")
+    u = torch.as_tensor(uniforms).to(verts.device, torch.float64).reshape(-1, 3).contiguous()
+    out = torch.empty((u.shape[0], 3), dtype=torch.float64, device=verts.device)
+    lib = _lib.load()
+    with torch.cuda.device(verts.device):
+        nbytes = lib.goslam_mesh_sample_workspace_bytes(faces.shape[0])
+        if nbytes == 0:
+            raise RuntimeError("sample_surface: cannot size the workspace for %d faces" % faces.shape[0])
+        ws = _workspace(nbytes, verts.device)
+        _lib.check(lib.goslam_mesh_sample_surface(_lib.ptr(verts), verts.shape[0], _lib.ptr(faces), faces.shape[0],
+                                                  _lib.ptr(u), u.shape[0], _lib.ptr(out), None, _lib.ptr(ws), nbytes,
+                                                  _lib.stream_ptr()), "mesh_sample_surface")
+    return out
+
+
+def sample_surface(verts, faces, count, generator=None):
+    """[count, 3] f64 area-weighted samples of the mesh's surface, uniforms from torch.rand on the mesh's device"""
+    verts = torch.as_tensor(verts)
+    if not verts.is_cuda:
+        raise RuntimeError("sample_surface: CUDA tensors required (no CPU fallback)")
+    return sample_surface_from(verts, faces, _uniforms(int(count), generator, verts.device))
+
+
+def icp_point_to_point(src, dst, threshold, init=None, max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6):
+    """Open3D's registration_icp(src, dst, threshold, init, TransformationEstimationPointToPoint()) with its default
+    criteria: (T [4,4] f64 on the host, fitness, inlier_rmse, iterations).  dst is a point tensor or an NNIndex built
+    with min_cell = threshold.  One host synchronisation."""
+    src = _points(src, "icp_point_to_point")
+    index = dst if isinstance(dst, NNIndex) else NNIndex(dst, float(threshold))
+    dev = src.device
+    if index.points.device != dev:
+        raise ValueError("icp_point_to_point: source and target on different devices")
+    T0 = torch.eye(4, dtype=torch.float64) if init is None else torch.as_tensor(np.asarray(init, np.float64))
+    T0 = T0.to(dev, torch.float64).reshape(4, 4).contiguous()
+    out = torch.empty(19, dtype=torch.float64, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        nbytes = lib.goslam_icp_workspace_bytes(src.shape[0])
+        if nbytes == 0:
+            raise RuntimeError("icp_point_to_point: cannot size the workspace for %d points" % src.shape[0])
+        ws = _workspace(nbytes, dev)
+        _lib.check(lib.goslam_icp_point_to_point(_lib.ptr(src), src.shape[0], _lib.ptr(index.buf), index.buf.numel(),
+                                                 len(index), float(threshold), _lib.ptr(T0), int(max_iteration),
+                                                 float(relative_fitness), float(relative_rmse), _lib.ptr(out),
+                                                 _lib.ptr(ws), nbytes, _lib.stream_ptr()), "icp_point_to_point")
+        host = out.cpu()
+    return host[:16].reshape(4, 4).clone(), float(host[16]), float(host[17]), int(host[18])
+
+
+def _ratio(count, n):
+    """np.mean((dist < th).astype(np.float32)) * 100: a float32 mean of exact 0/1 values"""
+    return np.float32(np.float32(count) / np.float32(n)) * np.float32(100)
+
+
+def mesh_metrics(est_pts, gt_pts, dist_th):
+    """eval_mesh's five numbers for two point sets: accuracy / completion (mean nearest distance, cm), their ratios
+    under dist_th (%) and the F-score, with the reference's dtypes (float64 means, float32 ratios).  One host read."""
+    est, gt = _points(est_pts, "mesh_metrics"), _points(gt_pts, "mesh_metrics")
+    stats = torch.empty(4, dtype=torch.float64, device=est.device)
+    lib = _lib.load()
+    with torch.cuda.device(est.device):
+        comp, _ = NNIndex(est).query(gt)
+        _lib.check(lib.goslam_nn_distance_stats(_lib.ptr(comp), comp.numel(), float(dist_th), _lib.ptr(stats[0:2]),
+                                                _lib.stream_ptr()), "nn_distance_stats")
+        acc, _ = NNIndex(gt).query(est)
+        _lib.check(lib.goslam_nn_distance_stats(_lib.ptr(acc), acc.numel(), float(dist_th), _lib.ptr(stats[2:4]),
+                                                _lib.stream_ptr()), "nn_distance_stats")
+        s = stats.tolist()
+    completion = np.float64(s[0]) / gt.shape[0] * 100
+    accuracy = np.float64(s[2]) / est.shape[0] * 100
+    completion_ratio, accuracy_ratio = _ratio(int(s[1]), gt.shape[0]), _ratio(int(s[3]), est.shape[0])
+    with np.errstate(invalid="ignore", divide="ignore"):
+        f_score = (2.0 * accuracy_ratio * completion_ratio) / (accuracy_ratio + completion_ratio)
+    return dict(accuracy=accuracy, completion=completion, accuracy_ratio=accuracy_ratio,
+                completion_ratio=completion_ratio, f_score=f_score)
+
+
+def metrics_message(m):
+    return (f'\n\nMetrics of reconstructed mesh are:\n'
+            f'\tAccuracy: {m["accuracy"]:.2f}cm\n'
+            f'\tCompletion: {m["completion"]:.2f}cm\n'
+            f'\tAccuracy Ratio: {m["accuracy_ratio"]:.2f}%\n'
+            f'\tCompletion Ratio: {m["completion_ratio"]:.2f}%\n'
+            f'\tF-score: {m["f_score"]:.2f}%\n\n')
+
+
+def _mesh_tensors(mesh, dev, what):
+    verts = torch.as_tensor(np.ascontiguousarray(np.asarray(mesh.vertices, np.float64)[:, :3])).to(dev)
+    faces = torch.as_tensor(np.ascontiguousarray(np.asarray(mesh.faces, np.int64).reshape(-1, 3))).to(dev)
+    if verts.shape[0] == 0:
+        raise ValueError("%s: the mesh is empty" % what)
+    return verts, faces
+
+
+@torch.no_grad()
+def align_mesh(est_mesh, gt_mesh, threshold=0.1, trans_init=None, return_transformation=False):
+    """align_mesh (src/mesher.py:339-357): point-to-point ICP of est_mesh's vertices onto gt_mesh's, from trans_init
+    (identity if None), then est_mesh.apply_transform(T).  Returns the aligned mesh (and T, numpy [4,4] f64)."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    src, _ = _mesh_tensors(est_mesh, dev, "align_mesh")
+    dst, _ = _mesh_tensors(gt_mesh, dev, "align_mesh")
+    T, _, _, _ = icp_point_to_point(src, dst, threshold, np.eye(4) if trans_init is None else trans_init)
+    transformation = T.numpy()
+    aligned_mesh = est_mesh.apply_transform(transformation)
+    if return_transformation:
+        return aligned_mesh, transformation
+    return aligned_mesh
+
+
+@torch.no_grad()
+def eval_mesh(est_mesh, gt_mesh, N3d=2e5, dist_th=0.05, out_path=None, metric_2d=False, generator=None):
+    """eval_mesh (src/mesher.py:390-421): N3d area-weighted samples of each mesh (est first, from torch's CUDA
+    generator), nearest distances both ways, the reference's message written to out_path and printed.  Returns the
+    metrics as a dict (the reference returns None).  metric_2d is accepted and ignored, as in the reference."""
+    N3d = int(N3d)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    ev, ef = _mesh_tensors(est_mesh, dev, "eval_mesh")
+    gv, gf = _mesh_tensors(gt_mesh, dev, "eval_mesh")
+    if ef.shape[0] == 0 or gf.shape[0] == 0:
+        raise ValueError("eval_mesh: the mesh has no faces")
+    est_pc = sample_surface_from(ev, ef, _uniforms(N3d, generator, dev))
+    gt_pc = sample_surface_from(gv, gf, _uniforms(N3d, generator, dev))
+    m = mesh_metrics(est_pc, gt_pc, dist_th)
+    msg = metrics_message(m)
+    if out_path is not None:
+        with open(out_path, 'w') as fp:
+            fp.write(msg)
+    print(msg)
+    return {k: float(v) for k, v in m.items()}

@@ -693,6 +693,49 @@ int goslam_fill_interpolate(float* timestamp, float* poses, float* intrinsics, f
                             int M, const float* tt, const float* intr_full, const float* depth, int H, int W,
                             int64_t* t0, int64_t* t1, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Reconstruction evaluation: align_mesh / eval_mesh (src/mesher.py:339-421): surface sampling, exact nearest-neighbour
+ * search and point-to-point ICP.  Device pointers; points [n,3] f64, faces [F,3] int64.  No host synchronisation.
+ *
+ * goslam_mesh_sample_surface — trimesh.sample.sample_surface from caller-drawn uniforms [count,3] (u, l0, l1): face =
+ *   the first f with cum[f] >= u * cum[F-1] (cum = fp64 inclusive scan of the faces' fp64 areas, a face with an index
+ *   outside [0, n_verts) has area 0 and samples NaN), point = ((v1 - v0) l0 + (v2 - v0) l1) + v0 per component after
+ *   (l0, l1) <- (|l0 - 1|, |l1 - 1|) when l0 + l1 > 1, every operation rounded (no FMA).  samples [count,3];
+ *   face_index [count] or NULL.  Workspace: goslam_mesh_sample_workspace_bytes(n_faces); n_faces >= 1.
+ *
+ * goslam_nn_index_build — a uniform grid over points [n_points,3] (1 <= n_points <= 2^28, finite coordinates) built
+ *   into the caller's buffer `index` (goslam_nn_index_workspace_bytes(n_points) bytes), which must stay alive and
+ *   unchanged while it is queried.  Cells are at least min_cell (>= 0) wide; pass the query radius for radius queries.
+ * goslam_nn_query — for each of query [n_query,3] the nearest indexed point with d2 < max_dist^2 (max_dist = +inf: no
+ *   bound), d2 = (dx^2 + dy^2) + dz^2 rounded operation by operation: dist = sqrt(d2) (+inf if none) and idx = its
+ *   point id (-1 if none; the smallest id among equal d2).  Exact: the result does not depend on the grid.  Either
+ *   output may be NULL.
+ * goslam_nn_distance_stats — out[0] = sum of dist [n], out[1] = number of dist < threshold (fixed summation order).
+ *
+ * goslam_icp_point_to_point — Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) of
+ *   source [n_source,3] onto the indexed target: init [4,4] row-major (device, any 4x4; points are divided by w),
+ *   correspondences = nearest target with d2 < threshold^2, update = Umeyama's rotation and translation of the
+ *   correspondences (identity without any), T <- update T, stop after max_iteration updates or when |d fitness| <
+ *   relative_fitness and |d rmse| < relative_rmse.  result [19] (device f64): T [16] row-major, fitness, inlier rmse,
+ *   number of updates.  All max_iteration iterations are enqueued; kernels after convergence return at once.
+ *   Workspace: goslam_icp_workspace_bytes(n_source).
+ * ---------------------------------------------------------------------------------- */
+size_t goslam_mesh_sample_workspace_bytes(int64_t n_faces);
+int goslam_mesh_sample_surface(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces,
+                               const double* uniforms, int64_t count, double* samples, int64_t* face_index,
+                               void* workspace, size_t workspace_bytes, void* stream);
+size_t goslam_nn_index_workspace_bytes(int64_t n_points);
+int goslam_nn_index_build(const double* points, int64_t n_points, double min_cell, void* index, size_t index_bytes,
+                          void* stream);
+int goslam_nn_query(const void* index, size_t index_bytes, int64_t n_points, const double* query, int64_t n_query,
+                    double max_dist, double* dist, int64_t* idx, void* stream);
+int goslam_nn_distance_stats(const double* dist, int64_t n, double threshold, double* out, void* stream);
+size_t goslam_icp_workspace_bytes(int64_t n_source);
+int goslam_icp_point_to_point(const double* source, int64_t n_source, const void* index, size_t index_bytes,
+                              int64_t n_target, double threshold, const double* init, int max_iteration,
+                              double relative_fitness, double relative_rmse, double* result, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
