@@ -179,6 +179,15 @@ SIGNATURES = {
     "goslam_icp_workspace_bytes": (c_size_t, [c_int64]),
     "goslam_icp_point_to_point": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, c_int64, ctypes.c_double, c_void_p, c_int,
                                           ctypes.c_double, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "goslam_mapping_points_workspace_bytes": (c_size_t, [c_int] * 3),
+    "goslam_mapping_points_count": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p, c_void_p]),
+    "goslam_mapping_points_emit": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p, c_int64,
+                                                                          c_void_p]),
+    "goslam_hull_workspace_bytes": (c_size_t, [c_int64]),
+    "goslam_hull_vertices": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "goslam_hull_vertices_emit": (c_int, [c_void_p, c_size_t, c_int64, c_void_p, c_int64, c_void_p]),
+    "goslam_obb_from_hull": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, ctypes.c_double, c_void_p, c_void_p]),
+    "goslam_obb_in_bound": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

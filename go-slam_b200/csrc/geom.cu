@@ -2,6 +2,8 @@
 // frame_distance, projmap, iproj, depth_filter and the DepthVideo.reproject fusion.
 // All are a few flops per 4-byte pixel => HBM/latency bound; one thread per pixel,
 // coalesced along x, relative pose computed once per block into shared memory.
+#include <cub/cub.cuh>
+
 #include "common.cuh"
 #include "se3.cuh"
 
@@ -601,6 +603,52 @@ mv_commit_kernel(const float* __restrict__ poses, const float* __restrict__ disp
   }
 }
 
+// ---------------------------------------------------------------------------------
+// Mapping point selection  (Mesher.update_param_from_mapping, src/mesher.py:256-276): the world points of the
+// keyframes' full-resolution inverse depths with count >= 3 votes (depth_filter, thresh 0.01) and d > 0.01 * the
+// frame's mean, i.e. mask1 of the multiview filter with visible_num = 3.  mv_mean_kernel + mv_vote_kernel count them
+// (MvState::n1); the emit is an ordered CUB select of iproj_point over mask1, [b, h, w] row-major, widened to f64.
+// ---------------------------------------------------------------------------------
+struct MapLayout {
+  size_t mean, mask1, nsel, tmp, total;
+  MapLayout(int T, size_t hw, size_t tmp_bytes) {
+    mean = kMvStateBytes;
+    mask1 = mean + mv_align((size_t)T * sizeof(float));
+    nsel = mask1 + mv_align((size_t)T * hw);
+    tmp = nsel + 256;
+    total = tmp + mv_align(tmp_bytes);
+  }
+};
+
+struct MapPoint3 {
+  double x, y, z;
+};
+
+struct MapPointOp {
+  const float* pw;
+  const float* disps;
+  const float* intr;
+  int hw, wd;
+  __device__ MapPoint3 operator()(long long g) const {
+    const int f = (int)(g / hw), k = (int)(g - (long long)f * hw);
+    float p[3];
+    iproj_point(pw + 7 * (size_t)f, intr[0], intr[1], intr[2], intr[3], (float)(k % wd), (float)(k / wd), disps[g], p);
+    return MapPoint3{(double)p[0], (double)p[1], (double)p[2]};
+  }
+};
+
+using MapIter = cub::TransformInputIterator<MapPoint3, MapPointOp, cub::CountingInputIterator<long long>>;
+
+size_t map_select_tmp(long long n) {
+  size_t t = 0;
+  cub::DeviceSelect::Flagged(nullptr, t, MapIter(cub::CountingInputIterator<long long>(0), MapPointOp{}),
+                             (const unsigned char*)nullptr, (MapPoint3*)nullptr, (long long*)nullptr, n);
+  return std::max<size_t>(t, 1);
+}
+
+constexpr float kMapThresh = 0.01f;          // src/mesher.py:252-253
+constexpr float kMapVisible = 3.0f;
+
 }  // namespace
 
 extern "C" {
@@ -733,6 +781,63 @@ int goslam_mvfilter_commit(const float* poses, const float* disps, const void* w
   mv_commit_kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
       poses, disps, reinterpret_cast<const unsigned char*>(ws + L.fin), reinterpret_cast<const MvState*>(ws), T, n,
       poses_filtered, disps_filtered, mask_filtered, update_priority, filtered_id, bound, status);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+size_t goslam_mapping_points_workspace_bytes(int T, int ht, int wd) {
+  if (T < 1 || T > 65535 || ht <= 0 || wd <= 0 || (size_t)ht * wd > (size_t)INT_MAX / 2) return 0;
+  const size_t hw = (size_t)ht * wd;
+  return MapLayout(T, hw, map_select_tmp((long long)T * (long long)hw)).total;
+}
+
+int goslam_mapping_points_count(const float* poses, const float* poses_world, const float* disps,
+                                const float* intrinsic, int T, int ht, int wd, void* workspace, size_t workspace_bytes,
+                                int64_t* count, void* stream) {
+  if (T < 1 || T > 65535 || ht <= 0 || wd <= 0 || count == nullptr) return GOSLAM_EINVAL;
+  if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
+  const int hw = ht * wd;
+  const MapLayout L(T, (size_t)hw, map_select_tmp((long long)T * hw));
+  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  char* ws = static_cast<char*>(workspace);
+  MvState* st = reinterpret_cast<MvState*>(ws);
+  float* mean = reinterpret_cast<float*>(ws + L.mean);
+  unsigned char* mask1 = reinterpret_cast<unsigned char*>(ws + L.mask1);
+  cudaStream_t s = (cudaStream_t)stream;
+  mv_mean_kernel<<<T, kMvMeanThreads, 0, s>>>(disps, mean, st, T, hw);
+  GS_CHECK_LAUNCH();
+  mv_vote_kernel<<<dim3(gs_cdiv(hw, kMvTile), T), kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, mean,
+                                                                     kMapThresh, kMapVisible, mask1, st, T, ht, wd);
+  GS_CHECK_LAUNCH();
+  if (cudaMemcpyAsync(count, &st->n1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+    GS_CHECK_LAUNCH();
+    return GOSLAM_ELAUNCH;
+  }
+  return GOSLAM_OK;
+}
+
+int goslam_mapping_points_emit(const float* poses_world, const float* disps, const float* intrinsic, int T, int ht,
+                               int wd, void* workspace, size_t workspace_bytes, double* points, int64_t n_points,
+                               void* stream) {
+  if (T < 1 || T > 65535 || ht <= 0 || wd <= 0 || n_points < 0 || (n_points > 0 && points == nullptr))
+    return GOSLAM_EINVAL;
+  if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
+  const int hw = ht * wd;
+  const long long n = (long long)T * hw;
+  if (n_points > n) return GOSLAM_EINVAL;
+  const size_t tmp_bytes = map_select_tmp(n);
+  const MapLayout L(T, (size_t)hw, tmp_bytes);
+  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  if (n_points == 0) return GOSLAM_OK;
+  char* ws = static_cast<char*>(workspace);
+  size_t tb = tmp_bytes;
+  const MapIter it(cub::CountingInputIterator<long long>(0), MapPointOp{poses_world, disps, intrinsic, hw, wd});
+  if (cub::DeviceSelect::Flagged(ws + L.tmp, tb, it, reinterpret_cast<const unsigned char*>(ws + L.mask1),
+                                 reinterpret_cast<MapPoint3*>(points), reinterpret_cast<long long*>(ws + L.nsel), n,
+                                 (cudaStream_t)stream) != cudaSuccess) {
+    GS_CHECK_LAUNCH();
+    return GOSLAM_ELAUNCH;
+  }
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

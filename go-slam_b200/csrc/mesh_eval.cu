@@ -509,34 +509,8 @@ __global__ void __launch_bounds__(kThreads) icp_cov_kernel(const double* work, l
 // which the product reduces to u1 v1^T + u2 v2^T + det(V) (u1 x u2) v3^T, also for rank 2.  Rank < 2 (s2 <= 1e-14 s1):
 // the rotation is not unique and the identity is returned.
 __device__ void umeyama_rotation(const double A[9], double R[9]) {
-  double B[9], V[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-  for (int k = 0; k < 9; ++k) B[k] = A[k];
-  for (int sweep = 0; sweep < 64; ++sweep) {
-    bool rotated = false;
-    for (int pq = 0; pq < 3; ++pq) {
-      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
-      double al = 0.0, be = 0.0, ga = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        al += B[3 * r + p] * B[3 * r + p];
-        be += B[3 * r + q] * B[3 * r + q];
-        ga += B[3 * r + p] * B[3 * r + q];
-      }
-      if (ga == 0.0 || fabs(ga) <= 1e-16 * sqrt(al * be)) continue;
-      rotated = true;
-      const double zeta = (be - al) / (2.0 * ga);
-      const double t = copysign(1.0, zeta) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-      const double c = 1.0 / sqrt(1.0 + t * t), sn = c * t;
-      for (int r = 0; r < 3; ++r) {
-        const double bp = B[3 * r + p], bq = B[3 * r + q];
-        B[3 * r + p] = c * bp - sn * bq;
-        B[3 * r + q] = sn * bp + c * bq;
-        const double vp = V[3 * r + p], vq = V[3 * r + q];
-        V[3 * r + p] = c * vp - sn * vq;
-        V[3 * r + q] = sn * vp + c * vq;
-      }
-    }
-    if (!rotated) break;
-  }
+  double B[9], V[9];
+  gs_jacobi3(A, B, V);
   double sv[3];
   int ord[3] = {0, 1, 2};
   for (int j = 0; j < 3; ++j) sv[j] = sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);

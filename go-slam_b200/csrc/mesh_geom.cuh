@@ -1,4 +1,5 @@
-// mesh_geom.cuh — per-face geometry shared by the mesh kernels (component filter, surface sampling).
+// mesh_geom.cuh — geometry shared by the mesh kernels: per-face areas (component filter, surface sampling) and the
+// one-thread 3x3 Jacobi SVD (ICP's Umeyama update, the oriented box's principal axes).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -11,4 +12,40 @@ __device__ __forceinline__ double gs_face_area(const double* p0, const double* p
   const double cy = __dsub_rn(__dmul_rn(az, bx), __dmul_rn(ax, bz));
   const double cz = __dsub_rn(__dmul_rn(ax, by), __dmul_rn(ay, bx));
   return __dmul_rn(0.5, __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz))));
+}
+
+// One-sided Jacobi SVD of the 3x3 row-major A: B = A V with mutually orthogonal columns, V orthogonal (row-major).  The
+// singular values are the column norms of B; for a symmetric positive semi-definite A they are its eigenvalues and the
+// columns of V its eigenvectors.  One thread, at most 64 sweeps.
+__device__ __forceinline__ void gs_jacobi3(const double A[9], double B[9], double V[9]) {
+  for (int k = 0; k < 9; ++k) {
+    B[k] = A[k];
+    V[k] = (k % 4 == 0) ? 1.0 : 0.0;
+  }
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    bool rotated = false;
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
+      double al = 0.0, be = 0.0, ga = 0.0;
+      for (int r = 0; r < 3; ++r) {
+        al += B[3 * r + p] * B[3 * r + p];
+        be += B[3 * r + q] * B[3 * r + q];
+        ga += B[3 * r + p] * B[3 * r + q];
+      }
+      if (ga == 0.0 || fabs(ga) <= 1e-16 * sqrt(al * be)) continue;
+      rotated = true;
+      const double zeta = (be - al) / (2.0 * ga);
+      const double t = copysign(1.0, zeta) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+      const double c = 1.0 / sqrt(1.0 + t * t), sn = c * t;
+      for (int r = 0; r < 3; ++r) {
+        const double bp = B[3 * r + p], bq = B[3 * r + q];
+        B[3 * r + p] = c * bp - sn * bq;
+        B[3 * r + q] = sn * bp + c * bq;
+        const double vp = V[3 * r + p], vq = V[3 * r + q];
+        V[3 * r + p] = c * vp - sn * vq;
+        V[3 * r + q] = sn * vp + c * vq;
+      }
+    }
+    if (!rotated) break;
+  }
 }

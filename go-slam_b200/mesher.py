@@ -222,6 +222,8 @@ def cull_mesh(self, mesh, estimate_c2w_list, bound, mesh_out_file):
             if isinstance(bound, np.ndarray):
                 eps = 0.001
                 verts, faces, colors = _keep_box(verts, faces, bound[:, 0] - eps, bound[:, 1] + eps, colors)
+            elif isinstance(bound, OrientedBoundingBox):
+                verts, faces, colors = keep_faces(verts, faces, colors=colors, vert_mask=bound.in_bound(verts))
             else:
                 inb = bound.in_bound(_host(verts)[0])
                 verts, faces, colors = keep_faces(verts, faces, colors=colors, vert_mask=torch.as_tensor(np.asarray(inb)))
@@ -439,3 +441,198 @@ def eval_mesh(est_mesh, gt_mesh, N3d=2e5, dist_th=0.05, out_path=None, metric_2d
             fp.write(msg)
     print(msg)
     return {k: float(v) for k, v in m.items()}
+
+
+# ---- the scene bound (update_param_from_mapping, OrientedBoundingBox) ---------------------------------------------
+_HULL_STATUS = {1: "fewer than four affinely independent points", 2: "the hull has too many facets",
+                3: "a coordinate is not finite", 4: "inconsistent facet graph"}
+MAPPING_EXTEND = 0.1            # src/mesher.py:279
+
+
+def _hull_run(points, what):
+    """goslam_hull_vertices on points (CUDA, any float dtype, [n,3]): (points f64, workspace, info [4] on the device)"""
+    pts = _points(points, what)
+    n = pts.shape[0]
+    lib = _lib.load()
+    nbytes = lib.goslam_hull_workspace_bytes(n)
+    if nbytes == 0:
+        raise ValueError("%s: %d points (at most 2^28)" % (what, n))
+    ws = _workspace(nbytes, pts.device)
+    info = torch.empty(4, dtype=torch.int64, device=pts.device)
+    _lib.check(lib.goslam_hull_vertices(_lib.ptr(pts), n, _lib.ptr(ws), nbytes, _lib.ptr(info), _lib.stream_ptr()),
+               "hull_vertices")
+    return pts, ws, nbytes, info
+
+
+def _hull_info(info, what):
+    status, count, survivors, winners = info.tolist()
+    if status:
+        err = ValueError if status in (1, 3) else RuntimeError
+        raise err("%s: %s" % (what, _HULL_STATUS.get(status, "status %d" % status)))
+    return count
+
+
+def hull_vertices(points):
+    """sorted int64 ids of the convex-hull vertices of points [n,3] (CUDA): the exact extreme points, so a point on a
+    hull face or edge is not one and of equal points only the lowest index can be.  ValueError when the points span
+    less than three dimensions.  One host read."""
+    with torch.cuda.device(torch.as_tensor(points).device):
+        pts, ws, nbytes, info = _hull_run(points, "hull_vertices")
+        count = _hull_info(info, "hull_vertices")
+        out = torch.empty(count, dtype=torch.int64, device=pts.device)
+        _lib.check(_lib.load().goslam_hull_vertices_emit(_lib.ptr(ws), nbytes, pts.shape[0], _lib.ptr(out), count,
+                                                         _lib.stream_ptr()), "hull_vertices_emit")
+    return out
+
+
+def _oriented_box(points, extend):
+    """box [15] f64 on the device (center, R row-major, extent + extend).  One host read (the hull's status)."""
+    with torch.cuda.device(torch.as_tensor(points).device):
+        pts, ws, nbytes, info = _hull_run(points, "oriented_box")
+        box = torch.empty(15, dtype=torch.float64, device=pts.device)
+        _lib.check(_lib.load().goslam_obb_from_hull(_lib.ptr(pts), pts.shape[0], _lib.ptr(ws), nbytes, float(extend),
+                                                    _lib.ptr(box), _lib.stream_ptr()), "obb_from_hull")
+        _hull_info(info, "oriented_box")
+    return box
+
+
+def oriented_box(points, extend=0.0):
+    """Open3D 0.13's OrientedBoundingBox.create_from_points(points) as (center [3], R [3,3], extent [3]) f64 on the
+    device, extent + extend as in compute_from_pointcloud.  R's columns are the hull vertices' principal axes by
+    descending variance; columns 0 and 1 have their largest-magnitude component positive, column 2 = column 0 x 1."""
+    box = _oriented_box(points, extend)
+    return box[0:3], box[3:12].view(3, 3), box[12:15]
+
+
+def in_oriented_box(points, center, R, extent):
+    """bool [n]: Open3D's get_point_indices_within_bounding_box rule (six plane tests on the box corners) for points
+    [n,3] (CUDA).  The box is read on the device."""
+    pts = torch.as_tensor(points)
+    if not pts.is_cuda:
+        raise RuntimeError("in_oriented_box: CUDA tensors required (no CPU fallback)")
+    pts = pts.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    dev = pts.device
+    box = torch.cat([torch.as_tensor(t).to(dev, torch.float64).reshape(-1) for t in (center, R, extent)])
+    if box.numel() != 15:
+        raise ValueError("in_oriented_box: center [3], R [3,3] and extent [3] expected")
+    mask = torch.empty(pts.shape[0], dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().goslam_obb_in_bound(_lib.ptr(box), _lib.ptr(pts), pts.shape[0], _lib.ptr(mask),
+                                                   _lib.stream_ptr()), "obb_in_bound")
+    return mask.bool()
+
+
+class OrientedBoundingBox(torch.nn.Module):
+    """src/oriented_bounding_box.py with the hull, the box and the in-bound test on the device.  Buffers center [3],
+    R [3,3] and extent [3] are float64, as in the reference."""
+
+    def __init__(self):
+        super().__init__()
+        self.register_buffer('center', torch.zeros(3,).double())
+        self.register_buffer('R', torch.zeros(3, 3).double())
+        self.register_buffer('extent', torch.zeros(3,).double())
+
+    def _init(self, center, R, extent):
+        device = self.center.device
+        self.center[:] = torch.as_tensor(center).to(device).double()
+        self.R[:] = torch.as_tensor(R).to(device).double()
+        self.extent[:] = torch.as_tensor(extent).to(device).double()
+
+    def _clone(self, aabb):
+        self._init(aabb.center, aabb.R, aabb.extent)
+
+    def _device(self):
+        dev = self.center.device
+        return dev if dev.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+
+    def compute_from_pointcloud(self, pointcloud, extend=0.0):
+        """the oriented box of pointcloud (ndarray or CUDA tensor [n,3]), extent + extend"""
+        pts = torch.as_tensor(np.asarray(pointcloud) if isinstance(pointcloud, np.ndarray) else pointcloud)
+        if not pts.is_cuda:
+            pts = pts.to(self._device())
+        box = _oriented_box(pts, extend)
+        dev = self.center.device
+        self.center[:] = box[0:3].to(dev)
+        self.R[:] = box[3:12].view(3, 3).to(dev)
+        self.extent[:] = box[12:15].to(dev)
+
+    def in_bound(self, pointcloud):
+        """points inside the box: a numpy bool [n] for an ndarray, a CUDA bool [n] for a CUDA tensor"""
+        if isinstance(pointcloud, torch.Tensor) and pointcloud.is_cuda:
+            dev = pointcloud.device
+            return in_oriented_box(pointcloud, self.center.to(dev), self.R.to(dev), self.extent.to(dev))
+        dev = self._device()
+        pts = torch.as_tensor(np.asarray(pointcloud, np.float64)).to(dev)
+        mask = in_oriented_box(pts, self.center.to(dev), self.R.to(dev), self.extent.to(dev))
+        return mask.cpu().numpy().astype(np.bool_)
+
+    def get_aabb(self):
+        import open3d as o3d
+        center = self.center.detach().cpu().numpy().astype(np.float64)
+        R = self.R.detach().cpu().numpy().astype(np.float64)
+        extent = self.extent.detach().cpu().numpy().astype(np.float64)
+        return o3d.geometry.OrientedBoundingBox(center=center, R=R, extent=extent)
+
+    def box_points(self):
+        """the 8 corners [8,3] f64 in Open3D's GetBoxPoints order"""
+        c, R, e = (t.detach().cpu().double() for t in (self.center, self.R, self.extent))
+        ax = [R[:, j] * (e[j] / 2) for j in range(3)]
+        sg = [(-1, -1, -1), (1, -1, -1), (-1, 1, -1), (-1, -1, 1), (1, 1, 1), (-1, 1, 1), (1, -1, 1), (1, 1, -1)]
+        return torch.stack([c + s[0] * ax[0] + s[1] * ax[1] + s[2] * ax[2] for s in sg])
+
+    def get_axis_aligned_bounding_box(self):
+        """[3,2] float32: min and max of the 8 corners"""
+        pts = self.box_points().numpy()
+        return np.concatenate([pts.min(0).astype(np.float32)[:, None], pts.max(0).astype(np.float32)[:, None]], axis=1)
+
+
+def mapping_points(video, cur_idx):
+    """the points update_param_from_mapping(the_end=True) bounds (src/mesher.py:256-276) as f64 [n,3] on the video's
+    device: iproj of keyframes [0, cur_idx) at full resolution under w2w * SE3(poses).inv(), where depth_filter gives
+    >= 3 votes (thresh 0.01) and disps_up > 0.01 * the frame's mean, in [b, h, w] order.  One host read (the count)."""
+    from . import lietorch
+    T = int(cur_idx)
+    dev = video.poses.device
+    if dev.type != "cuda":
+        raise RuntimeError("mapping_points: a CUDA video is required (no CPU fallback)")
+    _, ht, wd = video.disps_up.shape
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        nbytes = lib.goslam_mapping_points_workspace_bytes(T, ht, wd)
+        if nbytes == 0:
+            raise ValueError("mapping_points: invalid shape (%d, %d, %d)" % (T, ht, wd))
+        poses = video.poses.detach()[:T].float().contiguous()
+        disps = video.disps_up.detach()[:T].float().contiguous()
+        intr = (video.intrinsics[0].detach() * video.scale_factor).float().contiguous()
+        w2w = lietorch.SE3(video.pose_compensate[0].clone().unsqueeze(dim=0)).to(dev)
+        poses_world = (w2w * lietorch.SE3(poses).inv()).data.float().contiguous()
+        ws = _workspace(nbytes, dev)
+        count = torch.empty(1, dtype=torch.int64, device=dev)
+        st = _lib.stream_ptr()
+        _lib.check(lib.goslam_mapping_points_count(_lib.ptr(poses), _lib.ptr(poses_world), _lib.ptr(disps),
+                                                   _lib.ptr(intr), T, ht, wd, _lib.ptr(ws), nbytes, _lib.ptr(count),
+                                                   st), "mapping_points_count")
+        n = int(count.item())
+        out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+        _lib.check(lib.goslam_mapping_points_emit(_lib.ptr(poses_world), _lib.ptr(disps), _lib.ptr(intr), T, ht, wd,
+                                                  _lib.ptr(ws), nbytes, _lib.ptr(out), n, st), "mapping_points_emit")
+    return out
+
+
+@torch.no_grad()
+def update_param_from_mapping(self, the_end=False):
+    """Mesher.update_param_from_mapping (src/mesher.py:242-281): (timestamp, cur_idx - 1, a device copy of the shared
+    mapping net, the scene's OrientedBoundingBox with extend 0.1 when the_end else None, keyframe camera-to-world
+    matrices on the CPU).  The point selection, hull and box stay on the device."""
+    import copy
+    from . import lietorch
+    net = copy.deepcopy(self.shared_mapping_net).to(self.device)
+    cur_idx = self.video.counter.value
+    timestamp = self.video.timestamp[cur_idx - 1]
+    aabb = None
+    kf_c2w_list = lietorch.SE3(self.video.poses.detach()[:cur_idx]).inv().matrix().data.cpu()
+    if the_end:
+        sel_points = mapping_points(self.video, cur_idx)
+        aabb = OrientedBoundingBox().to(self.device)
+        aabb.compute_from_pointcloud(sel_points, extend=MAPPING_EXTEND)
+    return timestamp, cur_idx - 1, net, aabb, kf_c2w_list

@@ -736,6 +736,45 @@ int goslam_icp_point_to_point(const double* source, int64_t n_source, const void
                               double relative_fitness, double relative_rmse, double* result, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Scene bound of Mesher.update_param_from_mapping (src/mesher.py:242-281, src/oriented_bounding_box.py): the mapping
+ * point selection, convex-hull vertices and Open3D 0.13's oriented bounding box.  Device pointers, no host
+ * synchronisation.
+ *
+ * goslam_mapping_points_count — the multiview filter's mask1 with thresh 0.01 and visible_num 3 over the T keyframes
+ *   (poses [T,7] for the votes, poses_world [T,7] = w2w * SE3(poses).inv() for the points, disps [T,ht,wd], intrinsic
+ *   [4] already scaled): *count (device int64) = number of selected pixels.
+ * goslam_mapping_points_emit — the selected pixels' iproj points, [b,h,w] row-major, widened to f64 [n_points,3];
+ *   n_points must be the count of the preceding _count call on the same workspace.
+ *   Workspace: goslam_mapping_points_workspace_bytes(T, ht, wd) (0 = invalid shape).
+ *
+ * goslam_hull_vertices — the vertices of the convex hull of points [n,3] f64 (1 <= n <= 2^28): the exact extreme
+ *   points (a point on a hull face or edge is not one; of equal points only the lowest index can be one), sorted, kept
+ *   in the workspace.  info [4] (device int64): status (0 ok, 1 fewer than four affinely independent points, 2 hull too
+ *   large, 3 non-finite coordinate, 4 inconsistent facet graph), vertex count, survivors of the interior cull,
+ *   distinct direction extremes.
+ *   Workspace: goslam_hull_workspace_bytes(n).
+ * goslam_hull_vertices_emit — the first count (= info[1]) vertex ids as int64.
+ * goslam_obb_from_hull — box [15] f64 = center [3], R [9] row-major, extent [3] (+ extend) of OrientedBoundingBox::
+ *   CreateFromPoints on the hull of the preceding goslam_hull_vertices call; unwritten unless its status is 0.
+ * goslam_obb_in_bound — mask [n] (1 = inside) of GetPointIndicesWithinBoundingBox for the box [15] in device memory.
+ * ---------------------------------------------------------------------------------- */
+size_t goslam_mapping_points_workspace_bytes(int T, int ht, int wd);
+int goslam_mapping_points_count(const float* poses, const float* poses_world, const float* disps,
+                                const float* intrinsic, int T, int ht, int wd, void* workspace, size_t workspace_bytes,
+                                int64_t* count, void* stream);
+int goslam_mapping_points_emit(const float* poses_world, const float* disps, const float* intrinsic, int T, int ht,
+                               int wd, void* workspace, size_t workspace_bytes, double* points, int64_t n_points,
+                               void* stream);
+size_t goslam_hull_workspace_bytes(int64_t n);
+int goslam_hull_vertices(const double* points, int64_t n, void* workspace, size_t workspace_bytes, int64_t* info,
+                         void* stream);
+int goslam_hull_vertices_emit(const void* workspace, size_t workspace_bytes, int64_t n, int64_t* out, int64_t count,
+                              void* stream);
+int goslam_obb_from_hull(const double* points, int64_t n, const void* workspace, size_t workspace_bytes, double extend,
+                         double* box, void* stream);
+int goslam_obb_in_bound(const double* box, const double* points, int64_t n, uint8_t* mask, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
