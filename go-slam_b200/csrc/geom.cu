@@ -678,7 +678,7 @@ int goslam_frame_distance_bidir(const float* poses, const float* disps, const fl
 int goslam_projmap(const float* poses, const float* disps, const float* intrinsics,
                    const int64_t* ii, const int64_t* jj, float* coords, float* valid, int K,
                    int ht, int wd, void* stream) {
-  if (K < 0 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if (K < 0 || K > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
   if (K == 0) return GOSLAM_OK;
   dim3 grid(gs_cdiv(ht * wd, kThreads), K);
   projmap_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, ii, jj,
@@ -690,7 +690,7 @@ int goslam_projmap(const float* poses, const float* disps, const float* intrinsi
 int goslam_reproject(const float* poses, const float* disps, const float* intrinsics_all,
                      const int64_t* ii, const int64_t* jj, float* coords, float* valid, int K,
                      int ht, int wd, void* stream) {
-  if (K < 0 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if (K < 0 || K > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
   if (K == 0) return GOSLAM_OK;
   dim3 grid(gs_cdiv(ht * wd, kThreads), K);
   reproject_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics_all, ii,
@@ -702,7 +702,7 @@ int goslam_reproject(const float* poses, const float* disps, const float* intrin
 int goslam_reproject_motion(const float* poses, const float* disps, const float* intrinsics_all,
                             const int64_t* ii, const int64_t* jj, const float* target, float* coords,
                             float* valid, float* motion, int K, int ht, int wd, void* stream) {
-  if (K < 0 || ht <= 0 || wd <= 0 || target == nullptr || motion == nullptr) return GOSLAM_EINVAL;
+  if (K < 0 || K > 65535 || ht <= 0 || wd <= 0 || target == nullptr || motion == nullptr) return GOSLAM_EINVAL;
   if (K == 0) return GOSLAM_OK;
   dim3 grid(gs_cdiv(ht * wd, kThreads), K);
   reproject_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics_all, ii,
@@ -713,7 +713,7 @@ int goslam_reproject_motion(const float* poses, const float* disps, const float*
 
 int goslam_iproj(const float* poses, const float* disps, const float* intrinsics, float* points,
                  int num, int ht, int wd, void* stream) {
-  if (num < 0 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if (num < 0 || num > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
   if (num == 0) return GOSLAM_OK;
   dim3 grid(gs_cdiv(ht * wd, kThreads), num);
   iproj_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, points, ht,
@@ -725,7 +725,7 @@ int goslam_iproj(const float* poses, const float* disps, const float* intrinsics
 int goslam_depth_filter(const float* poses, const float* disps, const float* intrinsics,
                         const int64_t* ix, const float* thresh, float* counter, int K, int num,
                         int ht, int wd, void* stream) {
-  if (K < 0 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if (K < 0 || K > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
   if (K == 0) return GOSLAM_OK;
   dim3 grid(gs_cdiv(ht * wd, kThreads), K);
   depth_filter_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, ix,

@@ -128,6 +128,9 @@ int goslam_altcorr_pyramid(const void* const* pyramid, int num_levels, const flo
  * Geometry kernels of droid_backends (src/lib/droid.cpp:120-160,220-225).
  *   poses [num,7] f32 (tx,ty,tz,qx,qy,qz,qw); disps [num,ht,wd] f32; intrinsics [4]
  *   f32 (fx,fy,cx,cy); ii,jj int64.
+ *   projmap, reproject, reproject_motion and depth_filter launch one grid row per edge and
+ *   iproj one per frame: K (num for iproj) above 65535 returns GOSLAM_EINVAL before any CUDA
+ *   call.
  * ---------------------------------------------------------------------------------- */
 /* frame_distance (src/lib/droid_kernels.cu:518-657,1438-1460): dist [K] f32.
  * Reduction order reproduces the reference's 256-thread strided sum + 128/64/32..1 tree

@@ -162,3 +162,60 @@ def altcorr_forward(fmap1, fmap2, coords, r=3):
         # v[b,h,w,oy,ox] -> channel ox*rd + oy
         out[:, s] = v.transpose(0, 4, 3, 1, 2).reshape(B, rd * rd, H, W)
     return out
+
+
+def altcorr_pyramid(pyr, coords, ii, jj, num_levels, dtype=torch.float64, chunk=16):
+    """AltCorrBlock.__call__ (src/modules/corr.py:113-145) on the half pyramid values widened to `dtype`:
+    pyr[l] [F, H >> l, W >> l, C] (torch or numpy, any device), coords [N, H, W, 2] f32, ii / jj [N] frame ids.
+    Returns (out, mag), both [N, L * 49, H, W] in `dtype` on pyr's device:
+      out = sum over the 4 bilinear taps of w * <f1, f2>, with dx, dy the float32 fractions of coords * 2^-l
+            (scaling by a power of two and flooring are exact in float32) and w in `dtype`;
+      mag = sum over the taps of |w| * sum_c |f1_c * f2_c|, the magnitude a rounding-error bound scales with.
+    Channel = ox * 7 + oy inside a level (x-offset-major), level-major across levels."""
+    pyr = [torch.as_tensor(p) for p in pyr[:num_levels]]
+    dev = pyr[0].device
+    coords = torch.as_tensor(coords).to(dev, torch.float32)
+    ii = torch.as_tensor(ii).to(dev).long()
+    jj = torch.as_tensor(jj).to(dev).long()
+    N, H, W, _ = coords.shape
+    C = pyr[0].shape[-1]
+    r, rd = 3, 7
+    out = torch.zeros((N, num_levels * rd * rd, H * W), dtype=dtype, device=dev)
+    mag = torch.zeros_like(out)
+    p1 = pyr[0].to(dtype).reshape(-1, H * W, C)
+    for lvl in range(num_levels):
+        H2, W2 = pyr[lvl].shape[1], pyr[lvl].shape[2]
+        p2 = pyr[lvl].to(dtype).reshape(-1, H2 * W2, C)
+        c = coords.reshape(N, H * W, 2) * (1.0 / (1 << lvl))
+        f = torch.floor(c)
+        fr = (c - f).to(dtype)                                  # exact in float32, widened
+        f = f.clamp(-2.0 ** 30, 2.0 ** 30).long()
+        dx, dy = fr[..., 0], fr[..., 1]
+        wts = {(0, 0): (1 - dy) * (1 - dx), (0, 1): (1 - dy) * dx, (1, 0): dy * (1 - dx), (1, 1): dy * dx}
+        for n0 in range(0, N, chunk):
+            sl = slice(n0, min(N, n0 + chunk))
+            f1 = p1[ii[sl]]                                                          # [n, HW, C]
+            f2 = p2[jj[sl]]                                                          # [n, H2W2, C]
+            taps = torch.zeros((f1.shape[0], H * W, rd + 1, rd + 1), dtype=dtype, device=dev)
+            atap = torch.zeros_like(taps)
+            for iy in range(rd + 1):
+                for ix in range(rd + 1):
+                    y = f[sl, :, 1] - r + iy
+                    x = f[sl, :, 0] - r + ix
+                    ok = (y >= 0) & (y < H2) & (x >= 0) & (x < W2)
+                    idx = (y.clamp(0, H2 - 1) * W2 + x.clamp(0, W2 - 1))
+                    g = torch.gather(f2, 1, idx[..., None].expand(-1, -1, C))
+                    prod = f1 * g
+                    taps[..., iy, ix] = torch.where(ok, prod.sum(-1), 0)
+                    atap[..., iy, ix] = torch.where(ok, prod.abs().sum(-1), 0)
+            for ox in range(rd):
+                for oy in range(rd):
+                    ch = lvl * rd * rd + ox * rd + oy
+                    o = torch.zeros_like(dx[sl])
+                    m = torch.zeros_like(dx[sl])
+                    for (jy, jx), w in wts.items():
+                        o = o + w[sl] * taps[..., oy + jy, ox + jx]
+                        m = m + w[sl].abs() * atap[..., oy + jy, ox + jx]
+                    out[sl, ch] = o
+                    mag[sl, ch] = m
+    return out.reshape(N, -1, H, W), mag.reshape(N, -1, H, W)

@@ -279,14 +279,21 @@ def depth_filter(poses, disps, intrinsics, ix, thresh):
 
 
 # ----------------------------------------------------------------------------- reproject
-def reproject(poses, disps, intrinsics_all, ii, jj):
-    """pops.projective_transform(jacobian=False): Python-side constants (MIN_DEPTH 0.2)."""
+def reproject(poses, disps, intrinsics_all, ii, jj, dtype=F, return_z=False):
+    """pops.projective_transform(jacobian=False): Python-side constants (MIN_DEPTH 0.2).
+
+    dtype=np.float64 evaluates the same formula in float64 from the float32 inputs (relative pose, back-projection,
+    action, projection), keeping the float32 thresholds the reference compares against (0.5 * 0.2 and 0.2, both
+    rounded to float32 as torch rounds a Python scalar against a float32 tensor).  return_z adds X1z [N, ht, wd];
+    with dtype=np.float64, return_z="points" returns X1 [N, ht, wd, 3] alone."""
     poses, disps, Kall = _f(poses), _f(disps), _f(intrinsics_all)
     ii, jj = np.asarray(ii, np.int64), np.asarray(jj, np.int64)
     N = ii.shape[0]
     num, ht, wd = disps.shape
     hw = ht * wd
     u, v = pixel_grid(ht, wd)
+    if dtype == np.float64:
+        return _reproject64(poses, disps, Kall, ii, jj, u, v, return_z)
     Ki, Kj = Kall[ii], Kall[jj]
     X0 = np.stack([(u[None] - Ki[:, 2:3]) / Ki[:, 0:1], (v[None] - Ki[:, 3:4]) / Ki[:, 1:2],
                    np.ones((N, hw), F), disps[ii].reshape(N, hw)], axis=-1).astype(F)
@@ -297,4 +304,71 @@ def reproject(poses, disps, intrinsics_all, ii, jj):
     y = Kj[:, 1:2] * (X1[..., 1] / Z) + Kj[:, 3:4]
     coords = np.stack([x, y], axis=-1).reshape(1, N, ht, wd, 2).astype(F)
     valid = ((X1[..., 2] > F(0.2)) & (X0[..., 2] > F(0.2))).astype(F).reshape(1, N, ht, wd, 1)
+    if return_z:
+        return coords, valid, X1[..., 2].reshape(N, ht, wd)
     return coords, valid
+
+
+def _rot64(q, X):
+    """R(q) X in float64 (the act_so3 formula; q need not be exactly unit, as the stored quaternions are not)."""
+    q0, q1, q2, q3 = [q[..., i] for i in range(4)]
+    X0, X1, X2 = [X[..., i] for i in range(3)]
+    u0 = 2.0 * (q1 * X2 - q2 * X1)
+    u1 = 2.0 * (q2 * X0 - q0 * X2)
+    u2 = 2.0 * (q0 * X1 - q1 * X0)
+    return np.stack([X0 + q3 * u0 + (q1 * u2 - q2 * u1),
+                     X1 + q3 * u1 + (q2 * u0 - q0 * u2),
+                     X2 + q3 * u2 + (q0 * u1 - q1 * u0)], axis=-1)
+
+
+def edge_pose64(poses, ii, jj):
+    """edge_pose(stereo_special=True) in float64 from float32 poses."""
+    P = np.asarray(poses, F).astype(np.float64)
+    ti, qi, tj, qj = P[ii, :3], P[ii, 3:], P[jj, :3], P[jj, 3:]
+    q = np.stack([
+        -qj[..., 3] * qi[..., 0] + qj[..., 0] * qi[..., 3] - qj[..., 1] * qi[..., 2] + qj[..., 2] * qi[..., 1],
+        -qj[..., 3] * qi[..., 1] + qj[..., 1] * qi[..., 3] - qj[..., 2] * qi[..., 0] + qj[..., 0] * qi[..., 2],
+        -qj[..., 3] * qi[..., 2] + qj[..., 2] * qi[..., 3] - qj[..., 0] * qi[..., 1] + qj[..., 1] * qi[..., 0],
+        qj[..., 3] * qi[..., 3] + qj[..., 0] * qi[..., 0] + qj[..., 1] * qi[..., 1] + qj[..., 2] * qi[..., 2],
+    ], axis=-1)
+    t = tj - _rot64(q, ti)
+    s = np.asarray(ii) == np.asarray(jj)
+    t[s] = [-0.1, 0.0, 0.0]
+    q[s] = [0.0, 0.0, 0.0, 1.0]
+    return t, q
+
+
+def _reproject64(poses, disps, Kall, ii, jj, u, v, return_z):
+    N = ii.shape[0]
+    num, ht, wd = disps.shape
+    K64 = Kall.astype(np.float64)
+    Ki, Kj = K64[ii], K64[jj]
+    u, v = u.astype(np.float64), v.astype(np.float64)
+    d = disps[ii].reshape(N, -1).astype(np.float64)
+    X0 = np.stack([(u[None] - Ki[:, 2:3]) / Ki[:, 0:1], (v[None] - Ki[:, 3:4]) / Ki[:, 1:2], np.ones_like(d)], -1)
+    t, q = edge_pose64(poses, ii, jj)
+    X1 = _rot64(q[:, None, :], X0) + d[..., None] * t[:, None, :]
+    if return_z == "points":
+        return X1.reshape(N, ht, wd, 3)
+    z = X1[..., 2]
+    Z = np.where(z < float(F(0.5) * F(0.2)), 1.0, z)
+    x = Kj[:, 0:1] * (X1[..., 0] / Z) + Kj[:, 2:3]
+    y = Kj[:, 1:2] * (X1[..., 1] / Z) + Kj[:, 3:4]
+    coords = np.stack([x, y], axis=-1).reshape(1, N, ht, wd, 2)
+    valid = (z > float(F(0.2))).astype(np.float64).reshape(1, N, ht, wd, 1)
+    if return_z:
+        return coords, valid, z.reshape(N, ht, wd)
+    return coords, valid
+
+
+def reproject_motion(coords1, target):
+    """FactorGraph.update's motion features (src/factor_graph.py:202-206), in the inputs' dtype:
+    cat([coords1 - coords0, target - coords1], -1).permute(0, 1, 4, 2, 3).clamp(-64, 64) with coords0 the pixel
+    grid (x, y).  coords1, target [1, N, ht, wd, 2] -> motion [1, N, 4, ht, wd] = [dx, dy, tx - x, ty - y]."""
+    coords1 = np.asarray(coords1)
+    target = np.asarray(target, coords1.dtype)
+    ht, wd = coords1.shape[2], coords1.shape[3]
+    v, u = np.meshgrid(np.arange(ht), np.arange(wd), indexing="ij")
+    coords0 = np.stack([u, v], axis=-1).astype(coords1.dtype)
+    motion = np.concatenate([coords1 - coords0, target - coords1], axis=-1)
+    return np.clip(motion.transpose(0, 1, 4, 2, 3), -64.0, 64.0).astype(coords1.dtype)

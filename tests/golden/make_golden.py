@@ -16,6 +16,7 @@ What each fixture pins:
     cvx_upsample.npz  cvx_upsample (f32 and f16 masks)            src/droid_net.py:9-23
     proximity.npz     FactorGraph.add_proximity_factors edges     src/factor_graph.py:384-450
     altcorr_pyramid.npz AltCorrBlock.__init__ pyramid            src/modules/corr.py:97-111
+    features.npz      projective_transform + motion, crafted rig  src/geom/projective_ops.py:114-144, src/factor_graph.py:202-206
     backend_edges.npz Backend.ba edge selection (loop=False)      src/backend.py:25-99
     factor_graph.npz  FactorGraph + DepthVideo state machine      src/factor_graph.py:85-450, src/depth_video.py:194-269
     conv_gru.npz      ConvGRU.forward (fp32)                      src/modules/gru.py:21-39
@@ -669,11 +670,42 @@ def gen_update_module():
                         wsum=np.float64(sum(float(p.detach().double().sum()) for p in upd.parameters())))
 
 
+def gen_features():
+    """the reference's pops.projective_transform (src/geom/projective_ops.py:114-144) and FactorGraph.update's motion
+    lines (src/factor_graph.py:202-206) on the crafted rig window of tests/test_features_cases.py (frames facing
+    away, per-frame intrinsics, stereo self-edges, planted threshold pixels, targets beyond +-64)."""
+    pops = ref_import("src.geom.projective_ops")
+    import lietorch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_features_cases import reproject_case
+    c = reproject_case("rig_37x45")
+    # a < 0.5 MB subset of the edges: every planted one (z translation, exact thresholds), two stereo, three others
+    st, other = np.nonzero(c["ii"] == c["jj"])[0], np.nonzero((c["ii"] != c["jj"]) & ~c["planted"])[0]
+    keep = np.sort(np.concatenate([np.nonzero(c["planted"])[0], st[:2], other[:3]]))
+    for k in ("ii", "jj", "planted", "tz"):
+        c[k] = c[k][keep]
+    c["target"] = c["target"][:, keep]
+    ii, jj = torch.from_numpy(c["ii"]), torch.from_numpy(c["jj"])
+    coords1, valid = pops.projective_transform(lietorch.SE3(torch.from_numpy(c["poses"])[None]),
+                                               torch.from_numpy(c["disps"])[None],
+                                               torch.from_numpy(c["intrinsics"])[None], ii, jj)
+    ht, wd = c["ht"], c["wd"]
+    y, x = torch.meshgrid(torch.arange(ht).float(), torch.arange(wd).float(), indexing="ij")
+    coords0 = torch.stack([x, y], dim=-1)
+    target = torch.from_numpy(c["target"])
+    motion = torch.cat([coords1 - coords0, target - coords1], dim=-1)
+    motion = motion.permute(0, 1, 4, 2, 3).clamp(-64.0, 64.0)
+    np.savez_compressed(os.path.join(HERE, "features.npz"), poses=c["poses"], disps=c["disps"],
+                        intrinsics=c["intrinsics"], ii=c["ii"], jj=c["jj"], planted=c["planted"], tz=c["tz"],
+                        target=c["target"], coords=coords1.numpy(), valid=valid.numpy(), motion=motion.numpy())
+
+
 if __name__ == "__main__":
     if not os.path.isdir(REF):
         raise SystemExit("needs /root/reference (build container only)")
     install_stubs()
-    which = sys.argv[1:] or ["corr_block", "reproject", "ba_torch", "neus", "render_z", "cvx_upsample", "proximity", "backend_edges", "altcorr_pyramid", "altcorr_block"]
+    which = sys.argv[1:] or ["corr_block", "reproject", "ba_torch", "neus", "render_z", "cvx_upsample", "proximity", "backend_edges", "altcorr_pyramid", "altcorr_block", "features"]
     for name in which:
         globals()["gen_" + name]()
         print("wrote", name)
+

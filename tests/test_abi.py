@@ -77,6 +77,15 @@ def test_argument_validation_without_gpu(lib):
     assert lib.goslam_corr_build(null, null, 0, null, 4, 0, 128, 40, 80, null) == 0               # N == 0: no-op
     assert lib.goslam_corr_pool_build(null, 8, 1, null, null, null, null, 4, 1, 128, 40, 160, null) == -1  # w > 128
     assert lib.goslam_frame_distance(null, null, null, null, null, null, 0, 4, 4, 0.3, null) == 0
+    # the per-pixel geometry entries put edges (frames for iproj) on grid.y: more than 65535 is a shape error,
+    # not a failed launch; 65535 itself passes validation (null stream / pointers never reach a device at K = 0)
+    for K in (65536, 1 << 30):
+        assert lib.goslam_reproject(null, null, null, null, null, null, null, K, 4, 4, null) == -1
+        assert lib.goslam_reproject_motion(null, null, null, null, null, null, null, null, null, K, 4, 4, null) == -1
+        assert lib.goslam_projmap(null, null, null, null, null, null, null, K, 4, 4, null) == -1
+        assert lib.goslam_depth_filter(null, null, null, null, null, null, K, 8, 4, 4, null) == -1
+        assert lib.goslam_iproj(null, null, null, null, K, 4, 4, null) == -1
+    assert lib.goslam_reproject(null, null, null, null, null, null, null, 0, 4, 4, null) == 0
     assert lib.goslam_altcorr_forward(null, null, null, null, 1, 1, 4, 4, 4, 4, 128, 2, null) == -1  # r != 3
     assert lib.goslam_ba(null, null, null, null, null, null, null, 0, null, null, 4, 8, 4, 4, 1, 8, 2,
                          1e-4, 0.1, 0, null, null, null, null, 0, null) == -1     # eta missing
