@@ -90,7 +90,7 @@ struct TcParams {
   const int64_t* ii; const int64_t* jj; int rig;
   const int* out_slot;        // optional edge -> output slot of the level buffers (CorrPool)
   // levels 0 and 1 are stored as 4x4-element (32-byte) tiles, tile-row-major inside each
-  // source pixel's plane (plane = H4*W4 tiles, padded with zeros); levels 2, 3 stay row-major.
+  // source pixel's plane (plane = H4*W4 tiles; the padding is unspecified); levels 2, 3 stay row-major.
   int w4_0, h4_0, w4_1, h4_1;
   int pitch2, pitch3;         // bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
 };

@@ -20,6 +20,12 @@
 //        tap order (x outer, y inner);
 //   f16: every product and every add is rounded to half, weights rounded to half first —
 //        what `corr += s * scalar_t(w)` does for c10::Half (src/lib/correlation_kernels.cu:53-63).
+// A tap outside the level adds nothing, as the reference's within_bounds test has it.  With a finite
+// coordinate the zeroed taps give the same sums.  A NaN or infinite one makes every weight NaN, so a
+// rarely taken branch gives the outside taps weight 0: an output whose four taps all lie outside is 0,
+// the others NaN, as in the reference (float-to-int conversion takes NaN to 0 and saturates).  Window
+// origins are clamped to +-2^30 first, so that the tap indices of a huge or infinite coordinate cannot
+// overflow; every tap of a clamped origin is outside the level.
 #include "common.cuh"
 
 namespace {
@@ -114,6 +120,11 @@ __device__ __forceinline__ void fetch_row8_tiled_h(const __half* __restrict__ pl
 }
 
 __device__ __forceinline__ __half2 u2h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
+__device__ __forceinline__ uint32_t h22u(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+
+// floor(x) as the device converts it (NaN -> 0, saturating), clamped so that the taps' indices cannot overflow
+constexpr int kFarOrigin = 1 << 30;
+__device__ __forceinline__ int origin(float f) { return min(max((int)f, -kFarOrigin), kFarOrigin); }
 
 // zero the taps whose column x1+t is outside [0,w2)
 __device__ __forceinline__ void mask_cols_h(uint32_t (&w)[4], int x1, int w2) {
@@ -139,8 +150,8 @@ __device__ __forceinline__ void lookup_pass_h(const __half* __restrict__ vol, lo
   static_assert(RD + 1 == 8, "row-lane mapping assumes radius 3 (8-tap windows)");
   const float fx0 = floorf(x0), fy0 = floorf(y0);
   const float dx = x0 - fx0, dy = y0 - fy0;
-  const int x1 = (int)fx0 - R;
-  const int y1 = (int)fy0 - R + row;
+  const int x1 = origin(fx0) - R;
+  const int y1 = origin(fy0) - R + row;
 
   uint32_t own[4] = {0, 0, 0, 0};
   if (active && y1 >= 0 && y1 < h2 && x1 > -8 && x1 < w2) {
@@ -159,21 +170,43 @@ __device__ __forceinline__ void lookup_pass_h(const __half* __restrict__ vol, lo
   const __half2 w11 = __float2half2_rn(dx * dy);
 
   if (row < RD && active) {
+    if (__builtin_expect(dx == dx && dy == dy, 1)) {       // dx, dy are NaN iff x0 or y0 is not finite
 #pragma unroll
-    for (int m = 0; m < 4; ++m) {
-      // P = taps (2m, 2m+1), Q = taps (2m+1, 2m+2)
-      const uint32_t ownn = (m < 3) ? own[m + 1] : 0u;
-      const uint32_t dnn = (m < 3) ? dn[m + 1] : 0u;
-      const __half2 P = u2h2(own[m]), Pd = u2h2(dn[m]);
-      const __half2 Q = u2h2(__funnelshift_r(own[m], ownn, 16));
-      const __half2 Qd = u2h2(__funnelshift_r(dn[m], dnn, 16));
-      __half2 acc = __hmul2_rn(P, w00);
-      acc = __hadd2_rn(acc, __hmul2_rn(Pd, w01));
-      acc = __hadd2_rn(acc, __hmul2_rn(Q, w10));
-      acc = __hadd2_rn(acc, __hmul2_rn(Qd, w11));
-      // outputs i = 2m (low), 2m+1 (high); channel = i*RD + row
-      stage[(2 * m * RD + row) * stage_ld + px_in_tile] = __low2half(acc);
-      if (2 * m + 1 < RD) stage[((2 * m + 1) * RD + row) * stage_ld + px_in_tile] = __high2half(acc);
+      for (int m = 0; m < 4; ++m) {
+        // P = taps (2m, 2m+1), Q = taps (2m+1, 2m+2)
+        const uint32_t ownn = (m < 3) ? own[m + 1] : 0u;
+        const uint32_t dnn = (m < 3) ? dn[m + 1] : 0u;
+        const __half2 P = u2h2(own[m]), Pd = u2h2(dn[m]);
+        const __half2 Q = u2h2(__funnelshift_r(own[m], ownn, 16));
+        const __half2 Qd = u2h2(__funnelshift_r(dn[m], dnn, 16));
+        __half2 acc = __hmul2_rn(P, w00);
+        acc = __hadd2_rn(acc, __hmul2_rn(Pd, w01));
+        acc = __hadd2_rn(acc, __hmul2_rn(Q, w10));
+        acc = __hadd2_rn(acc, __hmul2_rn(Qd, w11));
+        // outputs i = 2m (low), 2m+1 (high); channel = i*RD + row
+        stage[(2 * m * RD + row) * stage_ld + px_in_tile] = __low2half(acc);
+        if (2 * m + 1 < RD) stage[((2 * m + 1) * RD + row) * stage_ld + px_in_tile] = __high2half(acc);
+      }
+    } else {
+      // non-finite coordinate: the same sums with each outside tap's weight masked to 0
+      uint32_t cp[4] = {~0u, ~0u, ~0u, ~0u}, cq[4] = {~0u, ~0u, ~0u, ~0u};
+      mask_cols_h(cp, x1, w2);                              // columns of taps (2m, 2m+1)
+      mask_cols_h(cq, x1 + 1, w2);                          // columns of taps (2m+1, 2m+2)
+      const uint32_t r0 = (y1 >= 0 && y1 < h2) ? ~0u : 0u, r1 = (y1 + 1 >= 0 && y1 + 1 < h2) ? ~0u : 0u;
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const uint32_t ownn = (m < 3) ? own[m + 1] : 0u;
+        const uint32_t dnn = (m < 3) ? dn[m + 1] : 0u;
+        const __half2 P = u2h2(own[m]), Pd = u2h2(dn[m]);
+        const __half2 Q = u2h2(__funnelshift_r(own[m], ownn, 16));
+        const __half2 Qd = u2h2(__funnelshift_r(dn[m], dnn, 16));
+        __half2 acc = __hmul2_rn(P, u2h2(h22u(w00) & cp[m] & r0));
+        acc = __hadd2_rn(acc, __hmul2_rn(Pd, u2h2(h22u(w01) & cp[m] & r1)));
+        acc = __hadd2_rn(acc, __hmul2_rn(Q, u2h2(h22u(w10) & cq[m] & r0)));
+        acc = __hadd2_rn(acc, __hmul2_rn(Qd, u2h2(h22u(w11) & cq[m] & r1)));
+        stage[(2 * m * RD + row) * stage_ld + px_in_tile] = __low2half(acc);
+        if (2 * m + 1 < RD) stage[((2 * m + 1) * RD + row) * stage_ld + px_in_tile] = __high2half(acc);
+      }
     }
   }
 }
@@ -186,8 +219,8 @@ __device__ __forceinline__ void lookup_pass_f(const float* __restrict__ vol, lon
   constexpr int RD = 2 * R + 1;
   const float fx0 = floorf(x0), fy0 = floorf(y0);
   const float dx = x0 - fx0, dy = y0 - fy0;
-  const int x1 = (int)fx0 - R;
-  const int y1 = (int)fy0 - R + row;
+  const int x1 = origin(fx0) - R;
+  const int y1 = origin(fy0) - R + row;
   float own[8];
 #pragma unroll
   for (int t = 0; t < 8; ++t) own[t] = 0.f;
@@ -205,13 +238,27 @@ __device__ __forceinline__ void lookup_pass_f(const float* __restrict__ vol, lon
   const float w00 = (1.0f - dx) * (1.0f - dy), w01 = (1.0f - dx) * dy;
   const float w10 = dx * (1.0f - dy), w11 = dx * dy;
   if (row < RD && active) {
+    if (__builtin_expect(dx == dx && dy == dy, 1)) {       // dx, dy are NaN iff x0 or y0 is not finite
 #pragma unroll
-    for (int i = 0; i < RD; ++i) {
-      float acc = __fmul_rn(own[i], w00);
-      acc = __fmaf_rn(dn[i], w01, acc);
-      acc = __fmaf_rn(own[i + 1], w10, acc);
-      acc = __fmaf_rn(dn[i + 1], w11, acc);
-      stage[(i * RD + row) * stage_ld + px_in_tile] = acc;
+      for (int i = 0; i < RD; ++i) {
+        float acc = __fmul_rn(own[i], w00);
+        acc = __fmaf_rn(dn[i], w01, acc);
+        acc = __fmaf_rn(own[i + 1], w10, acc);
+        acc = __fmaf_rn(dn[i + 1], w11, acc);
+        stage[(i * RD + row) * stage_ld + px_in_tile] = acc;
+      }
+    } else {
+      // non-finite coordinate: the same sums with each outside tap's weight masked to 0
+      const bool r0 = y1 >= 0 && y1 < h2, r1 = y1 + 1 >= 0 && y1 + 1 < h2;
+#pragma unroll
+      for (int i = 0; i < RD; ++i) {
+        const bool c0 = x1 + i >= 0 && x1 + i < w2, c1 = x1 + i + 1 >= 0 && x1 + i + 1 < w2;
+        float acc = __fmul_rn(own[i], c0 && r0 ? w00 : 0.f);
+        acc = __fmaf_rn(dn[i], c0 && r1 ? w01 : 0.f, acc);
+        acc = __fmaf_rn(own[i + 1], c1 && r0 ? w10 : 0.f, acc);
+        acc = __fmaf_rn(dn[i + 1], c1 && r1 ? w11 : 0.f, acc);
+        stage[(i * RD + row) * stage_ld + px_in_tile] = acc;
+      }
     }
   }
 }

@@ -44,6 +44,10 @@ const char* goslam_last_cuda_error(void);
  * src/lib/correlation_kernels.cu:19-70,126-155).
  *   volume [N,h1,w1,h2,w2] (f16|f32), coords [N,2,h1,w1] f32 (x then y),
  *   corr   [N,2r+1,2r+1,h1,w1] same dtype as volume, x-offset-major, fully overwritten.
+ * A tap outside the level adds nothing (the reference's within_bounds).  So a NaN or infinite coordinate,
+ * whose bilinear weights are NaN, gives NaN in the outputs with a tap inside the level and 0 in the others
+ * (floor(NaN) converts to 0, an infinite or huge floor saturates and leaves every tap outside).  This holds for
+ * every lookup entry point below.
  * ---------------------------------------------------------------------------------- */
 int goslam_corr_index_forward(const void* volume, int dtype, const float* coords,
                               void* corr, int N, int h1, int w1, int h2, int w2,
@@ -86,8 +90,10 @@ int goslam_fmaps_to_kmajor(const void* fmaps, void* out, int F, int D, int h, in
  *
  * layout: GOSLAM_LAYOUT_ROWMAJOR = the reference's [slot,h,w,h>>i,w>>i];
  *         GOSLAM_LAYOUT_TILED    = levels 0 and 1 stored as 4x4-element (32-byte = one DRAM sector)
- *         tiles, tile-row-major inside each source pixel's plane, planes padded with zeros to whole
- *         tiles; levels 2 and 3 as one padded piece per 8-row band of level 0.  Nothing in the
+ *         tiles, tile-row-major inside each source pixel's plane, planes padded to whole tiles; levels 2
+ *         and 3 as one padded piece per 8-row band of level 0.  Padding contents are unspecified (the
+ *         build pools the coarser levels' padding from the finer level's, and skips some of it); the
+ *         lookup never reads them into a result.  Nothing in the
  *         reference outside CorrBlock reads the pyramid, so its layout is private to build + lookup:
  *         the tiled form turns the build's per-thread output into one 128-byte run and cuts the sectors
  *         an 8x8 lookup window touches from ~11.5 to ~7.6.  goslam_corr_level_plane_elems gives the

@@ -5,7 +5,10 @@
                        module imported from /root/reference)
   corr_index_forward   src/lib/correlation_kernels.cu:19-70 — same tap order (x outer, y inner)
                        and the same rounding sequence: fp32 instantiation = chained FMAs,
-                       c10::Half instantiation = every product and every add rounded to half
+                       c10::Half instantiation = every product and every add rounded to half;
+                       a tap outside the level adds nothing (the reference's within_bounds), so a
+                       NaN or infinite coordinate, whose weights are NaN, leaves 0 wherever all
+                       four taps of an output lie outside
   altcorr_forward      src/lib/altcorr_kernel.cu:27-149 (fp32)
 Parity pin: on the GPU box the reference's own CUDA kernels (oracle/_ref) are run on the same
 inputs; here, corr_index_forward is additionally checked against F.grid_sample (SURVEY §8c).
@@ -39,19 +42,22 @@ def corr_build(fmap1, fmap2, num_levels=4):
 
 
 def _gather_taps(volume, coords, r):
-    """taps[n,y,x,i,j] = volume[n,y,x, floor(y0)-r+j, floor(x0)-r+i] or 0 outside."""
+    """taps[n,y,x,i,j] = volume[n,y,x, floor(y0)-r+j, floor(x0)-r+i] or 0 outside, and the mask of the
+    taps inside.  floor(NaN) counts as 0 and huge floors are clamped, as the device's saturating
+    float-to-int conversion treats them (every tap of a clamped coordinate is outside)."""
     N, h1, w1, h2, w2 = volume.shape
     x0 = coords[:, 0].astype(F32)
     y0 = coords[:, 1].astype(F32)
     with np.errstate(invalid="ignore"):
         fx = np.floor(x0)
         fy = np.floor(y0)
-    dx = (x0 - fx).astype(F32)
-    dy = (y0 - fy).astype(F32)
+        dx = (x0 - fx).astype(F32)          # NaN for a NaN or infinite coordinate
+        dy = (y0 - fy).astype(F32)
     fxi = np.clip(np.nan_to_num(fx, nan=0.0), -2 ** 30, 2 ** 30).astype(np.int64)
     fyi = np.clip(np.nan_to_num(fy, nan=0.0), -2 ** 30, 2 ** 30).astype(np.int64)
     rd = 2 * r + 1
     taps = np.zeros((N, h1, w1, rd + 1, rd + 1), volume.dtype)
+    inside = np.zeros(taps.shape, bool)
     nn, yy, xx = np.meshgrid(np.arange(N), np.arange(h1), np.arange(w1), indexing="ij")
     for i in range(rd + 1):
         for j in range(rd + 1):
@@ -60,7 +66,8 @@ def _gather_taps(volume, coords, r):
             ok = (x1 >= 0) & (x1 < w2) & (y1 >= 0) & (y1 < h2)
             v = volume[nn, yy, xx, np.clip(y1, 0, h2 - 1), np.clip(x1, 0, w2 - 1)]
             taps[..., i, j] = np.where(ok, v, 0)
-    return taps, dx, dy
+            inside[..., i, j] = ok
+    return taps, inside, dx, dy
 
 
 def corr_index_forward(volume, coords, r=3):
@@ -69,12 +76,17 @@ def corr_index_forward(volume, coords, r=3):
     coords = np.asarray(coords, F32)
     N, h1, w1, h2, w2 = volume.shape
     rd = 2 * r + 1
-    taps, dx, dy = _gather_taps(volume, coords, r)
+    taps, inside, dx, dy = _gather_taps(volume, coords, r)
     one = F32(1.0)
-    w00 = ((one - dx) * (one - dy)).astype(F32)[..., None, None]
-    w01 = ((one - dx) * dy).astype(F32)[..., None, None]
-    w10 = (dx * (one - dy)).astype(F32)[..., None, None]
-    w11 = (dx * dy).astype(F32)[..., None, None]
+    # an outside tap gets weight 0: it adds +0 where the reference adds nothing.  With finite
+    # coordinates that changes no value (the tap is 0 and the weight finite); with a non-finite one it
+    # keeps 0 * NaN out of the sum.
+    def weight(w, i, j):
+        return np.where(inside[..., i:i + rd, j:j + rd], w.astype(F32)[..., None, None], F32(0))
+    w00 = weight((one - dx) * (one - dy), 0, 0)
+    w01 = weight((one - dx) * dy, 0, 1)
+    w10 = weight(dx * (one - dy), 1, 0)
+    w11 = weight(dx * dy, 1, 1)
     s00 = taps[..., :rd, :rd]
     s01 = taps[..., :rd, 1:]
     s10 = taps[..., 1:, :rd]
