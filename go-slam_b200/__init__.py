@@ -29,10 +29,10 @@ def install(force=True):
 
 
 def __getattr__(name):
-    """goslam_b200.FactorGraph / DepthVideo / MultiviewFilter / MotionFilter / PoseTrajectoryFiller / CorrBlock /
-    AltCorrBlock / BasicEncoder / InstantNeuS, imported on first use"""
+    """goslam_b200.FactorGraph / DepthVideo / Frontend / Backend / MultiviewFilter / MotionFilter /
+    PoseTrajectoryFiller / CorrBlock / AltCorrBlock / BasicEncoder / InstantNeuS, imported on first use"""
     import importlib
-    where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video",
+    where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video", "Frontend": ".frontend", "Backend": ".backend",
              "MultiviewFilter": ".multiview_filter", "MotionFilter": ".motion_filter",
              "PoseTrajectoryFiller": ".trajectory_filler", "CorrBlock": ".modules.corr",
              "AltCorrBlock": ".modules.corr", "BasicEncoder": ".modules.extractor", "InstantNeuS": ".neus"}

@@ -86,6 +86,9 @@ SIGNATURES = {
     "goslam_altcorr_pyramid": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "goslam_frame_distance": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float, c_void_p]),
     "goslam_frame_distance_bidir": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float, c_void_p]),
+    "goslam_frame_distance_grid_workspace_bytes": (c_size_t, [c_int] * 4),
+    "goslam_frame_distance_grid": (c_int, [c_void_p] * 3 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_size_t,
+                                                                        c_void_p]),
     "goslam_projmap": (c_int, [c_void_p] * 7 + [c_int] * 3 + [c_void_p]),
     "goslam_iproj": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
     "goslam_depth_filter": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p]),

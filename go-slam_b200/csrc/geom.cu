@@ -124,6 +124,63 @@ frame_distance_bidir_kernel(const float* __restrict__ poses, const float* __rest
 }
 
 // ---------------------------------------------------------------------------------
+// Banded frame-distance grid: the bidirectional distance over rows [r0, r1) x columns [c0, c1), computed only where
+// j - i <= k (Backend.ba reads nothing else, DESIGN.md §3.18) and +inf elsewhere, straight from the ranges.
+// Row i of the band holds n(i) = clamp(i + k + 1 - c0, 0, W) entries (W = c1 - c0), so the band's first entry of row
+// i sits at S(i) = T(i + a) - T(r0 + a) with a = k + 1 - c0 and T(m) = sum_{t < m} clamp(t, 0, W), and a block finds
+// its row by bisection on S.  Blocks [0, P) each own one band entry (P = S(r1)); blocks [P, P + F) write the +inf.
+// When the mirror (j, i) is in the band too, the block with i < j computes the pair once and writes both entries
+// (0.5 * (d1 + d2) with IEEE addition, which commutes) and the block with i > j has nothing to do.
+// ---------------------------------------------------------------------------------
+struct GridBand {
+  int r0, r1, c0, c1, k;
+  __device__ long long tri(long long m) const {           // T(m)
+    const long long W = c1 - c0;
+    if (m <= 0) return 0;
+    if (m <= W + 1) return m * (m - 1) / 2;
+    return W * (W + 1) / 2 + (m - W - 1) * W;
+  }
+  __device__ long long start(int i) const {               // S(i): band entries in rows [r0, i)
+    const long long a = (long long)k + 1 - c0;
+    return tri(i + a) - tri(r0 + a);
+  }
+  __device__ bool has(int i, int j) const { return i >= r0 && i < r1 && j >= c0 && j < c1 && j - i <= k; }
+};
+
+__global__ void __launch_bounds__(kThreads)
+frame_distance_grid_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
+                           const float* __restrict__ intr, GridBand band, long long n_band, int fill_blocks,
+                           float* __restrict__ dist, int ht, int wd, float beta) {
+  __shared__ float red[kThreads];
+  const long long W = band.c1 - band.c0;
+  const long long b = blockIdx.x;
+  if (b >= n_band) {                                      // +inf outside the band, grid-stride over the matrix
+    const long long n = (long long)(band.r1 - band.r0) * W;
+    const float inf = __int_as_float(0x7f800000);
+    for (long long q = (b - n_band) * kThreads + threadIdx.x; q < n; q += (long long)fill_blocks * kThreads) {
+      const int i = band.r0 + (int)(q / W), j = band.c0 + (int)(q % W);
+      if (j - i > band.k) dist[q] = inf;
+    }
+    return;
+  }
+  int lo = band.r0, hi = band.r1 - 1;                     // largest row i with S(i) <= b (uniform over the block)
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (band.start(mid) <= b) lo = mid; else hi = mid - 1;
+  }
+  const int i = lo, j = band.c0 + (int)(b - band.start(i));
+  const bool mirrored = i != j && band.has(j, i);
+  if (mirrored && i > j) return;
+  const float d1 = pair_distance(poses, disps, intr, i, j, ht, wd, beta, red);
+  const float d2 = pair_distance(poses, disps, intr, j, i, ht, wd, beta, red);
+  if (threadIdx.x == 0) {
+    const float d = __fmul_rn(0.5f, __fadd_rn(d1, d2));
+    dist[(i - band.r0) * W + (j - band.c0)] = d;
+    if (mirrored) dist[(j - band.r0) * W + (i - band.c0)] = d;
+  }
+}
+
+// ---------------------------------------------------------------------------------
 // projmap  (reference: src/lib/droid_kernels.cu:427-516)
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads)
@@ -671,6 +728,46 @@ int goslam_frame_distance_bidir(const float* poses, const float* disps, const fl
   if (K == 0) return GOSLAM_OK;
   frame_distance_bidir_kernel<<<K, kThreads, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, ii, jj, dist, ht,
                                                                         wd, beta);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+size_t goslam_frame_distance_grid_workspace_bytes(int r0, int r1, int c0, int c1) {
+  if (r0 < 0 || c0 < 0 || r1 <= r0 || c1 <= c0) return 0;
+  return gs_align((size_t)7 * std::max(r1, c1) * sizeof(float));
+}
+
+int goslam_frame_distance_grid(const float* poses, const float* disps, const float* intrinsics, int r0, int r1, int c0,
+                               int c1, int k, int ht, int wd, float beta, float* dist, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  if (r0 < 0 || c0 < 0 || r1 < r0 || c1 < c0 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
+  if ((long long)(r1 - r0) * (c1 - c0) > (long long)INT_MAX) return GOSLAM_EINVAL;
+  if (r1 == r0 || c1 == c0) return GOSLAM_OK;
+  if (poses == nullptr || disps == nullptr || intrinsics == nullptr || dist == nullptr) return GOSLAM_EINVAL;
+  const size_t need = goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1);
+  if (workspace == nullptr || workspace_bytes < need) return GOSLAM_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  // the poses of frames [0, max(r1, c1)) as they are when this call reaches the stream: other processes write the
+  // shared pose buffer while a backend pass runs, and every pair must see one consistent set
+  float* snap = static_cast<float*>(workspace);
+  if (cudaMemcpyAsync(snap, poses, (size_t)7 * std::max(r1, c1) * sizeof(float), cudaMemcpyDeviceToDevice, s) !=
+      cudaSuccess) {
+    GS_CHECK_LAUNCH();
+    return GOSLAM_ELAUNCH;
+  }
+  // band size S(r1) on the host (same closed form as GridBand::start)
+  const long long W = c1 - c0, a = (long long)k + 1 - c0;
+  auto tri = [W](long long m) -> long long {
+    if (m <= 0) return 0;
+    if (m <= W + 1) return m * (m - 1) / 2;
+    return W * (W + 1) / 2 + (m - W - 1) * W;
+  };
+  const long long n_band = tri(r1 + a) - tri(r0 + a);
+  const long long n_all = (long long)(r1 - r0) * W;
+  const int fill_blocks = n_band == n_all ? 0 : (int)std::min<long long>((n_all + 4 * kThreads - 1) / (4 * kThreads), 1024);
+  const GridBand band{r0, r1, c0, c1, k};
+  frame_distance_grid_kernel<<<(unsigned)(n_band + fill_blocks), kThreads, 0, s>>>(snap, disps, intrinsics, band, n_band,
+                                                                                  fill_blocks, dist, ht, wd, beta);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

@@ -132,6 +132,29 @@ def frame_distance_bidirectional(poses, disps, intrinsics, ii, jj, beta):
     return dist
 
 
+def frame_distance_grid(poses, disps, intrinsics, r0, r1, c0, c1, k, beta):
+    """Not in the reference module: the distance matrix Backend.ba builds (src/backend.py:31-44) over frames
+    [r0, r1) x [c0, c1) -> Tensor[r1-r0, c1-c0].  Entry (i, j) equals frame_distance_bidirectional of the pair bit for
+    bit where j - i <= k and is +inf elsewhere; no index tensors, and the poses are snapshot on the stream first."""
+    _contig(poses=poses, disps=disps, intrinsics=intrinsics)
+    _need_cuda(poses, disps, intrinsics)
+    r0, r1, c0, c1 = int(r0), int(r1), int(c0), int(c1)
+    if max(r1, c1) > min(poses.shape[0], disps.shape[0]):
+        raise RuntimeError("frame_distance_grid: frame range [%d, %d) x [%d, %d) exceeds the video (%d frames)"
+                           % (r0, r1, c0, c1, min(poses.shape[0], disps.shape[0])))
+    ht, wd = disps.shape[1], disps.shape[2]
+    dist = torch.empty((max(r1 - r0, 0), max(c1 - c0, 0)), dtype=torch.float32, device=poses.device)
+    lib = _lib.load()
+    with torch.cuda.device(poses.device):
+        nbytes = lib.goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1)
+        ws = _workspace(nbytes, poses.device) if nbytes else None
+        rc = lib.goslam_frame_distance_grid(
+            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), r0, r1, c0, c1, int(k), ht, wd, float(beta),
+            _lib.ptr(dist), _lib.ptr(ws), ctypes.c_size_t(0 if ws is None else ws.numel()), _lib.stream_ptr())
+    _lib.check(rc, "frame_distance_grid")
+    return dist
+
+
 def projmap(poses, disps, intrinsics, ii, jj):
     """src/lib/droid.cpp:139-144 -> [coords(N,h,w,3), valid(N,h,w,1)]."""
     _contig(poses=poses, disps=disps, intrinsics=intrinsics, ii=ii, jj=jj)

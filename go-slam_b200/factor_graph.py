@@ -116,6 +116,25 @@ class FactorGraph:
         self.net = None
         self.inp = None
 
+    @torch.no_grad()
+    def adopt_edges(self, other):
+        """take copies of another graph's active edges and their state: ii / jj / age / net / target / weight, each
+        only where `other` has it (what Backend.loop_ba does with setattr + deepcopy, src/backend.py:151-156).  The
+        host mirrors come from `other`'s own when it is a goslam_b200.FactorGraph, otherwise from one device->host
+        copy of its edge lists; `other` is left untouched."""
+        ii, jj, age = (getattr(other, k) for k in ("ii", "jj", "age"))
+        self._set_edges(self.ii if ii is None else ii.clone(), self.jj if jj is None else jj.clone(),
+                        self.age if age is None else age.clone())
+        for k in ("net", "target", "weight"):
+            val = getattr(other, k)
+            if val is not None:
+                setattr(self, k, val.clone())
+        if isinstance(other, FactorGraph):
+            self._h["ii"], self._h["jj"] = other._h["ii"].copy(), other._h["jj"].copy()
+        else:
+            h = torch.stack([self.ii.long(), self.jj.long()]).cpu().numpy()
+            self._h["ii"], self._h["jj"] = h[0].copy(), h[1].copy()
+
     # ------------------------------------------------------------------------------------ edits
     @torch.no_grad()
     def add_factors(self, ii, jj, remove=False):

@@ -149,6 +149,19 @@ int goslam_frame_distance(const float* poses, const float* disps, const float* i
 int goslam_frame_distance_bidir(const float* poses, const float* disps, const float* intrinsics,
                                 const int64_t* ii, const int64_t* jj, float* dist, int K, int ht,
                                 int wd, float beta, void* stream);
+/* Banded bidirectional distance grid for Backend.ba (src/backend.py:31-44) without index tensors:
+ * dist [r1-r0, c1-c0] f32 row-major, entry (i, j) (frames i in [r0, r1), j in [c0, c1)) is
+ * goslam_frame_distance_bidir of the pair, bit for bit, where j - i <= k and +inf elsewhere.
+ * Backend.ba reads nothing else with k = -radius (dense) or k = 2 - radius (loop closure).
+ * The poses of frames [0, max(r1, c1)) are first copied into the workspace on `stream`, so
+ * every pair sees the poses as they were when the call reached the stream.
+ *   Empty ranges are a no-op; negative starts or ends below starts return GOSLAM_EINVAL, as do
+ *   null tensors for a non-empty grid.
+ *   workspace: goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1) (0 for empty ranges). */
+size_t goslam_frame_distance_grid_workspace_bytes(int r0, int r1, int c0, int c1);
+int goslam_frame_distance_grid(const float* poses, const float* disps, const float* intrinsics,
+                               int r0, int r1, int c0, int c1, int k, int ht, int wd, float beta,
+                               float* dist, void* workspace, size_t workspace_bytes, void* stream);
 /* projmap (src/lib/droid_kernels.cu:427-516,1463-1488): coords [K,ht,wd,3] (3rd
  * component left zero, as the reference does), valid [K,ht,wd,1]. */
 int goslam_projmap(const float* poses, const float* disps, const float* intrinsics,
