@@ -35,7 +35,6 @@
 #include "se3.cuh"
 #include <algorithm>
 #include <cstdio>
-#include <mutex>
 #include <cooperative_groups.h>
 
 namespace {
@@ -1588,56 +1587,43 @@ bool make_dims(int N, int num, int ht, int wd, int t0, int t1, BaDims* d) {
 
 constexpr int kSmemSolveMaxN = 160;   // (160*160 + 160) * 8 B = 206 KB of the 227 KB
 constexpr int kWarpSolveMaxN = 96;    // single-warp solve up to 16 poses
-constexpr int kMaxDevices = 64;
 constexpr size_t kClusterSmemMax = 226 * 1024;   // dynamic part of the 227 KB per-CTA opt-in maximum (static: a few bytes)
 
 // Function attributes (opt-in dynamic shared memory) and the occupancy of the cooperative kernel
-// are PER DEVICE: a process that runs BA on a second GPU must set them there too.  One slot per
-// device ordinal, initialised once under a mutex (the C-ABI may be called from several threads).
+// are PER DEVICE: a process that runs BA on a second GPU must set them there too.  ba_setup fills
+// ba_devices[dev] once per device ordinal (gs_device_setup).
 struct BaDevice {
-  bool ready = false;
   int sms = 0;
   int blocks_per_sm = 0;      // 0: cooperative launch unavailable -> multi-kernel driver
 };
+BaDevice ba_devices[kGsMaxDevices];
 
-void ba_persistent_kernel_attrs(BaDevice* dv, int dev) {
+inline size_t prep_smem_bytes(int num) { return ((size_t)3 * num + 1 + 33) * sizeof(int); }
+
+int ba_setup(int dev) {
+  GS_CUDA(cudaFuncSetAttribute(ba_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)prep_smem_bytes(kPrepMaxFrames)));
+  GS_CUDA(cudaFuncSetAttribute(ba_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(((size_t)kSmemSolveMaxN * kSmemSolveMaxN + kSmemSolveMaxN) * 8)));
+  GS_CUDA(cudaFuncSetAttribute(ba_solve_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)(((size_t)kWarpSolveMaxN * kWarpSolveMaxN + 2 * kWarpSolveMaxN) * 8)));
+  GS_CUDA(cudaFuncSetAttribute(ba_solve_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)kClusterSmemMax));
+  BaDevice& dv = ba_devices[dev];
   int occ = 0, coop = 0;
   const size_t smem_max = ((size_t)kWarpSolveMaxN * kWarpSolveMaxN + 2 * kWarpSolveMaxN) * sizeof(double);
-  cudaDeviceGetAttribute(&dv->sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  cudaFuncSetAttribute(ba_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ba_persistent_kernel, kTP, smem_max);
+  GS_CUDA(cudaDeviceGetAttribute(&dv.sms, cudaDevAttrMultiProcessorCount, dev));
+  GS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  GS_CUDA(cudaFuncSetAttribute(ba_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+  GS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ba_persistent_kernel, kTP, smem_max));
 #ifndef GOSLAM_BA_BLOCKS_PER_SM     // build-time A/B switch (tools/build_variant.py), never set in the shipped library
 #define GOSLAM_BA_BLOCKS_PER_SM 2
 #endif
   // 2 blocks/SM (H100 80GB HBM3, 700 W, main leg): 99.8 us per call against 111.9 us with 1 block/SM; the
   // second block halves the linearise rounds and the Schur units per block, which outweighs its barrier arrivals
   constexpr int kWant = GOSLAM_BA_BLOCKS_PER_SM;
-  dv->blocks_per_sm = (!coop || occ < 1) ? 0 : (occ > kWant ? kWant : occ);
-}
-
-inline size_t prep_smem_bytes(int num) { return ((size_t)3 * num + 1 + 33) * sizeof(int); }
-
-const BaDevice& ba_device() {
-  static BaDevice table[kMaxDevices];
-  static std::mutex mu;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= kMaxDevices) dev = 0;
-  std::lock_guard<std::mutex> lock(mu);
-  BaDevice& dv = table[dev];
-  if (!dv.ready) {
-    cudaFuncSetAttribute(ba_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prep_smem_bytes(kPrepMaxFrames));
-    cudaFuncSetAttribute(ba_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)(((size_t)kSmemSolveMaxN * kSmemSolveMaxN + kSmemSolveMaxN) * 8));
-    cudaFuncSetAttribute(ba_solve_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)(((size_t)kWarpSolveMaxN * kWarpSolveMaxN + 2 * kWarpSolveMaxN) * 8));
-    cudaFuncSetAttribute(ba_solve_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)kClusterSmemMax);
-    ba_persistent_kernel_attrs(&dv, dev);
-    dv.ready = true;
-  }
-  return dv;
+  dv.blocks_per_sm = (!coop || occ < 1) ? 0 : (occ > kWant ? kWant : occ);
+  return GOSLAM_OK;
 }
 
 
@@ -1650,7 +1636,7 @@ int launch_phase1(const float* poses, const float* disps, const float* intr,
     ba_prep_kernel<<<1, kPrepThreads, prep_smem_bytes(d.num), st>>>(ii, jj, d, ws, 0, motion_only ? 0 : eta_rows);
     GS_CHECK_LAUNCH();
   }
-  cudaMemsetAsync(ws.sys, 0, ((size_t)d.n * d.n + d.n) * sizeof(double), st);
+  GS_CUDA(cudaMemsetAsync(ws.sys, 0, ((size_t)d.n * d.n + d.n) * sizeof(double), st));
   if (d.N > 0) {
     dim3 grid(ws.ntiles, d.num);
     ba_linearize_kernel<<<grid, kTP, 0, st>>>(in, d, ws, motion_only);
@@ -1669,8 +1655,8 @@ int launch_phase2(float* poses, float* disps, const SysSrc& sys_in,
                   const BaDims& d, const BaWs& ws, float lm, float ep, int motion_only,
                   int owner_lo, int owner_hi, float* dx_out, float* dz_out, int* status_out,
                   cudaStream_t st, const PeerRows& peer_rows = PeerRows{}) {
-  const BaDevice& dv = ba_device();    // per-device function attributes are set on first use
-  (void)dv;
+  const int rc = gs_device_setup<ba_setup>();    // per-device function attributes are set on first use
+  if (rc) return rc;
   if (d.n <= kWarpSolveMaxN) {
     const size_t smem = ((size_t)d.n * d.n + 2 * d.n) * sizeof(double);
     ba_solve_warp_kernel<<<1, 128, smem, st>>>(poses, d, ws, sys_in, lm, ep, dx_out, status_out);
@@ -1687,9 +1673,8 @@ int launch_phase2(float* poses, float* disps, const SysSrc& sys_in,
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     const int rows_doubles = (int)cl_rows_doubles(d.P);
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, ba_solve_cluster_kernel, poses, d, ws, sys_in, lm, ep,
-                                              rows_doubles, dx_out, status_out);
-    if (le != cudaSuccess) { gs_note_cuda_error(le); return GOSLAM_ELAUNCH; }
+    GS_CUDA(cudaLaunchKernelEx(&cfg, ba_solve_cluster_kernel, poses, d, ws, sys_in, lm, ep, rows_doubles, dx_out,
+                               status_out));
   } else {
     const int use_smem = d.n <= kSmemSolveMaxN;
     const size_t smem = use_smem ? ((size_t)d.n * d.n + d.n) * sizeof(double) : 0;
@@ -1741,8 +1726,10 @@ int goslam_ba(float* poses, float* disps, const float* intrinsics, const float* 
   constexpr bool multi_kernel = false;
 #endif
   if (d.n <= kWarpSolveMaxN && !multi_kernel) {
-    const BaDevice& dv = ba_device();
-    const int blocks_per_sm = dv.blocks_per_sm, sms = dv.sms;
+    int dev = 0;
+    const int rc = gs_device_setup<ba_setup>(&dev);
+    if (rc) return rc;
+    const int blocks_per_sm = ba_devices[dev].blocks_per_sm, sms = ba_devices[dev].sms;
     const size_t smem = ((size_t)d.n * d.n + 2 * d.n) * sizeof(double);
     if (blocks_per_sm > 0) {
       // two launches per call: the table kernel (which also zeroes the first reduced system and the
@@ -1757,13 +1744,12 @@ int goslam_ba(float* poses, float* disps, const float* intrinsics, const float* 
       BaWs wsv = ws;
       void* args[] = {&poses, &disps, &in, &dd, &wsv, &iterations, &lm, &ep, &motion_only,
                       &dx_out, &dz_out, &status_out, &barrier, &arrived, &solved};
-      const cudaError_t le = cudaLaunchCooperativeKernel((const void*)ba_persistent_kernel,
-                                                         dim3(sms * blocks_per_sm), dim3(kTP), args, smem, st);
-      if (le != cudaSuccess) { gs_note_cuda_error(le); return GOSLAM_ELAUNCH; }
+      GS_CUDA(cudaLaunchCooperativeKernel((const void*)ba_persistent_kernel, dim3(sms * blocks_per_sm), dim3(kTP), args,
+                                          smem, st));
       return GOSLAM_OK;
     }
   }
-  if (dz_out) cudaMemsetAsync(dz_out, 0, (size_t)num * d.hw * sizeof(float), st);
+  if (dz_out) GS_CUDA(cudaMemsetAsync(dz_out, 0, (size_t)num * d.hw * sizeof(float), st));
   for (int it = 0; it < iterations; ++it) {
     int rc = launch_phase1(poses, disps, intrinsics, disps_sens, targets, weights, eta, eta_rows,
                            ii, jj, d, ws, motion_only, it == 0, st);
@@ -1793,8 +1779,7 @@ int goslam_ba_phase1(const float* poses, const float* disps, const float* intrin
                          jj, d, ws, motion_only, true, st);
   if (rc) return rc;
   if (system != ws.sys)
-    cudaMemcpyAsync(system, ws.sys, ((size_t)d.n * d.n + d.n) * sizeof(double),
-                    cudaMemcpyDeviceToDevice, st);
+    GS_CUDA(cudaMemcpyAsync(system, ws.sys, ((size_t)d.n * d.n + d.n) * sizeof(double), cudaMemcpyDeviceToDevice, st));
   return GOSLAM_OK;
 }
 
@@ -1843,7 +1828,8 @@ int goslam_ba_phase1_peers(const float* poses, const float* intrinsics, const fl
                          motion_only, true, st);
   if (rc) return rc;
   if (peers->system[me] != ws.sys)
-    cudaMemcpyAsync(peers->system[me], ws.sys, ((size_t)d.n * d.n + d.n) * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    GS_CUDA(cudaMemcpyAsync(peers->system[me], ws.sys, ((size_t)d.n * d.n + d.n) * sizeof(double),
+                            cudaMemcpyDeviceToDevice, st));
   // (2) publish: my partial system of iteration `epoch` is complete
   if (W > 1) {
     PeerRows rows{};
@@ -1911,8 +1897,7 @@ int goslam_peer_alloc(size_t bytes, void** ptr, void* handle_out) {
 
 int goslam_peer_free(void* ptr) {
   if (!ptr) return GOSLAM_EINVAL;
-  const cudaError_t e = cudaFree(ptr);
-  if (e != cudaSuccess) { gs_note_cuda_error(e); return GOSLAM_ELAUNCH; }
+  GS_CUDA(cudaFree(ptr));
   return GOSLAM_OK;
 }
 
@@ -1920,15 +1905,13 @@ int goslam_ipc_open(const void* handle, void** ptr) {
   if (!handle || !ptr) return GOSLAM_EINVAL;
   cudaIpcMemHandle_t h;
   memcpy(&h, handle, sizeof(h));
-  const cudaError_t e = cudaIpcOpenMemHandle(ptr, h, cudaIpcMemLazyEnablePeerAccess);
-  if (e != cudaSuccess) { gs_note_cuda_error(e); return GOSLAM_ELAUNCH; }
+  GS_CUDA(cudaIpcOpenMemHandle(ptr, h, cudaIpcMemLazyEnablePeerAccess));
   return GOSLAM_OK;
 }
 
 int goslam_ipc_close(void* ptr) {
   if (!ptr) return GOSLAM_EINVAL;
-  const cudaError_t e = cudaIpcCloseMemHandle(ptr);
-  if (e != cudaSuccess) { gs_note_cuda_error(e); return GOSLAM_ELAUNCH; }
+  GS_CUDA(cudaIpcCloseMemHandle(ptr));
   return GOSLAM_OK;
 }
 

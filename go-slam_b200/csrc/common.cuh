@@ -1,8 +1,10 @@
 // common.cuh — shared device/host helpers for libgoslam_b200 (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include <mutex>
 #include "goslam_b200.h"
 
 // Streaming-multiprocessor count of the H100 SXM: grid size of the persistent kernels and of the fixed-grid
@@ -19,6 +21,77 @@ void gs_note_cuda_error(cudaError_t e);
     cudaError_t e__ = cudaGetLastError();                        \
     if (e__ != cudaSuccess) { gs_note_cuda_error(e__); return GOSLAM_ELAUNCH; } \
   } while (0)
+
+// Evaluates a CUDA runtime or CUB call; if it fails, notes its error and returns GOSLAM_ELAUNCH.  The runtime's copy
+// of the error is cleared, so a later GS_CHECK_LAUNCH (maybe in another entry point) does not report it again.
+#define GS_CUDA(expr)                                            \
+  do {                                                           \
+    const cudaError_t e__ = (expr);                              \
+    if (e__ != cudaSuccess) { (void)cudaGetLastError(); gs_note_cuda_error(e__); return GOSLAM_ELAUNCH; } \
+  } while (0)
+
+// host helpers shared by the .cu files (api.cu); hidden, so that the library exports only its C-ABI
+#define GS_HIDDEN __attribute__((visibility("hidden")))
+
+// Function attributes, occupancy and constant memory are per device.  gs_device_setup<Setup>() runs Setup(dev) on the
+// current device unless it has already succeeded there, and returns its GOSLAM_* code; thread-safe.  A failed setup
+// is not remembered, so the next call tries again.  No current device, or an ordinal of kGsMaxDevices or more, gives
+// GOSLAM_ELAUNCH with the CUDA error noted.  dev_out, if given, receives the ordinal.
+constexpr int kGsMaxDevices = 64;
+GS_HIDDEN int gs_device_setup_once(int (*setup)(int dev), bool* done, int* dev_out);
+template <int (*Setup)(int dev)>
+int gs_device_setup(int* dev_out = nullptr) {
+  static bool done[kGsMaxDevices];
+  return gs_device_setup_once(Setup, done, dev_out);
+}
+
+// multiprocessor count of the current device, read once per device; fails as gs_device_setup
+GS_HIDDEN int gs_sm_count(int* sms);
+
+// cuTensorMapEncodeTiled, looked up from the driver once per process (thread-safe); GOSLAM_ELAUNCH, error noted, if
+// the driver lacks it
+typedef CUresult (*GsEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+GS_HIDDEN int gs_encode_tiled(GsEncodeTiled* fn);
+
+// Tensor maps depend only on what the caller's Key holds (a base pointer, a shape, a kind), and launches use the same
+// buffers call after call, so each map is encoded once (~2 us of host time) and kept in a most-recently-used table of
+// Slots entries shared by all threads.  Encode makes the map of a key; Key needs ==.
+template <typename Key, int Slots, bool (*Encode)(GsEncodeTiled, const Key&, CUtensorMap*)>
+class GsTensorMapCache {
+ public:
+  // false, with the CUDA error noted, when the map cannot be made
+  bool get(const Key& k, CUtensorMap* out) {
+    std::lock_guard<std::mutex> lock(mu_);
+    int victim = -1;
+    for (int i = 0; i < Slots; ++i) {
+      Slot& s = table_[i];
+      if (s.used && s.key == k) {
+        s.stamp = ++clock_;
+        *out = s.map;
+        return true;
+      }
+      // victim: a free slot if there is one, else the least recently used
+      if (victim < 0 || (table_[victim].used && (!s.used || s.stamp < table_[victim].stamp))) victim = i;
+    }
+    Slot& v = table_[victim];
+    v.used = false;
+    GsEncodeTiled enc;
+    if (gs_encode_tiled(&enc) != GOSLAM_OK) return false;
+    // the encoder returns a driver CUresult, not a runtime error: report a rejected encode as an invalid argument
+    if (!Encode(enc, k, &v.map)) { gs_note_cuda_error(cudaErrorInvalidValue); return false; }
+    v.key = k; v.used = true; v.stamp = ++clock_;
+    *out = v.map;
+    return true;
+  }
+
+ private:
+  struct Slot { Key key; CUtensorMap map; unsigned long long stamp; bool used; };
+  Slot table_[Slots] = {};
+  unsigned long long clock_ = 0;
+  std::mutex mu_;
+};
 
 __host__ __device__ static inline int gs_cdiv(int a, int b) { return (a + b - 1) / b; }
 #define gs_cdiv_dev gs_cdiv

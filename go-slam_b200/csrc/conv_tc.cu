@@ -31,7 +31,6 @@
 // oracle/update_oracle.py (round16=True) restates this in float64.
 #include "common.cuh"
 #include "tc_ptx.cuh"
-#include <mutex>
 
 using namespace gs_tc;
 
@@ -533,63 +532,30 @@ scatter_mean_kernel(const __half* __restrict__ a1, const int* __restrict__ slot,
   *reinterpret_cast<uint4*>(mean + ((size_t)m * hw + px) * 128 + c8 * 8) = *reinterpret_cast<const uint4*>(o);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn conv_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* ptr = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) != cudaSuccess ||
-      q != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  return fn;
-}
-
 // Tensor maps depend only on (base pointer, shape): the update operator runs the same layers on the same workspace
 // buffers call after call, so the driver's encode (~1.5 us of host time each, ~50 per operator call) is cached.
-struct CMapKey { const void* base; int a, b, c, d, kind; };
-struct CMapSlot { CMapKey key; CUtensorMap map; unsigned long long stamp; bool used; };
-constexpr int kCMapSlots = 128;
-bool act_map_raw(EncodeTiledFn enc, const void* base, int B, int h, int w, int C, CUtensorMap* out);
-bool weight_map_raw(EncodeTiledFn enc, const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile);
-
-bool cached_cmap(EncodeTiledFn enc, const CMapKey& k, CUtensorMap* out) {
-  static CMapSlot table[kCMapSlots];
-  static unsigned long long clock = 0;
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
-  int victim = -1;
-  for (int i = 0; i < kCMapSlots; ++i) {
-    CMapSlot& s = table[i];
-    if (s.used && s.key.base == k.base && s.key.a == k.a && s.key.b == k.b && s.key.c == k.c && s.key.d == k.d &&
-        s.key.kind == k.kind) {
-      s.stamp = ++clock;
-      *out = s.map;
-      return true;
-    }
-    if (victim < 0 || (table[victim].used && (!s.used || s.stamp < table[victim].stamp))) victim = i;
+struct CMapKey {
+  const void* base; int a, b, c, d, kind;
+  bool operator==(const CMapKey& o) const {
+    return base == o.base && a == o.a && b == o.b && c == o.c && d == o.d && kind == o.kind;
   }
-  CMapSlot& v = table[victim];
-  const bool ok = k.kind == 0 ? act_map_raw(enc, k.base, k.a, k.b, k.c, k.d, &v.map)
-                              : weight_map_raw(enc, k.base, k.a, k.b, k.c, &v.map, k.d);
-  if (!ok) { v.used = false; return false; }
-  v.key = k; v.used = true; v.stamp = ++clock;
-  *out = v.map;
-  return true;
+};
+bool act_map_raw(GsEncodeTiled enc, const void* base, int B, int h, int w, int C, CUtensorMap* out);
+bool weight_map_raw(GsEncodeTiled enc, const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile);
+bool encode_cmap(GsEncodeTiled enc, const CMapKey& k, CUtensorMap* out) {
+  return k.kind == 0 ? act_map_raw(enc, k.base, k.a, k.b, k.c, k.d, out)
+                     : weight_map_raw(enc, k.base, k.a, k.b, k.c, out, k.d);
 }
-bool act_map(EncodeTiledFn enc, const void* base, int B, int h, int w, int C, CUtensorMap* out) {
-  return cached_cmap(enc, CMapKey{base, B, h, w, C, 0}, out);
+GsTensorMapCache<CMapKey, 128, encode_cmap> g_cmaps;
+bool act_map(const void* base, int B, int h, int w, int C, CUtensorMap* out) {
+  return g_cmaps.get(CMapKey{base, B, h, w, C, 0}, out);
 }
-bool weight_map(EncodeTiledFn enc, const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile = 0) {
-  return cached_cmap(enc, CMapKey{base, taps, N, Cin, n_tile, 1}, out);
+bool weight_map(const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile = 0) {
+  return g_cmaps.get(CMapKey{base, taps, N, Cin, n_tile, 1}, out);
 }
 
 // activation map: NHWC [B, h, w, C] as (ch, x, y, image), box 64 ch x 16 x 8
-bool act_map_raw(EncodeTiledFn enc, const void* base, int B, int h, int w, int C, CUtensorMap* out) {
+bool act_map_raw(GsEncodeTiled enc, const void* base, int B, int h, int w, int C, CUtensorMap* out) {
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)w * C * 2, (cuuint64_t)h * w * C * 2};
   cuuint32_t box[4] = {(cuuint32_t)kKC, (cuuint32_t)kPX, (cuuint32_t)kPY, 1};
@@ -599,7 +565,7 @@ bool act_map_raw(EncodeTiledFn enc, const void* base, int B, int h, int w, int C
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 // weight map: [taps, N, Cin] as (cin, cout, tap), box 64 x N
-bool weight_map_raw(EncodeTiledFn enc, const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile) {
+bool weight_map_raw(GsEncodeTiled enc, const void* base, int taps, int N, int Cin, CUtensorMap* out, int n_tile) {
   cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)N, (cuuint64_t)taps};
   cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)N * Cin * 2};
   cuuint32_t box[3] = {(cuuint32_t)kKC, (cuuint32_t)(n_tile > 0 ? n_tile : N), 1};
@@ -611,42 +577,27 @@ bool weight_map_raw(EncodeTiledFn enc, const void* base, int taps, int N, int Ci
 
 // one instantiation per output-channel tile width N = 16, 32, .., 256
 template <int N>
+int conv_setup(int) {
+  GS_CUDA(cudaFuncSetAttribute(conv_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemC));
+  return GOSLAM_OK;
+}
+template <int N>
 int conv_launch_n(const ConvMaps& maps, const ConvParams& p, int grid, cudaStream_t st) {
-  static bool attr_set[64];
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (!attr_set[dev]) {
-    if (cudaFuncSetAttribute(conv_tc_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemC) != cudaSuccess)
-      return GOSLAM_ELAUNCH;
-    attr_set[dev] = true;
-  }
+  const int rc = gs_device_setup<conv_setup<N>>();
+  if (rc) return rc;
   conv_tc_kernel<N><<<grid, kThreadsC, kSmemC, st>>>(maps, p);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }
 
 int conv_launch(const ConvMaps& maps, ConvParams p, cudaStream_t st) {
-  static int sm_count[64];
-  static std::mutex mu;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  int sms;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (sm_count[dev] == 0) {
-      int n = kNumSms;
-      cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-      sm_count[dev] = n > 0 ? n : kNumSms;
-    }
-    sms = sm_count[dev];
-  }
+  int sms = 0;
+  const int rc = gs_sm_count(&sms);
+  if (rc) return rc;
   p.n_yb = gs_cdiv(p.h, kPY); p.n_xb = gs_cdiv(p.w, kPX);
   if (p.n_nt < 1) p.n_nt = 1;
   p.n_tiles = p.B * p.n_yb * p.n_xb * p.n_nt;
   const int grid = p.n_tiles < sms ? p.n_tiles : sms;
-  std::lock_guard<std::mutex> lock(mu);
   switch (p.N) {
     case 16: return conv_launch_n<16>(maps, p, grid, st);
     case 32: return conv_launch_n<32>(maps, p, grid, st);
@@ -666,6 +617,11 @@ int conv_launch(const ConvMaps& maps, ConvParams p, cudaStream_t st) {
     case 256: return conv_launch_n<256>(maps, p, grid, st);
     default: return GOSLAM_EINVAL;
   }
+}
+
+int flow7x7_setup(int) {
+  GS_CUDA(cudaFuncSetAttribute(flow7x7_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kF7Smem));
+  return GOSLAM_OK;
 }
 
 struct GruWs {
@@ -728,8 +684,6 @@ int goslam_conv2d_nhwc(const goslam_conv_desc* d, int B, int h, int w, void* str
   // the epilogue stages the whole bias vector in shared memory
   if (d->cout_pad % N || d->cout_pad > kVecMax) return GOSLAM_EINVAL;
   if (B == 0) return GOSLAM_OK;
-  EncodeTiledFn enc = conv_encode_fn();
-  if (!enc) return GOSLAM_ELAUNCH;
   ConvMaps m{};
   ConvParams p{};
   p.B = B; p.h = h; p.w = w; p.taps = d->taps; p.n_in = d->n_in; p.N = N; p.n_nt = d->cout_pad / N;
@@ -738,9 +692,9 @@ int goslam_conv2d_nhwc(const goslam_conv_desc* d, int B, int h, int w, void* str
     if (d->cin[i] <= 0 || d->cin[i] % kKC || d->cin_off[i] % kKC || d->cin_stride[i] < d->cin_off[i] + d->cin[i]) return GOSLAM_EINVAL;
     p.chunks[i] = d->cin[i] / kKC; p.coff[i] = d->cin_off[i];
     cin_total += d->cin[i];
-    if (!act_map(enc, d->in[i], B, h, w, d->cin_stride[i], &m.in[i])) return GOSLAM_ELAUNCH;
+    if (!act_map(d->in[i], B, h, w, d->cin_stride[i], &m.in[i])) return GOSLAM_ELAUNCH;
   }
-  if (!weight_map(enc, d->weight, d->taps, d->cout_pad, cin_total, &m.w, N)) return GOSLAM_ELAUNCH;
+  if (!weight_map(d->weight, d->taps, d->cout_pad, cin_total, &m.w, N)) return GOSLAM_ELAUNCH;
   p.epi = EPI_ACT; p.bias = d->bias; p.act = d->act; p.cout = d->cout; p.out = d->out; p.out_f32 = d->out_f32;
   p.out_stride = d->out_stride; p.out_offset = d->out_offset; p.out_scale = d->out_scale;
   p.split = d->split; p.act2 = d->act2; p.out2 = d->out2;
@@ -830,26 +784,12 @@ int goslam_update_op(const goslam_update_weights* W, const void* net, const void
   GS_TRY(layer(ws.c1, 128, 0, 128, W->corr2_w, W->corr2_b, 9, 128, 128, ACT_RELU, 1.f, ws.c2, 0, 128, N, h, w, stream));
   {
     // 7x7 motion encoder: im2col + wgmma (flow0_w f16 [128][256], K = (ky*7+kx)*4 + ci, zero beyond 196)
-    EncodeTiledFn enc = conv_encode_fn();
     CUtensorMap wm;
-    if (!enc || !weight_map(enc, W->flow0_w, 1, 128, kF7K, &wm, 128)) return GOSLAM_ELAUNCH;
-    static int sm_count[64];
-    static std::mutex mu;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    int sms;
-    {
-      std::lock_guard<std::mutex> lock(mu);
-      if (sm_count[dev] == 0) {
-        if (cudaFuncSetAttribute(flow7x7_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kF7Smem) != cudaSuccess)
-          return GOSLAM_ELAUNCH;
-        int n = kNumSms;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sm_count[dev] = n > 0 ? n : kNumSms;
-      }
-      sms = sm_count[dev];
-    }
+    if (!weight_map(W->flow0_w, 1, 128, kF7K, &wm, 128)) return GOSLAM_ELAUNCH;
+    int sms = 0;
+    rc = gs_device_setup<flow7x7_setup>();
+    if (rc == GOSLAM_OK) rc = gs_sm_count(&sms);
+    if (rc) return rc;
     const int n_tiles = N * gs_cdiv(h, kPY) * gs_cdiv(w, kPX);
     flow7x7_tc_kernel<<<n_tiles < sms ? n_tiles : sms, kF7Threads, kF7Smem, st>>>(wm, flow, W->flow0_b, ws.f1, N, h, w);
     GS_CHECK_LAUNCH();
@@ -893,15 +833,13 @@ int goslam_conv_gru(const goslam_gru_weights* wts, const void* net, const void* 
   GruWs ws;
   const size_t need = gru_layout(B, h, w, workspace, workspace_bytes, &ws);
   if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
-  EncodeTiledFn enc = conv_encode_fn();
-  if (!enc) return GOSLAM_ELAUNCH;
   cudaStream_t st = (cudaStream_t)stream;
   ConvMaps m{};
   ConvParams p{};
   p.B = B; p.h = h; p.w = w;
   p.net = reinterpret_cast<const __half*>(net);
   // ---- pass G: glo_sum = sum_px sigmoid(w(net)) * net
-  if (!act_map(enc, net, B, h, w, 128, &m.in[0]) || !weight_map(enc, wts->w_w, 1, 128, 128, &m.w)) return GOSLAM_ELAUNCH;
+  if (!act_map(net, B, h, w, 128, &m.in[0]) || !weight_map(wts->w_w, 1, 128, 128, &m.w)) return GOSLAM_ELAUNCH;
   p.n_nt = 1;
   p.taps = 1; p.n_in = 1; p.chunks[0] = 2; p.N = 128; p.epi = EPI_GLO; p.bias = wts->b_w; p.glo = nullptr;
   p.glo_sum = ws.glo_sum;
@@ -911,15 +849,15 @@ int goslam_conv_gru(const goslam_gru_weights* wts, const void* net, const void* 
                                        1.0f / (float)(h * w));
   GS_CHECK_LAUNCH();
   // ---- pass ZR: z, r*net
-  if (!act_map(enc, inp, B, h, w, 128, &m.in[1]) || !act_map(enc, corr, B, h, w, 128, &m.in[2]) ||
-      !act_map(enc, flow, B, h, w, 64, &m.in[3]) || !weight_map(enc, wts->w_zr, 9, 256, 448, &m.w))
+  if (!act_map(inp, B, h, w, 128, &m.in[1]) || !act_map(corr, B, h, w, 128, &m.in[2]) ||
+      !act_map(flow, B, h, w, 64, &m.in[3]) || !weight_map(wts->w_zr, 9, 256, 448, &m.w))
     return GOSLAM_ELAUNCH;
   p.taps = 9; p.n_in = 4; p.chunks[0] = 2; p.chunks[1] = 2; p.chunks[2] = 2; p.chunks[3] = 1;
   p.N = 256; p.epi = EPI_ZR; p.bias = wts->b_zr; p.glo = ws.glo; p.z_out = ws.z; p.rnet_out = ws.rnet;
   rc = conv_launch(m, p, st);
   if (rc) return rc;
   // ---- pass Q: net' = (1 - z) net + z tanh(convq([r*net | inp | corr | flow]) + glo_q)
-  if (!act_map(enc, ws.rnet, B, h, w, 128, &m.in[0]) || !weight_map(enc, wts->w_q, 9, 128, 448, &m.w)) return GOSLAM_ELAUNCH;
+  if (!act_map(ws.rnet, B, h, w, 128, &m.in[0]) || !weight_map(wts->w_q, 9, 128, 448, &m.w)) return GOSLAM_ELAUNCH;
   p.N = 128; p.epi = EPI_Q; p.bias = wts->b_q; p.z_in = ws.z; p.net_out = reinterpret_cast<__half*>(net_out);
   return conv_launch(m, p, st);
 }

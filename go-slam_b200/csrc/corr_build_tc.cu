@@ -34,7 +34,6 @@
 // re-layout prepass, exactly as the reference does it, so the accumulator needs no scaling.
 #include "common.cuh"
 #include "tc_ptx.cuh"
-#include <mutex>
 #include <cstdio>
 #include <cuda.h>
 #include <cstdlib>
@@ -481,33 +480,19 @@ to_kmajor_kernel(const __half* __restrict__ in, __half* __restrict__ out, int hw
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-      q != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<EncodeTiledFn>(p);
-  return fn;
-}
-
 // Tensor maps depend only on (base pointer, frame count, h, w, kind): a factor graph builds from the same
 // video-level K-major buffer into the same slot pool for its whole life, so the cuTensorMapEncodeTiled driver
 // calls of a launch (~2 us of host time each) are paid once.  Small most-recently-used table, shared by all
 // threads.  kind: 0 = A operand, 1 = B operand, 2 .. 5 = tiled level 0 .. 3 output (F unused).  A tiled launch
 // needs six maps, so the table holds those of a few pools at once.
-struct MapKey { const void* base; int F, h, w, kind; };
-struct MapSlot { MapKey key; CUtensorMap map; unsigned long long stamp; bool used; };
-constexpr int kMapSlots = 32;
+struct MapKey {
+  const void* base; int F, h, w, kind;
+  bool operator==(const MapKey& o) const {
+    return base == o.base && F == o.F && h == o.h && w == o.w && kind == o.kind;
+  }
+};
 
-bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
+bool encode_map(GsEncodeTiled enc, const MapKey& k, CUtensorMap* out) {
   const cuuint64_t hw = (cuuint64_t)k.h * k.w;
   if (k.kind == 0) {           // A: [F, hw, 128] as (ch, pixel, frame), box 64 ch x 128 pixels
     cuuint64_t dims[3] = {(cuuint64_t)kD, hw, (cuuint64_t)k.F};
@@ -568,46 +553,28 @@ bool encode_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-bool cached_map(EncodeTiledFn enc, const MapKey& k, CUtensorMap* out) {
-  static MapSlot table[kMapSlots];
-  static unsigned long long clock = 0;
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
-  int victim = -1;
-  for (int i = 0; i < kMapSlots; ++i) {
-    MapSlot& s = table[i];
-    if (s.used && s.key.base == k.base && s.key.F == k.F && s.key.h == k.h && s.key.w == k.w &&
-        s.key.kind == k.kind) {
-      s.stamp = ++clock;
-      *out = s.map;
-      return true;
-    }
-    // victim: a free slot if there is one, else the least recently used
-    if (victim < 0 || (table[victim].used && (!s.used || s.stamp < table[victim].stamp))) victim = i;
-  }
-  MapSlot& v = table[victim];
-  if (!encode_map(enc, k, &v.map)) { v.used = false; return false; }
-  v.key = k; v.used = true; v.stamp = ++clock;
-  *out = v.map;
-  return true;
+GsTensorMapCache<MapKey, 32, encode_map> g_maps;
+
+// opt-in dynamic shared memory is a per-device function attribute (gs_device_setup)
+int corr_build_setup(int) {
+  GS_CUDA(cudaFuncSetAttribute(corr_build_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(kMaxXB)));
+  return GOSLAM_OK;
 }
 
 // launch the tensor-core kernel on the video-level K-major (pre-scaled) feature maps f = [F, hw, 128]
 int launch_tc(const __half* f, int F, const int64_t* ii, const int64_t* jj, int rig, const int* out_slot,
               __half* const* levels, int num_levels, int N, int h, int w, cudaStream_t st) {
   const int hw = h * w;
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return GOSLAM_ELAUNCH;
   // the tensor stores need 16-byte aligned level buffers
   for (int i = 0; i < num_levels; ++i)
     if (reinterpret_cast<uintptr_t>(levels[i]) & 15) return GOSLAM_EINVAL;
   CUtensorMap mapA, mapB, mapL0, mapL1, mapL2, mapL3;
-  if (!cached_map(enc, MapKey{f, F, h, w, 0}, &mapA) || !cached_map(enc, MapKey{f, F, h, w, 1}, &mapB))
+  if (!g_maps.get(MapKey{f, F, h, w, 0}, &mapA) || !g_maps.get(MapKey{f, F, h, w, 1}, &mapB))
     return GOSLAM_ELAUNCH;
   mapL0 = mapL1 = mapL2 = mapL3 = mapA;      // the maps of levels >= num_levels are unused
   CUtensorMap* maps[4] = {&mapL0, &mapL1, &mapL2, &mapL3};
   for (int i = 0; i < num_levels; ++i)
-    if (!cached_map(enc, MapKey{levels[i], 0, h, w, 2 + i}, maps[i])) return GOSLAM_ELAUNCH;
+    if (!g_maps.get(MapKey{levels[i], 0, h, w, 2 + i}, maps[i])) return GOSLAM_ELAUNCH;
   TcParams p{};
   p.num_levels = num_levels; p.N = N; p.h = h; p.w = w; p.hw = hw;
   p.n_mt = gs_cdiv(hw, kBM); p.n_yb = gs_cdiv(h, kPY); p.n_xb = gs_cdiv(w, kPX);
@@ -616,25 +583,10 @@ int launch_tc(const __half* f, int F, const int64_t* ii, const int64_t* jj, int 
   p.w4_0 = gs_cdiv(w, 4); p.h4_0 = gs_cdiv(h, 4);
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
   p.pitch2 = pitch2_of(p.n_xb); p.pitch3 = 32;
-  // per-device: opt-in shared memory + SM count, looked up once per device
-  static int sm_count[64];
-  static std::mutex dev_mu;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  int sms;
-  {
-    std::lock_guard<std::mutex> lock(dev_mu);
-    if (sm_count[dev] == 0) {
-      if (cudaFuncSetAttribute(corr_build_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               smem_bytes(kMaxXB)) != cudaSuccess)
-        return GOSLAM_ELAUNCH;
-      int n = kNumSms;
-      cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-      sm_count[dev] = n > 0 ? n : kNumSms;
-    }
-    sms = sm_count[dev];
-  }
+  int sms = 0;
+  int rc = gs_device_setup<corr_build_setup>();
+  if (rc == GOSLAM_OK) rc = gs_sm_count(&sms);
+  if (rc) return rc;
   const int grid = p.n_items < sms ? p.n_items : sms;
   corr_build_tc_kernel<<<grid, kThreadsTC, smem_bytes(p.n_xb), st>>>(mapA, mapB, mapL0, mapL1, mapL2, mapL3, p);
   GS_CHECK_LAUNCH();

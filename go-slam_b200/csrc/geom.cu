@@ -696,6 +696,7 @@ struct MapPointOp {
 
 using MapIter = cub::TransformInputIterator<MapPoint3, MapPointOp, cub::CountingInputIterator<long long>>;
 
+// a failed size query is reported by the select call itself (GS_CUDA)
 size_t map_select_tmp(long long n) {
   size_t t = 0;
   cub::DeviceSelect::Flagged(nullptr, t, MapIter(cub::CountingInputIterator<long long>(0), MapPointOp{}),
@@ -750,11 +751,7 @@ int goslam_frame_distance_grid(const float* poses, const float* disps, const flo
   // the poses of frames [0, max(r1, c1)) as they are when this call reaches the stream: other processes write the
   // shared pose buffer while a backend pass runs, and every pair must see one consistent set
   float* snap = static_cast<float*>(workspace);
-  if (cudaMemcpyAsync(snap, poses, (size_t)7 * std::max(r1, c1) * sizeof(float), cudaMemcpyDeviceToDevice, s) !=
-      cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cudaMemcpyAsync(snap, poses, (size_t)7 * std::max(r1, c1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
   // band size S(r1) on the host (same closed form as GridBand::start)
   const long long W = c1 - c0, a = (long long)k + 1 - c0;
   auto tri = [W](long long m) -> long long {
@@ -906,10 +903,7 @@ int goslam_mapping_points_count(const float* poses, const float* poses_world, co
   mv_vote_kernel<<<dim3(gs_cdiv(hw, kMvTile), T), kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, mean,
                                                                      kMapThresh, kMapVisible, mask1, st, T, ht, wd);
   GS_CHECK_LAUNCH();
-  if (cudaMemcpyAsync(count, &st->n1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cudaMemcpyAsync(count, &st->n1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
   return GOSLAM_OK;
 }
 
@@ -929,12 +923,9 @@ int goslam_mapping_points_emit(const float* poses_world, const float* disps, con
   char* ws = static_cast<char*>(workspace);
   size_t tb = tmp_bytes;
   const MapIter it(cub::CountingInputIterator<long long>(0), MapPointOp{poses_world, disps, intrinsic, hw, wd});
-  if (cub::DeviceSelect::Flagged(ws + L.tmp, tb, it, reinterpret_cast<const unsigned char*>(ws + L.mask1),
-                                 reinterpret_cast<MapPoint3*>(points), reinterpret_cast<long long*>(ws + L.nsel), n,
-                                 (cudaStream_t)stream) != cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, it, reinterpret_cast<const unsigned char*>(ws + L.mask1),
+                                     reinterpret_cast<MapPoint3*>(points), reinterpret_cast<long long*>(ws + L.nsel), n,
+                                     (cudaStream_t)stream));
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

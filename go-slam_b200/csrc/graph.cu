@@ -205,7 +205,7 @@ int goslam_proximity_edges(const float* dist, int t0, int t1, int t, int rad, in
   proximity_kernel<<<1, kGT, 0, (cudaStream_t)stream>>>(a);
   GS_CHECK_LAUNCH();
   if (num_edges)
-    cudaMemcpyAsync(num_edges, a.counters + 1, sizeof(int), cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+    GS_CUDA(cudaMemcpyAsync(num_edges, a.counters + 1, sizeof(int), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return GOSLAM_OK;
 }
 

@@ -469,10 +469,7 @@ int goslam_mesh_cull_count(const double* verts, int64_t n_verts, const int64_t* 
   cudaStream_t st = (cudaStream_t)stream;
   CullBox b;
   for (int c = 0; c < 3; ++c) { b.lo[c] = (double)lo[c]; b.hi[c] = (double)hi[c]; }
-  if (n_verts > 0 && cudaMemsetAsync(w.vref, 0, (size_t)n_verts * sizeof(unsigned), st) != cudaSuccess) {
-    gs_note_cuda_error(cudaGetLastError());
-    return GOSLAM_ELAUNCH;
-  }
+  if (n_verts > 0) GS_CUDA(cudaMemsetAsync(w.vref, 0, (size_t)n_verts * sizeof(unsigned), st));
   if (n_faces > 0) {
     cull_face_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(verts, n_verts, (const long long*)faces, n_faces, b, w.fkeep, w.vref);
     GS_CHECK_LAUNCH();
@@ -511,10 +508,7 @@ int goslam_mesh_cull_mask_count(int64_t n_verts, const int64_t* faces, int64_t n
   CullWork w;
   if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n_verts > 0 && cudaMemsetAsync(w.vref, 0, (size_t)n_verts * sizeof(unsigned), st) != cudaSuccess) {
-    gs_note_cuda_error(cudaGetLastError());
-    return GOSLAM_ELAUNCH;
-  }
+  if (n_verts > 0) GS_CUDA(cudaMemsetAsync(w.vref, 0, (size_t)n_verts * sizeof(unsigned), st));
   if (n_faces > 0) {
     cull_mask_face_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(n_verts, (const long long*)faces, n_faces, face_mask,
                                                                      vert_mask, w.fkeep, w.vref);

@@ -38,12 +38,6 @@ __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a,
 
 unsigned blocks_for(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
-bool note(cudaError_t e) {
-  if (e == cudaSuccess) return true;
-  gs_note_cuda_error(e);
-  return false;
-}
-
 // K sums of a block of kThreads threads, in a fixed tree; the result is valid in thread 0
 template <int K>
 __device__ __forceinline__ void block_sum(double (&v)[K], double (*sh)[kThreads]) {
@@ -99,10 +93,9 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const double* verts, l
   if (face_index) face_index[i] = lo;
 }
 
-size_t sample_cub_bytes(long long nf) {
-  size_t b = 0;
-  if (cub::DeviceScan::InclusiveSum(nullptr, b, (const double*)nullptr, (double*)nullptr, (int)nf) != cudaSuccess) return 0;
-  return b;
+int sample_cub_bytes(long long nf, size_t* b) {
+  GS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, *b, (const double*)nullptr, (double*)nullptr, (int)nf));
+  return GOSLAM_OK;
 }
 
 struct SampleWork { double* area; double* cum; void* cub_tmp; size_t cub_bytes; };
@@ -145,11 +138,10 @@ int key_bits(long long n) {
   return b;
 }
 
-size_t nn_cub_bytes(long long n) {
-  size_t b = 0;
+int nn_cub_bytes(long long n, size_t* b) {
   cub::DoubleBuffer<unsigned> k(nullptr, nullptr), v(nullptr, nullptr);
-  if (cub::DeviceRadixSort::SortPairs(nullptr, b, k, v, (int)n) != cudaSuccess) return 0;
-  return b;
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, *b, k, v, (int)n));
+  return GOSLAM_OK;
 }
 
 size_t nn_layout(long long n, size_t cub_bytes, const void* base, NnIndex* x) {
@@ -584,8 +576,8 @@ extern "C" {
 
 size_t goslam_mesh_sample_workspace_bytes(int64_t n_faces) {
   if (n_faces < 1 || n_faces > kMaxFaces) return 0;
-  const size_t cb = sample_cub_bytes(n_faces);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return 0; }
+  size_t cb = 0;
+  if (sample_cub_bytes(n_faces, &cb) != GOSLAM_OK) return 0;
   SampleWork w;
   return sample_layout(n_faces, cb, nullptr, &w);
 }
@@ -597,8 +589,8 @@ int goslam_mesh_sample_surface(const double* verts, int64_t n_verts, const int64
       (count > 0 && (!uniforms || !samples)))
     return GOSLAM_EINVAL;
   if (!workspace) return GOSLAM_EWORKSPACE;
-  const size_t cb = sample_cub_bytes(n_faces);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  size_t cb = 0;
+  if (const int rc = sample_cub_bytes(n_faces, &cb)) return rc;
   SampleWork w;
   if (workspace_bytes < sample_layout(n_faces, cb, workspace, &w)) return GOSLAM_EWORKSPACE;
   if (count == 0) return GOSLAM_OK;
@@ -606,7 +598,7 @@ int goslam_mesh_sample_surface(const double* verts, int64_t n_verts, const int64
   area_kernel<<<blocks_for(n_faces, kThreads), kThreads, 0, st>>>(verts, n_verts, (const long long*)faces, n_faces, w.area);
   GS_CHECK_LAUNCH();
   size_t tb = w.cub_bytes;
-  if (!note(cub::DeviceScan::InclusiveSum(w.cub_tmp, tb, w.area, w.cum, (int)n_faces, st))) return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceScan::InclusiveSum(w.cub_tmp, tb, w.area, w.cum, (int)n_faces, st));
   sample_kernel<<<blocks_for(count, kThreads), kThreads, 0, st>>>(verts, n_verts, (const long long*)faces, n_faces, w.cum,
                                                                   uniforms, count, samples, (long long*)face_index);
   GS_CHECK_LAUNCH();
@@ -615,8 +607,8 @@ int goslam_mesh_sample_surface(const double* verts, int64_t n_verts, const int64
 
 size_t goslam_nn_index_workspace_bytes(int64_t n_points) {
   if (n_points < 1 || n_points > kMaxPoints) return 0;
-  const size_t cb = nn_cub_bytes(n_points);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return 0; }
+  size_t cb = 0;
+  if (nn_cub_bytes(n_points, &cb) != GOSLAM_OK) return 0;
   NnIndex x;
   return nn_layout(n_points, cb, nullptr, &x);
 }
@@ -626,8 +618,8 @@ int goslam_nn_index_build(const double* points, int64_t n_points, double min_cel
   if (n_points < 1 || n_points > kMaxPoints || !points || !(min_cell >= 0.0) || !(min_cell < INFINITY))
     return GOSLAM_EINVAL;
   if (!index) return GOSLAM_EWORKSPACE;
-  const size_t cb = nn_cub_bytes(n_points);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  size_t cb = 0;
+  if (const int rc = nn_cub_bytes(n_points, &cb)) return rc;
   NnIndex x;
   if (index_bytes < nn_layout(n_points, cb, index, &x)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
@@ -640,8 +632,7 @@ int goslam_nn_index_build(const double* points, int64_t n_points, double min_cel
   GS_CHECK_LAUNCH();
   cub::DoubleBuffer<unsigned> kb(x.keys[0], x.keys[1]), vb(x.vals[0], x.vals[1]);
   size_t tb = x.cub_bytes;
-  if (!note(cub::DeviceRadixSort::SortPairs(x.cub_tmp, tb, kb, vb, (int)n_points, 0, key_bits(n_points), st)))
-    return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(x.cub_tmp, tb, kb, vb, (int)n_points, 0, key_bits(n_points), st));
   gather_kernel<<<blocks_for(n_points, kThreads), kThreads, 0, st>>>(points, n_points, vb.Current(), x.ids, x.pts);
   GS_CHECK_LAUNCH();
   const long long nc = max_cells(n_points);
@@ -656,8 +647,8 @@ int goslam_nn_query(const void* index, size_t index_bytes, int64_t n_points, con
       !(max_dist > 0.0))
     return GOSLAM_EINVAL;
   if (!index) return GOSLAM_EWORKSPACE;
-  const size_t cb = nn_cub_bytes(n_points);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  size_t cb = 0;
+  if (const int rc = nn_cub_bytes(n_points, &cb)) return rc;
   NnIndex x;
   if (index_bytes < nn_layout(n_points, cb, index, &x)) return GOSLAM_EWORKSPACE;
   if (n_query == 0) return GOSLAM_OK;
@@ -691,8 +682,8 @@ int goslam_icp_point_to_point(const double* source, int64_t n_source, const void
       relative_rmse != relative_rmse)
     return GOSLAM_EINVAL;
   if (!index || !workspace) return GOSLAM_EWORKSPACE;
-  const size_t cb = nn_cub_bytes(n_target);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  size_t cb = 0;
+  if (const int rc = nn_cub_bytes(n_target, &cb)) return rc;
   NnIndex x;
   if (index_bytes < nn_layout(n_target, cb, index, &x)) return GOSLAM_EWORKSPACE;
   IcpWork w;

@@ -259,22 +259,21 @@ struct IsRunStart {
   __device__ bool operator()(unsigned i) const { return i == 0 || lab[i] != lab[i - 1]; }
 };
 
-// CUB's temporary storage for the largest of the count pass's calls (needs a device to size); 0 on failure
-size_t comp_cub_bytes(long long nf) {
+// CUB's temporary storage for the largest of the count pass's calls (needs a device to size)
+int comp_cub_bytes(long long nf, size_t* bytes) {
   const int ne = (int)(3 * nf), n = (int)nf;
   size_t a = 0, b = 0, c = 0, d = 0;
   cub::DoubleBuffer<u64> k(nullptr, nullptr);
   cub::DoubleBuffer<unsigned> v(nullptr, nullptr), l(nullptr, nullptr);
   cub::DoubleBuffer<double> ar(nullptr, nullptr);
-  if (cub::DeviceRadixSort::SortPairs(nullptr, a, k, v, ne) != cudaSuccess) return 0;
-  if (cub::DeviceRadixSort::SortPairs(nullptr, b, l, ar, n) != cudaSuccess) return 0;
-  if (cub::DeviceSelect::If(nullptr, c, cub::CountingInputIterator<unsigned>(0), (unsigned*)nullptr, (long long*)nullptr, n,
-                            IsRunStart{nullptr}) != cudaSuccess)
-    return 0;
-  if (cub::DeviceSegmentedReduce::Sum(nullptr, d, (const double*)nullptr, (double*)nullptr, n, (const unsigned*)nullptr,
-                                      (const unsigned*)nullptr) != cudaSuccess)
-    return 0;
-  return std::max(std::max(a, b), std::max(c, d));
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, a, k, v, ne));
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, b, l, ar, n));
+  GS_CUDA(cub::DeviceSelect::If(nullptr, c, cub::CountingInputIterator<unsigned>(0), (unsigned*)nullptr, (long long*)nullptr,
+                                n, IsRunStart{nullptr}));
+  GS_CUDA(cub::DeviceSegmentedReduce::Sum(nullptr, d, (const double*)nullptr, (double*)nullptr, n, (const unsigned*)nullptr,
+                                          (const unsigned*)nullptr));
+  *bytes = std::max(std::max(a, b), std::max(c, d));
+  return GOSLAM_OK;
 }
 
 size_t comp_layout(long long nf, size_t cub_bytes, void* base, CompWork* w) {
@@ -396,12 +395,6 @@ __global__ void __launch_bounds__(256) face_keep_kernel(const unsigned* labels, 
 
 unsigned blocks_for(long long n, int threads) { return (unsigned)cdiv64(n, threads); }
 
-bool note(cudaError_t e) {
-  if (e == cudaSuccess) return true;
-  gs_note_cuda_error(e);
-  return false;
-}
-
 // faces and vertices are counted in u32 inside the component filter
 constexpr long long kMaxCompFaces = (1ll << 31) - 1;
 
@@ -449,10 +442,7 @@ int goslam_mesh_view_masks(const double* verts, int64_t n_verts, const float* w2
 size_t goslam_mesh_components_workspace_bytes(int64_t n_verts, int64_t n_faces) {
   if (n_verts < 0 || n_faces < 0 || n_faces > kMaxCompFaces) return 0;
   size_t cb = 0;
-  if (n_faces > 0 && (cb = comp_cub_bytes(n_faces)) == 0) {
-    gs_note_cuda_error(cudaGetLastError());
-    return 0;
-  }
+  if (n_faces > 0 && comp_cub_bytes(n_faces, &cb) != GOSLAM_OK) return 0;
   CompWork w;
   return comp_layout(n_faces, cb, nullptr, &w);
 }
@@ -463,9 +453,12 @@ int goslam_mesh_components_count(const double* verts, int64_t n_verts, const int
     return GOSLAM_EINVAL;
   if (!workspace) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n_faces == 0) return note(cudaMemsetAsync(counts, 0, sizeof(int64_t), st)) ? GOSLAM_OK : GOSLAM_ELAUNCH;
-  const size_t cb = comp_cub_bytes(n_faces);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  if (n_faces == 0) {
+    GS_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t), st));
+    return GOSLAM_OK;
+  }
+  size_t cb = 0;
+  if (const int rc = comp_cub_bytes(n_faces, &cb)) return rc;
   CompWork w;
   if (workspace_bytes < comp_layout(n_faces, cb, workspace, &w)) return GOSLAM_EWORKSPACE;
   const long long ne = 3 * n_faces;
@@ -475,29 +468,25 @@ int goslam_mesh_components_count(const double* verts, int64_t n_verts, const int
   cub::DoubleBuffer<u64> kb(w.keys[0], w.keys[1]);
   cub::DoubleBuffer<unsigned> fb(w.efaces[0], w.efaces[1]);
   size_t tb = w.cub_bytes;
-  if (!note(cub::DeviceRadixSort::SortPairs(w.cub_tmp, tb, kb, fb, (int)ne, 0, 64, st))) return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, tb, kb, fb, (int)ne, 0, 64, st));
   union_kernel<<<blocks_for(ne, 256), 256, 0, st>>>(kb.Current(), fb.Current(), ne, w.parent);
   GS_CHECK_LAUNCH();
   label_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(w.parent, n_faces, w.labels[0]);
   GS_CHECK_LAUNCH();
   // the labels stay in labels[0] for the face verdicts: sort copies of them
-  if (!note(cudaMemcpyAsync(w.labels[1], w.labels[0], n_faces * sizeof(unsigned), cudaMemcpyDeviceToDevice, st)))
-    return GOSLAM_ELAUNCH;
+  GS_CUDA(cudaMemcpyAsync(w.labels[1], w.labels[0], n_faces * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
   cub::DoubleBuffer<unsigned> lb(w.labels[1], (unsigned*)w.keys[0]);
   cub::DoubleBuffer<double> ab(w.area[0], w.area[1]);
   tb = w.cub_bytes;
-  if (!note(cub::DeviceRadixSort::SortPairs(w.cub_tmp, tb, lb, ab, (int)n_faces, 0, 32, st))) return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, tb, lb, ab, (int)n_faces, 0, 32, st));
   // keep the sorted labels and areas where the emit pass finds them
-  if (lb.Current() != w.labels[1] &&
-      !note(cudaMemcpyAsync(w.labels[1], lb.Current(), n_faces * sizeof(unsigned), cudaMemcpyDeviceToDevice, st)))
-    return GOSLAM_ELAUNCH;
-  if (ab.Current() != w.area[1] &&
-      !note(cudaMemcpyAsync(w.area[1], ab.Current(), n_faces * sizeof(double), cudaMemcpyDeviceToDevice, st)))
-    return GOSLAM_ELAUNCH;
+  if (lb.Current() != w.labels[1])
+    GS_CUDA(cudaMemcpyAsync(w.labels[1], lb.Current(), n_faces * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+  if (ab.Current() != w.area[1])
+    GS_CUDA(cudaMemcpyAsync(w.area[1], ab.Current(), n_faces * sizeof(double), cudaMemcpyDeviceToDevice, st));
   tb = w.cub_bytes;
-  if (!note(cub::DeviceSelect::If(w.cub_tmp, tb, cub::CountingInputIterator<unsigned>(0), w.seg_begin, (long long*)counts,
-                                  (int)n_faces, IsRunStart{w.labels[1]}, st)))
-    return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceSelect::If(w.cub_tmp, tb, cub::CountingInputIterator<unsigned>(0), w.seg_begin, (long long*)counts,
+                                (int)n_faces, IsRunStart{w.labels[1]}, st));
   seg_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(w.labels[1], (const long long*)counts, n_faces, w.seg_begin,
                                                        w.seg_of_label);
   GS_CHECK_LAUNCH();
@@ -512,14 +501,13 @@ int goslam_mesh_components_keep(int64_t n_faces, int64_t n_components, double th
   if (!workspace) return GOSLAM_EWORKSPACE;
   if (n_faces == 0) return GOSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t cb = comp_cub_bytes(n_faces);
-  if (cb == 0) { gs_note_cuda_error(cudaGetLastError()); return GOSLAM_ELAUNCH; }
+  size_t cb = 0;
+  if (const int rc = comp_cub_bytes(n_faces, &cb)) return rc;
   CompWork w;
   if (workspace_bytes < comp_layout(n_faces, cb, workspace, &w)) return GOSLAM_EWORKSPACE;
   size_t tb = w.cub_bytes;
-  if (!note(cub::DeviceSegmentedReduce::Sum(w.cub_tmp, tb, w.area[1], w.comp_area, (int)n_components, w.seg_begin,
-                                            w.seg_begin + 1, st)))
-    return GOSLAM_ELAUNCH;
+  GS_CUDA(cub::DeviceSegmentedReduce::Sum(w.cub_tmp, tb, w.area[1], w.comp_area, (int)n_components, w.seg_begin,
+                                          w.seg_begin + 1, st));
   decide_kernel<<<1, kDecideThreads, 0, st>>>(w.comp_area, n_components, threshold, largest, w.comp_keep);
   GS_CHECK_LAUNCH();
   face_keep_kernel<<<blocks_for(n_faces, 256), 256, 0, st>>>(w.labels[0], w.seg_of_label, w.comp_keep, n_faces, face_keep);

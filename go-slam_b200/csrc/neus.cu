@@ -23,7 +23,6 @@
 #include "common.cuh"
 #include <math.h>
 #include <algorithm>
-#include <mutex>
 
 namespace {
 
@@ -1315,15 +1314,8 @@ __global__ void __launch_bounds__(kMbWarps * 32, 1) neus_mlp_bwd_kernel(const Ml
   }
 }
 
-// hash-grid constants are per DEVICE (constant memory) and the opt-in shared memory is per device too
-int neus_device_init() {
-  static bool ready[64];
-  static std::mutex mu;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return GOSLAM_EINVAL;
-  std::lock_guard<std::mutex> lock(mu);
-  if (ready[dev]) return GOSLAM_OK;
+// hash-grid constants are per DEVICE (constant memory), so is the opt-in shared memory (gs_device_setup)
+int neus_device_init(int) {
   GridMeta g = make_grid_meta(nullptr);
   LevelConst lc[kLevels];
   for (int l = 0; l < kLevels; ++l) {
@@ -1336,14 +1328,12 @@ int neus_device_init() {
     const bool hashed = dense > g.size[l];
     if (hashed != (l >= kDenseLevels) || (hashed && g.size[l] != (1u << 19))) return GOSLAM_EINVAL;
   }
-  if (cudaMemcpyToSymbol(c_lvl, lc, sizeof(lc)) != cudaSuccess) return GOSLAM_ELAUNCH;
-  if (cudaFuncSetAttribute(neus_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(Smem)) != cudaSuccess) return GOSLAM_ELAUNCH;
-  if (cudaFuncSetAttribute(neus_vertex_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(Smem)) != cudaSuccess) return GOSLAM_ELAUNCH;
-  if (cudaFuncSetAttribute(neus_mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(MlpBwdSmem)) != cudaSuccess) return GOSLAM_ELAUNCH;
-  ready[dev] = true;
+  GS_CUDA(cudaMemcpyToSymbol(c_lvl, lc, sizeof(lc)));
+  GS_CUDA(cudaFuncSetAttribute(neus_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)));
+  GS_CUDA(cudaFuncSetAttribute(neus_vertex_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)sizeof(Smem)));
+  GS_CUDA(cudaFuncSetAttribute(neus_mlp_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)sizeof(MlpBwdSmem)));
   return GOSLAM_OK;
 }
 
@@ -1377,7 +1367,7 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, c
   if (workspace == nullptr || workspace_bytes < goslam_neus_workspace_bytes(R, S))
     return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
   GsArena ar(workspace, workspace_bytes);
   NeusArgs a{};
   a.p = *params; a.o = *out;
@@ -1439,7 +1429,7 @@ int goslam_neus_mlp_backward(const goslam_neus_params* params, const void* mlp_i
       !out->d_grad_total || R < 0 || S <= 0)
     return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
-  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
   MlpBwdArgs a{};
   a.mlp_w = reinterpret_cast<const __half*>(params->mlp_w); a.color_B = params->color_B;
   a.X = reinterpret_cast<const __half*>(mlp_in); a.enc = reinterpret_cast<const __half*>(enc); a.pos = pos;
@@ -1465,7 +1455,7 @@ int goslam_neus_grid_backward(const goslam_neus_params* params, const float* ray
       sample0 < 0)
     return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
-  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
   GridBwdArgs a{};
   a.p = *params; a.rays_o = rays_o; a.rays_d = rays_d; a.z_vals = z_vals; a.dists = dists;
   a.d_enc = d_enc; a.d_enc_scale = d_enc_scale; a.d_grad = d_grad; a.grid_grad = grid_grad; a.d_w0 = d_w0;
@@ -1482,7 +1472,7 @@ int goslam_neus_sdf_grid(const goslam_neus_params* params, const float* xs, cons
                          int ny, int nz, float* u, void* stream) {
   if (!params || !xs || !ys || !zs || !u || nx < 1 || ny < 1 || nz < 1 || (long long)nx * ny * nz > (1ll << 40))
     return GOSLAM_EINVAL;
-  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
   SdfGridArgs a{};
   a.p = *params; a.xs = xs; a.ys = ys; a.zs = zs; a.nx = nx; a.ny = ny; a.nz = nz; a.u = u;
   a.n = (long long)nx * ny * nz;
@@ -1497,7 +1487,7 @@ int goslam_neus_vertex_color(const goslam_neus_params* params, const double* ver
                              void* stream) {
   if (!params || n < 0 || (n > 0 && (!verts || !rgb))) return GOSLAM_EINVAL;
   if (n == 0) return GOSLAM_OK;
-  { const int rc = neus_device_init(); if (rc != GOSLAM_OK) return rc; }
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
   VertexColorArgs a{};
   a.p = *params; a.verts = verts; a.n = n; a.rgb = rgb;
   const long long groups = (n + 31) / 32;

@@ -197,7 +197,7 @@ struct ObbLayout {
     aown = take((size_t)n * sizeof(int));
     adist = take((size_t)n * sizeof(float));
     out = take((size_t)n * sizeof(int));
-    size_t t1 = 0;
+    size_t t1 = 0;   // a failed size query is reported by the select calls themselves (GS_CUDA)
     cub::DeviceSelect::Flagged(nullptr, t1, cub::CountingInputIterator<int>(0), (const unsigned char*)nullptr,
                                (int*)nullptr, (long long*)nullptr, (int)std::max<long long>(n, 1));
     tmp_bytes = std::max<size_t>(t1, 1);
@@ -960,11 +960,8 @@ int goslam_hull_vertices(const double* points, int64_t n, void* workspace, size_
   int* out = reinterpret_cast<int*>(ws + L.out);
   const HullMem wh = hull_mem(ws + L.win, kWinCap, kDirs, &gs->wh, nullptr, nullptr, nullptr);
   const HullMem mh = hull_mem(ws + L.main, facet_cap(n), 0, &gs->mh, apt, aown, adist);
-  if (cudaMemsetAsync(gs, 0, sizeof(ObbState), s) != cudaSuccess ||
-      cudaMemsetAsync(vflag, 0, (size_t)n, s) != cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cudaMemsetAsync(gs, 0, sizeof(ObbState), s));
+  GS_CUDA(cudaMemsetAsync(vflag, 0, (size_t)n, s));
   extremes_kernel<<<grid_for(n), kThreads, 0, s>>>(points, n, make_dirs(), gs);
   GS_CHECK_LAUNCH();
   winners_kernel<<<1, 32, 0, s>>>(gs);
@@ -974,19 +971,13 @@ int goslam_hull_vertices(const double* points, int64_t n, void* workspace, size_
   cull_kernel<<<grid_for(n), kThreads, 0, s>>>(points, n, wh, gs, keep);
   GS_CHECK_LAUNCH();
   size_t tb = L.tmp_bytes;
-  if (cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), keep, surv, &gs->n_surv, (int)n,
-                                 s) != cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), keep, surv, &gs->n_surv, (int)n,
+                                     s));
   hull_kernel<<<1, kHullThreads, 0, s>>>(points, surv, &gs->n_surv, mh, &gs->nonfinite, surv, vflag);
   GS_CHECK_LAUNCH();
   tb = L.tmp_bytes;
-  if (cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), vflag, out, &gs->n_vert, (int)n,
-                                 s) != cudaSuccess) {
-    GS_CHECK_LAUNCH();
-    return GOSLAM_ELAUNCH;
-  }
+  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), vflag, out, &gs->n_vert, (int)n,
+                                     s));
   info_kernel<<<1, 1, 0, s>>>(gs, info);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;

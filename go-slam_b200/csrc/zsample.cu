@@ -187,7 +187,7 @@ int goslam_sample_z(const float* rays_o, const float* rays_d, const float* bound
   cudaStream_t st = (cudaStream_t)stream;
   unsigned* scal = reinterpret_cast<unsigned*>(workspace);
   if (gt_depth) {
-    cudaMemsetAsync(scal, 0, sizeof(unsigned), st);
+    GS_CUDA(cudaMemsetAsync(scal, 0, sizeof(unsigned), st));
     const int blocks = gs_cdiv(R, 256 * 8) < kNumSms ? gs_cdiv(R, 256 * 8) : kNumSms;
     zs_max_kernel<<<blocks, 256, 0, st>>>(gt_depth, R, scal);
     GS_CHECK_LAUNCH();

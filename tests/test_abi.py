@@ -102,6 +102,58 @@ def test_argument_validation_without_gpu(lib):
         assert lib.goslam_conv2d_nhwc(ctypes.byref(d), 0, 8, 16, null) == -1, cout_pad
 
 
+def _has_cuda_device():
+    try:
+        import torch
+        return torch.cuda.is_available()
+    except Exception:  # noqa: BLE001
+        return False
+
+
+@pytest.mark.skipif(_has_cuda_device(), reason="checks the failure path without a CUDA device")
+def test_setup_failure_is_launch_error_with_cuda_error(lib):
+    """valid calls whose first CUDA work is per-device setup (function attributes, constant memory, the tensor-map
+    encoder) fail as GOSLAM_ELAUNCH and name the CUDA error behind it, as every other failed launch does."""
+    import threading
+    from goslam_b200 import _lib
+    p = ctypes.c_void_p(1 << 20)                       # never dereferenced: nothing reaches a device
+    pyramid = (ctypes.c_void_p * 4)(*[1 << 20] * 4)   # host array of (16-byte aligned) device pointers
+    conv = _lib.ConvDesc()
+    conv.inp[0], conv.cin[0], conv.cin_stride[0], conv.n_in = p, 64, 64, 1
+    conv.weight, conv.bias, conv.out = p, p, p
+    conv.taps, conv.cout, conv.cout_pad, conv.out_scale, conv.out_stride = 1, 64, 64, 1.0, 64
+    ba_ws = lib.goslam_ba_workspace_bytes(1, 2, 4, 4, 1, 2)
+    neus = _lib.NeusParams(p, p, p, p, p)
+    neus_out = _lib.NeusOut(*[p] * 15)
+    mlp_out = _lib.NeusMlpBwdOut(*[p] * 10)
+    calls = {
+        "altcorr_forward": lambda: lib.goslam_altcorr_forward(p, p, p, p, 1, 1, 8, 8, 8, 8, 128, 3, None),
+        "altcorr_pyramid": lambda: lib.goslam_altcorr_pyramid(pyramid, 4, p, p, p, p, 1, 16, 16, 128, 3, None),
+        "conv2d_nhwc": lambda: lib.goslam_conv2d_nhwc(ctypes.byref(conv), 1, 8, 16, None),
+        "corr_pool_build": lambda: lib.goslam_corr_pool_build(p, 2, 1, p, p, p, pyramid, 4, 1, 128, 32, 32, None),
+        "ba": lambda: lib.goslam_ba(p, p, p, p, p, p, None, 0, p, p, 1, 2, 4, 4, 1, 2, 1, 1e-4, 0.1, 1, None, None,
+                                    None, p, ba_ws, None),
+        "neus_forward": lambda: lib.goslam_neus_forward(ctypes.byref(neus), p, p, p, p, 1, 8, ctypes.byref(neus_out), p,
+                                                        lib.goslam_neus_workspace_bytes(1, 8), None),
+        "neus_mlp_backward": lambda: lib.goslam_neus_mlp_backward(ctypes.byref(neus), *[p] * 10, 1, 8,
+                                                                  ctypes.byref(mlp_out), None),
+        "neus_grid_backward": lambda: lib.goslam_neus_grid_backward(ctypes.byref(neus), p, p, p, p, None, 0, 1, 8, p,
+                                                                    None, p, p, p, None),
+        "neus_sdf_grid": lambda: lib.goslam_neus_sdf_grid(ctypes.byref(neus), p, p, p, 2, 2, 2, p, None),
+        "neus_vertex_color": lambda: lib.goslam_neus_vertex_color(ctypes.byref(neus), p, 1, p, None),
+    }
+    got = {}
+
+    def run(name):   # the noted error is per thread: a fresh thread starts with none
+        got[name] = (calls[name](), lib.goslam_last_cuda_error())
+    for name in calls:
+        t = threading.Thread(target=run, args=(name,))
+        t.start()
+        t.join()
+    for name, (rc, err) in got.items():
+        assert rc == -2 and err, (name, rc, err)
+
+
 def test_hashgrid_layout_matches_oracle(lib):
     from goslam_b200 import neus
     from oracle import neus_oracle
