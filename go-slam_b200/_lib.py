@@ -191,6 +191,8 @@ SIGNATURES = {
     "goslam_hull_vertices_emit": (c_int, [c_void_p, c_size_t, c_int64, c_void_p, c_int64, c_void_p]),
     "goslam_obb_from_hull": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, ctypes.c_double, c_void_p, c_void_p]),
     "goslam_obb_in_bound": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
+    "goslam_ape_workspace_bytes": (c_size_t, [c_int64]),
+    "goslam_ape_sim3": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "goslam_corr_index_backward": (c_int, []),
     "goslam_altcorr_backward": (c_int, []),
 }

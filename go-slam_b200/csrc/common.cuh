@@ -121,6 +121,25 @@ __device__ __forceinline__ long long gs_div_fast(long long a, long long b, doubl
   return q;
 }
 
+// K sums of a block of Threads threads in a fixed tree, every addition rounded on its own (no FMA), so the result does
+// not depend on scheduling or on the compiler; valid in thread 0.  The fp64 reductions with fixed-order block partials
+// (mesh_eval.cu, traj_eval.cu) are built on it.
+template <int K, int Threads>
+__device__ __forceinline__ void gs_block_sum(double (&v)[K], double (*sh)[Threads]) {
+#pragma unroll
+  for (int k = 0; k < K; ++k) sh[k][threadIdx.x] = v[k];
+  __syncthreads();
+  for (int h = Threads / 2; h > 0; h >>= 1) {
+    if (threadIdx.x < h) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) sh[k][threadIdx.x] = __dadd_rn(sh[k][threadIdx.x], sh[k][threadIdx.x + h]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) v[k] = sh[k][0];
+}
+
 __device__ __forceinline__ float gs_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -38,23 +38,6 @@ __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a,
 
 unsigned blocks_for(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
-// K sums of a block of kThreads threads, in a fixed tree; the result is valid in thread 0
-template <int K>
-__device__ __forceinline__ void block_sum(double (&v)[K], double (*sh)[kThreads]) {
-#pragma unroll
-  for (int k = 0; k < K; ++k) sh[k][threadIdx.x] = v[k];
-  __syncthreads();
-  for (int h = kThreads / 2; h > 0; h >>= 1) {
-    if (threadIdx.x < h) {
-#pragma unroll
-      for (int k = 0; k < K; ++k) sh[k][threadIdx.x] = dadd(sh[k][threadIdx.x], sh[k][threadIdx.x + h]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int k = 0; k < K; ++k) v[k] = sh[k][0];
-}
-
 // ---- surface sampling ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) area_kernel(const double* verts, long long nv, const long long* faces,
                                                         long long nf, double* area) {
@@ -436,7 +419,7 @@ __global__ void __launch_bounds__(kThreads) icp_correspond_kernel(const double* 
       v[5] = pts[3 * b.pos]; v[6] = pts[3 * b.pos + 1]; v[7] = pts[3 * b.pos + 2];
     }
   }
-  block_sum<8>(v, sh);
+  gs_block_sum(v, sh);
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) part[8 * (long long)blockIdx.x + k] = v[k];
@@ -453,7 +436,7 @@ __global__ void __launch_bounds__(kThreads) icp_reduce_kernel(const double* part
 #pragma unroll
     for (int k = 0; k < 8; ++k) v[k] = dadd(v[k], part[8 * (long long)b + k]);
   }
-  block_sum<8>(v, sh);
+  gs_block_sum(v, sh);
   if (threadIdx.x != 0) return;
   const double cnt = v[0];
   double fitness = 0.0, rmse = 0.0;
@@ -489,7 +472,7 @@ __global__ void __launch_bounds__(kThreads) icp_cov_kernel(const double* work, l
 #pragma unroll
       for (int q = 0; q < 3; ++q) v[3 * r + q] = dmul(a[r], b[q]);
   }
-  block_sum<9>(v, sh);
+  gs_block_sum(v, sh);
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int k = 0; k < 9; ++k) part[9 * (long long)blockIdx.x + k] = v[k];
@@ -497,18 +480,12 @@ __global__ void __launch_bounds__(kThreads) icp_cov_kernel(const double* work, l
 }
 
 // the rotation of Umeyama's method (no scaling) for the cross-covariance A: U diag(1, 1, det(U) det(V) < 0 ? -1 : 1) V^T.
-// One-sided Jacobi SVD (B = A V with orthogonal columns), singular values sorted descending; u3 is taken as u1 x u2, for
-// which the product reduces to u1 v1^T + u2 v2^T + det(V) (u1 x u2) v3^T, also for rank 2.  Rank < 2 (s2 <= 1e-14 s1):
-// the rotation is not unique and the identity is returned.
+// gs_umeyama_svd; u3 is taken as u1 x u2, for which the product reduces to u1 v1^T + u2 v2^T + det(V) (u1 x u2) v3^T,
+// also for rank 2.  Rank < 2 (s2 <= 1e-14 s1): the rotation is not unique and the identity is returned.
 __device__ void umeyama_rotation(const double A[9], double R[9]) {
-  double B[9], V[9];
-  gs_jacobi3(A, B, V);
-  double sv[3];
-  int ord[3] = {0, 1, 2};
-  for (int j = 0; j < 3; ++j) sv[j] = sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);
-  for (int a = 0; a < 3; ++a)
-    for (int b = a + 1; b < 3; ++b)
-      if (sv[ord[b]] > sv[ord[a]]) { const int t = ord[a]; ord[a] = ord[b]; ord[b] = t; }
+  double B[9], V[9], sv[3];
+  int ord[3];
+  gs_umeyama_svd(A, B, V, sv, ord);
   for (int k = 0; k < 9; ++k) R[k] = (k % 4 == 0) ? 1.0 : 0.0;
   const double s1 = sv[ord[0]], s2 = sv[ord[1]];
   if (!(s1 > 0.0) || !(s2 > 1e-14 * s1)) return;
@@ -537,7 +514,7 @@ __global__ void __launch_bounds__(kThreads) icp_solve_kernel(const double* part,
 #pragma unroll
     for (int k = 0; k < 9; ++k) v[k] = dadd(v[k], part[9 * (long long)b + k]);
   }
-  block_sum<9>(v, sh);
+  gs_block_sum(v, sh);
   if (threadIdx.x != 0) return;
   double U[16];
   for (int k = 0; k < 16; ++k) U[k] = (k % 5 == 0) ? 1.0 : 0.0;

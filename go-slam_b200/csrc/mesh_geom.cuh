@@ -1,5 +1,5 @@
 // mesh_geom.cuh — geometry shared by the mesh kernels: per-face areas (component filter, surface sampling) and the
-// one-thread 3x3 Jacobi SVD (ICP's Umeyama update, the oriented box's principal axes).
+// one-thread 3x3 Jacobi SVD (ICP's Umeyama update, the trajectory's Sim(3) alignment, the oriented box's principal axes).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -48,4 +48,18 @@ __device__ __forceinline__ void gs_jacobi3(const double A[9], double B[9], doubl
     }
     if (!rotated) break;
   }
+}
+
+// The SVD part of Umeyama's method for the 3x3 cross-covariance A (the ICP's update, the trajectory's Sim(3)
+// alignment): gs_jacobi3, then the singular values sv (the column norms of B) and the order ord that sorts them
+// descending, sv[ord[0]] >= sv[ord[1]] >= sv[ord[2]].  Column ord[k] of B is sigma_k u_k, column ord[k] of V is v_k.
+__device__ __forceinline__ void gs_umeyama_svd(const double A[9], double B[9], double V[9], double sv[3], int ord[3]) {
+  gs_jacobi3(A, B, V);
+  for (int j = 0; j < 3; ++j) {
+    ord[j] = j;
+    sv[j] = sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);
+  }
+  for (int a = 0; a < 3; ++a)
+    for (int b = a + 1; b < 3; ++b)
+      if (sv[ord[b]] > sv[ord[a]]) { const int t = ord[a]; ord[a] = ord[b]; ord[b] = t; }
 }

@@ -797,6 +797,37 @@ int goslam_obb_from_hull(const double* points, int64_t n, const void* workspace,
                          double* box, void* stream);
 int goslam_obb_in_bound(const double* box, const double* points, int64_t n, uint8_t* mask, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Trajectory evaluation of SLAM.terminate (src/slam.py:341-370): evo's APE w.r.t. the translation part with a Sim(3)
+ * Umeyama alignment (main_ape.ape(..., align=True, correct_scale=True)).  Device pointers, f64, no host
+ * synchronisation; the caller reads `out` once when the stream reaches it.
+ *
+ * goslam_ape_sim3 — est [n,3] estimated positions, ref [n,4,4] row-major reference c2w poses, 0 <= n <= 2^31 - 1.
+ *   Row i is kept iff the sum of its 16 reference entries (numpy's pairwise order) is finite; kept rows stay in input
+ *   order.  On the kept rows (x = est, y = ref translation): mx, my the means, sigma_x^2 = (1/n) sum |x - mx|^2,
+ *   C = (1/n) sum (y - my)(x - mx)^T = U diag(d) V^T (d descending), S = diag(1, 1, det U det V < 0 ? -1 : 1),
+ *   R = U S V^T, c = trace(diag(d) S) / sigma_x^2, t = my - c R mx; errors e_i = |(R (c x_i) + t) - y_i|.
+ *   out [GOSLAM_APE_OUT] (device f64): status (GOSLAM_APE_*), kept rows, sim3 [16] row-major = [[c R, t], [0, 1]],
+ *   the statistics rmse, mean, median (numpy's), std (population), min, max, sse, then d [3].  sim3 and the
+ *   statistics are NaN unless the status is GOSLAM_APE_OK; d is NaN unless the covariance was reached.
+ *   errors [n] (device f64): the kept rows' errors in input order in its first `kept` entries.  Degenerate: fewer than
+ *   three kept rows, or fewer than two d_k > 2.220446049250313e-16.  Two calls on the same input give the same bits.
+ *   Workspace: goslam_ape_workspace_bytes(n) (0 only for an invalid n).
+ * ---------------------------------------------------------------------------------- */
+#define GOSLAM_APE_OK                  0
+#define GOSLAM_APE_NO_ROWS             1  /* no reference row with a finite sum      */
+#define GOSLAM_APE_NONFINITE_ESTIMATE  2  /* a kept row's estimate is NaN or Inf     */
+#define GOSLAM_APE_DEGENERATE          3  /* Umeyama alignment is not possible       */
+#define GOSLAM_APE_STATUS    0
+#define GOSLAM_APE_KEPT      1
+#define GOSLAM_APE_SIM3      2
+#define GOSLAM_APE_STATS    18  /* rmse, mean, median, std, min, max, sse */
+#define GOSLAM_APE_SINGULAR 25
+#define GOSLAM_APE_OUT      28
+size_t goslam_ape_workspace_bytes(int64_t n);
+int goslam_ape_sim3(const double* est, const double* ref, int64_t n, void* workspace, size_t workspace_bytes,
+                    double* out, double* errors, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
