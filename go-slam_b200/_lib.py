@@ -1,17 +1,27 @@
-"""ctypes binding of libgoslam_b200.so (C-ABI in include/goslam_b200.h).
+"""ctypes binding of libgoslam_b200.so.
 
-No CPU fallback lives here or anywhere else in the product path: if the shared library is
-missing it is built with nvcc (go-slam_b200/build.py); if a kernel cannot launch the caller
-gets a RuntimeError.
+The C header include/goslam_b200.h is the one statement of the ABI: load() parses its prototypes and sets every
+entry's restype / argtypes from them.  Entries that return an int status are called through `call`, which passes
+tensors as device pointers, adds the current stream and raises on an error code.
+
+No CPU fallback lives here or anywhere else in the product path: if the shared library is missing it is built with
+nvcc (go-slam_b200/build.py); if a kernel cannot launch the caller gets a RuntimeError.
 """
 import ctypes
 import os
+import re
 import threading
+
+import torch
 
 from . import build as _build
 
 _lock = threading.Lock()
 _LIB = None
+HEADER = os.path.join(_build.ROOT, "include", "goslam_b200.h")
+SIGNATURES = {}            # name -> (restype, argtypes) of every function the header declares, filled by load()
+_TAKES_STREAM = set()      # names whose last parameter is `void* stream`
+_ws_cache = {}
 
 c_void_p, c_int, c_float, c_size_t, c_int64 = (
     ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_size_t, ctypes.c_int64)
@@ -69,133 +79,48 @@ class EncoderWeights(ctypes.Structure):
     _fields_ = [("stem", EncoderConv), ("block", (EncoderConv * 3) * 6), ("out", EncoderConv)]
 
 
-# name -> (restype, argtypes); every symbol include/goslam_b200.h declares
-SIGNATURES = {
-    "goslam_version": (c_int, []),
-    "goslam_sm_arch": (c_int, []),
-    "goslam_strerror": (ctypes.c_char_p, [c_int]),
-    "goslam_last_cuda_error": (ctypes.c_char_p, []),
-    "goslam_corr_index_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
-    "goslam_corr_pyramid_lookup": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
-    "goslam_corr_build": (c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "goslam_fmaps_to_kmajor": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
-    "goslam_corr_level_plane_elems": (c_size_t, [c_int] * 4),
-    "goslam_corr_pool_build": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "goslam_corr_pool_lookup": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
-    "goslam_altcorr_forward": (c_int, [c_void_p] * 4 + [c_int] * 8 + [c_void_p]),
-    "goslam_altcorr_pyramid": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
-    "goslam_frame_distance": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float, c_void_p]),
-    "goslam_frame_distance_bidir": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float, c_void_p]),
-    "goslam_frame_distance_grid_workspace_bytes": (c_size_t, [c_int] * 4),
-    "goslam_frame_distance_grid": (c_int, [c_void_p] * 3 + [c_int] * 7 + [c_float, c_void_p, c_void_p, c_size_t,
-                                                                        c_void_p]),
-    "goslam_projmap": (c_int, [c_void_p] * 7 + [c_int] * 3 + [c_void_p]),
-    "goslam_iproj": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
-    "goslam_depth_filter": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p]),
-    "goslam_mvfilter_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_mvfilter_compute": (c_int, [c_void_p] * 4 + [c_float, c_int, c_int] + [c_int] * 3 +
-                                [c_void_p, c_size_t, c_void_p]),
-    "goslam_mvfilter_commit": (c_int, [c_void_p] * 3 + [c_size_t] + [c_int] * 3 + [c_void_p] * 8),
-    "goslam_reproject": (c_int, [c_void_p] * 7 + [c_int] * 3 + [c_void_p]),
-    "goslam_reproject_motion": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_void_p]),
-    "goslam_ba_workspace_bytes": (c_size_t, [c_int] * 6),
-    "goslam_ba": (c_int, [c_void_p] * 7 + [c_int] + [c_void_p] * 2 + [c_int] * 7 +
-                  [c_float, c_float, c_int] + [c_void_p] * 3 + [c_void_p, c_size_t, c_void_p]),
-    "goslam_ba_system_doubles": (c_size_t, [c_int, c_int]),
-    "goslam_ba_phase1": (c_int, [c_void_p] * 7 + [c_int] + [c_void_p] * 2 + [c_int] * 7 +
-                         [c_void_p, c_void_p, c_size_t, c_void_p]),
-    "goslam_ba_phase2": (c_int, [c_void_p] * 3 + [c_int] * 6 + [c_float, c_float] + [c_int] * 3 +
-                         [c_void_p] * 3 + [c_void_p, c_size_t, c_void_p]),
-    "goslam_ba_phase1_peers": (c_int, [c_void_p] * 6 + [c_int] + [c_void_p] * 2 + [c_int] * 7 +
-                               [ctypes.POINTER(BaPeers), c_void_p, c_size_t, c_void_p]),
-    "goslam_ba_phase2_peers": (c_int, [c_void_p] + [c_int] * 6 + [c_float, c_float] + [c_int] * 3 +
-                               [ctypes.POINTER(BaPeers)] + [c_void_p] * 4 + [c_size_t, c_void_p]),
-    "goslam_ba_peers_wait": (c_int, [ctypes.POINTER(BaPeers), c_void_p]),
-    "goslam_peer_alloc": (c_int, [c_size_t, c_void_p, c_void_p]),
-    "goslam_peer_free": (c_int, [c_void_p]),
-    "goslam_ipc_open": (c_int, [c_void_p, c_void_p]),
-    "goslam_ipc_close": (c_int, [c_void_p]),
-    "goslam_neus_workspace_bytes": (c_size_t, [c_int, c_int]),
-    "goslam_neus_forward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 4 + [c_int, c_int] +
-                            [ctypes.POINTER(NeusOut), c_void_p, c_size_t, c_void_p]),
-    "goslam_neus_composite_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 13 + [c_int64, c_int64, c_int, c_int] +
-                                       [c_void_p] * 5),
-    "goslam_neus_grid_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 5 + [c_int64, c_int, c_int] + [c_void_p] * 6),
-    "goslam_neus_mlp_backward": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 10 + [c_int, c_int] +
-                                 [ctypes.POINTER(NeusMlpBwdOut), c_void_p]),
-    "goslam_hashgrid_layout": (c_int64, [c_void_p, c_void_p, c_void_p]),
-    "goslam_neus_sdf_grid": (c_int, [ctypes.POINTER(NeusParams)] + [c_void_p] * 3 + [c_int] * 3 + [c_void_p, c_void_p]),
-    "goslam_mc_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_mc_count": (c_int, [c_void_p] + [c_int] * 3 + [ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p]),
-    "goslam_mc_emit": (c_int, [c_void_p] + [c_int] * 3 + [ctypes.c_double] + [c_void_p] * 3 + [c_size_t] +
-                       [c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
-    "goslam_mesh_cull_workspace_bytes": (c_size_t, [c_int64, c_int64]),
-    "goslam_mesh_cull_count": (c_int, [c_void_p, c_int64, c_void_p, c_int64] + [c_void_p] * 3 + [c_size_t, c_void_p, c_void_p]),
-    "goslam_mesh_cull_emit": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_int64, c_void_p,
-                                      c_int64, c_void_p]),
-    "goslam_neus_vertex_color": (c_int, [ctypes.POINTER(NeusParams), c_void_p, c_int64, c_void_p, c_void_p]),
-    "goslam_mesh_cull_mask_count": (c_int, [c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
-                                            c_void_p]),
-    "goslam_mesh_cull_vertex_ids": (c_int, [c_int64, c_int64, c_void_p, c_size_t, c_void_p, c_int64, c_void_p]),
-    "goslam_mesh_depth_render": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p] + [c_int] * 3 +
-                                 [ctypes.c_double] * 6 + [c_void_p, c_void_p]),
-    "goslam_mesh_view_masks": (c_int, [c_void_p, c_int64, c_void_p, c_void_p] + [c_int] * 3 + [c_float] * 6 +
-                               [c_void_p] * 3),
-    "goslam_mesh_components_workspace_bytes": (c_size_t, [c_int64, c_int64]),
-    "goslam_mesh_components_count": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p]),
-    "goslam_mesh_components_keep": (c_int, [c_int64, c_int64, ctypes.c_double, c_int, c_void_p, c_size_t, c_void_p,
-                                            c_void_p]),
-    "goslam_sample_z": (c_int, [c_void_p] * 7 + [c_int] * 4 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "goslam_cvx_upsample": (c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 4 + [c_void_p]),
-    "goslam_proximity_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_proximity_edges": (c_int, [c_void_p] + [c_int] * 5 + [c_float, c_float, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                                               c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
-                                                               c_size_t, c_void_p]),
-    "goslam_conv_gru_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_conv_gru": (c_int, [ctypes.POINTER(GruWeights)] + [c_void_p] * 5 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p]),
-    "goslam_nchw_to_nhwc_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p]),
-    "goslam_nhwc_to_nchw_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p]),
-    "goslam_nchw_to_nhwc_f16_pad": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
-    "goslam_conv2d_nhwc": (c_int, [ctypes.POINTER(ConvDesc)] + [c_int] * 3 + [c_void_p]),
-    "goslam_update_op_workspace_bytes": (c_size_t, [c_int] * 4),
-    "goslam_update_op": (c_int, [ctypes.POINTER(UpdateWeights)] + [c_void_p] * 5 + [c_int] * 4 + [c_void_p] * 5 +
-                         [c_void_p, c_size_t, c_void_p]),
-    "goslam_mapping_snapshot_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_mapping_snapshot": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_float, c_void_p,
-                                                                        c_size_t, c_void_p, c_void_p]),
-    "goslam_mapping_rays": (c_int, [c_void_p, c_size_t] + [c_int] * 3 + [c_void_p, c_void_p, c_int64, c_int] +
-                            [c_void_p] * 3 + [ctypes.c_double] * 4 + [c_void_p] * 4 + [c_int64, c_void_p]),
-    "goslam_mapping_all_rays": (c_int, [c_void_p, c_int, c_int] + [ctypes.c_double] * 4 + [c_void_p] * 3),
-    "goslam_encoder_workspace_bytes": (c_size_t, [c_int] * 4),
-    "goslam_basic_encoder": (c_int, [ctypes.POINTER(EncoderWeights), c_int, c_int, c_void_p, c_int, c_void_p, c_void_p] +
-                             [c_int] * 3 + [c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
-    "goslam_fill_interpolate": (c_int, [c_void_p] * 5 + [c_int, c_int] + [c_void_p] * 3 + [c_int, c_int] +
-                                [c_void_p] * 3),
-    "goslam_mesh_sample_workspace_bytes": (c_size_t, [c_int64]),
-    "goslam_mesh_sample_surface": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
-                                           c_void_p, c_size_t, c_void_p]),
-    "goslam_nn_index_workspace_bytes": (c_size_t, [c_int64]),
-    "goslam_nn_index_build": (c_int, [c_void_p, c_int64, ctypes.c_double, c_void_p, c_size_t, c_void_p]),
-    "goslam_nn_query": (c_int, [c_void_p, c_size_t, c_int64, c_void_p, c_int64, ctypes.c_double, c_void_p, c_void_p,
-                                c_void_p]),
-    "goslam_nn_distance_stats": (c_int, [c_void_p, c_int64, ctypes.c_double, c_void_p, c_void_p]),
-    "goslam_icp_workspace_bytes": (c_size_t, [c_int64]),
-    "goslam_icp_point_to_point": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, c_int64, ctypes.c_double, c_void_p, c_int,
-                                          ctypes.c_double, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "goslam_mapping_points_workspace_bytes": (c_size_t, [c_int] * 3),
-    "goslam_mapping_points_count": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p, c_void_p]),
-    "goslam_mapping_points_emit": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p, c_size_t, c_void_p, c_int64,
-                                                                          c_void_p]),
-    "goslam_hull_workspace_bytes": (c_size_t, [c_int64]),
-    "goslam_hull_vertices": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p]),
-    "goslam_hull_vertices_emit": (c_int, [c_void_p, c_size_t, c_int64, c_void_p, c_int64, c_void_p]),
-    "goslam_obb_from_hull": (c_int, [c_void_p, c_int64, c_void_p, c_size_t, ctypes.c_double, c_void_p, c_void_p]),
-    "goslam_obb_in_bound": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "goslam_ape_workspace_bytes": (c_size_t, [c_int64]),
-    "goslam_ape_sim3": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
-    "goslam_corr_index_backward": (c_int, []),
-    "goslam_altcorr_backward": (c_int, []),
-}
+# C struct name -> its Structure above; a pointer to one binds as ctypes.POINTER of it
+STRUCTS = {"goslam_neus_params": NeusParams, "goslam_neus_out": NeusOut, "goslam_neus_mlp_bwd_out": NeusMlpBwdOut,
+           "goslam_ba_peers": BaPeers, "goslam_gru_weights": GruWeights, "goslam_update_weights": UpdateWeights,
+           "goslam_conv_desc": ConvDesc, "goslam_encoder_conv": EncoderConv, "goslam_encoder_weights": EncoderWeights}
+
+_SCALARS = {"void": None, "int": c_int, "unsigned": ctypes.c_uint, "float": c_float, "double": ctypes.c_double,
+            "size_t": c_size_t, "int64_t": c_int64, "long long": c_int64}
+
+
+def _ctype(decl, proto):
+    """the ctypes type of a C type without a name ('const float* ', 'int64_t', ...)"""
+    stars = decl.count("*")
+    base = " ".join(w for w in decl.replace("*", " ").split() if w != "const")
+    if stars == 0 and base in _SCALARS:
+        return _SCALARS[base]
+    if stars == 1 and base == "char":
+        return ctypes.c_char_p
+    if stars == 1 and base in STRUCTS:
+        return ctypes.POINTER(STRUCTS[base])
+    if stars > 0 and base:
+        return c_void_p
+    raise ValueError("%s: no ctypes binding for the C type %r" % (proto, decl.strip()))
+
+
+def parse_header(text):
+    """name -> (restype, argtypes, takes_stream) of every goslam_* prototype in the header text; takes_stream: the last
+    parameter is `void* stream`"""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#[^\n]*", " ", text, flags=re.M)
+    text = re.sub(r"\btypedef\s+struct\b[^{;]*\{.*?\}\s*\w+\s*;", " ", text, flags=re.S)
+    sigs = {}
+    for ret, name, params in re.findall(r"([\w\s*]+?)\b(goslam_\w+)\s*\(([^()]*)\)\s*;", text):
+        decls = [p.strip() for p in params.split(",")]
+        if decls == ["void"]:
+            decls = []
+        argtypes = []
+        for d in decls:
+            m = re.fullmatch(r"(.*?)\b[A-Za-z_]\w*", d, flags=re.S)      # the type, without the parameter name
+            argtypes.append(_ctype(m.group(1) if m else d, name))
+        stream = bool(decls) and re.sub(r"\s+", "", decls[-1]) == "void*stream"
+        sigs[name] = (_ctype(ret, name), argtypes, stream)
+    return sigs
 
 
 def lib_path():
@@ -203,7 +128,7 @@ def lib_path():
 
 
 def load(build_if_missing=True):
-    """Return the loaded CDLL (building it first if the .so is absent)."""
+    """Return the loaded CDLL (building it first if the .so is absent), bound as the header declares it."""
     global _LIB
     with _lock:
         if _LIB is not None:
@@ -214,11 +139,16 @@ def load(build_if_missing=True):
                 raise RuntimeError("libgoslam_b200.so not built (run python -m __graft_entry__ or "
                                    "go-slam_b200/build.py)")
             _build.build()
+        with open(HEADER) as f:
+            sigs = parse_header(f.read())
         lib = ctypes.CDLL(path)
-        for name, (res, args) in SIGNATURES.items():
+        for name, (res, args, stream) in sigs.items():
             fn = getattr(lib, name)          # AttributeError => header/library mismatch
             fn.restype = res
             fn.argtypes = args
+            SIGNATURES[name] = (res, args)
+            if stream:
+                _TAKES_STREAM.add(name)
         _LIB = lib
         return lib
 
@@ -231,11 +161,65 @@ def check(rc, what):
                                                           ": " + detail.decode() if detail else ""))
 
 
+def call(name, *args, device=None):
+    """goslam_<name>(*args) for an entry that returns an int status.  A tensor goes as its device pointer (a CPU tensor
+    raises), None as NULL, anything else (ctypes objects, ints, floats) as it is.  Runs on `device`, else on the device
+    of the first tensor, else on the current device, and appends that device's current stream when the prototype ends
+    in `void* stream`; raises RuntimeError on a non-zero status.  It neither synchronises, allocates nor queries the
+    device, so it may run inside a CUDA graph capture.  The tensors stay referenced until the launch has been issued."""
+    fname = "goslam_" + name
+    fn = getattr(_LIB or load(), fname)
+    conv = list(args)
+    dev = device
+    for i, a in enumerate(conv):
+        if isinstance(a, torch.Tensor):
+            if not a.is_cuda:
+                raise RuntimeError("%s: tensors must live on a CUDA device (there is no CPU fallback)" % fname)
+            if dev is None:
+                dev = a.device
+            conv[i] = a.data_ptr()
+    with torch.cuda.device(dev):
+        if fname in _TAKES_STREAM:
+            conv.append(torch.cuda.current_stream().cuda_stream)
+        rc = fn(*conv)
+    check(rc, name)
+
+
+def workspace(nbytes, device):
+    """grow-only per-device scratch (borrowed for the duration of one call on the current stream)."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
+    buf = _ws_cache.get(key)
+    if buf is None or buf.numel() < nbytes:
+        buf = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+        _ws_cache[key] = buf
+    return buf
+
+
+def need_cuda(what, *ts):
+    for t in ts:
+        if t is not None and not t.is_cuda:
+            raise RuntimeError("%s: tensors must live on a CUDA device (there is no CPU fallback)" % what)
+
+
+def contig(**kw):
+    for name, t in kw.items():
+        if not t.is_contiguous():
+            raise RuntimeError("%s must be contiguous" % name)
+
+
+def ptr_array(tensors):
+    """host array of the tensors' device pointers (the library's `const void* const*` parameters)"""
+    need_cuda("ptr_array", *tensors)
+    arr = (ctypes.c_void_p * len(tensors))()
+    for i, t in enumerate(tensors):
+        arr[i] = t.data_ptr()
+    return arr
+
+
 def ptr(t):
     """device pointer of a torch tensor (or None)."""
     return None if t is None else c_void_p(t.data_ptr())
 
 
 def stream_ptr():
-    import torch
     return c_void_p(torch.cuda.current_stream().cuda_stream)

@@ -11,36 +11,14 @@ module the reference builds from src/lib/*.cu:
 
 Install under the reference's import name with `goslam_b200.install()`.
 """
-import ctypes
-
 import torch
 
 from . import _lib
-
-_ws_cache = {}
+from ._lib import contig as _contig
 
 
 def _need_cuda(*ts):
-    for t in ts:
-        if t is not None and not t.is_cuda:
-            raise RuntimeError("goslam_b200.droid_backends: tensors must live on a CUDA device "
-                               "(there is no CPU fallback)")
-
-
-def _contig(**kw):
-    for name, t in kw.items():
-        if not t.is_contiguous():
-            raise RuntimeError("%s must be contiguous" % name)
-
-
-def _workspace(nbytes, device):
-    """grow-only per-device scratch (borrowed for the duration of one call on the current stream)."""
-    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
-    buf = _ws_cache.get(key)
-    if buf is None or buf.numel() < nbytes:
-        buf = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
-        _ws_cache[key] = buf
-    return buf
+    _lib.need_cuda("goslam_b200.droid_backends", *ts)
 
 
 def _dtype_code(t):
@@ -59,12 +37,7 @@ def corr_index_forward(volume, coords, radius):
     N, h1, w1, h2, w2 = volume.shape
     rd = 2 * radius + 1
     corr = torch.empty((N, rd, rd, h1, w1), dtype=volume.dtype, device=volume.device)
-    coords_f = coords.float()          # named: a converted copy must outlive the launch
-    with torch.cuda.device(volume.device):
-        rc = _lib.load().goslam_corr_index_forward(
-            _lib.ptr(volume), _dtype_code(volume), _lib.ptr(coords_f), _lib.ptr(corr),
-            N, h1, w1, h2, w2, int(radius), _lib.stream_ptr())
-    _lib.check(rc, "corr_index_forward")
+    _lib.call("corr_index_forward", volume, _dtype_code(volume), coords.float(), corr, N, h1, w1, h2, w2, int(radius))
     return [corr]
 
 
@@ -86,11 +59,7 @@ def altcorr_forward(fmap1, fmap2, coords, radius):
     S = coords.shape[1]
     rd = 2 * radius + 1
     corr = torch.empty((B, S, rd * rd, H, W), dtype=torch.float32, device=fmap1.device)
-    with torch.cuda.device(fmap1.device):
-        rc = _lib.load().goslam_altcorr_forward(
-            _lib.ptr(fmap1), _lib.ptr(fmap2), _lib.ptr(coords), _lib.ptr(corr),
-            B, S, H, W, H2, W2, C, int(radius), _lib.stream_ptr())
-    _lib.check(rc, "altcorr_forward")
+    _lib.call("altcorr_forward", fmap1, fmap2, coords, corr, B, S, H, W, H2, W2, C, int(radius))
     return [corr]
 
 
@@ -108,11 +77,7 @@ def frame_distance(poses, disps, intrinsics, ii, jj, beta):
     K = ii.shape[0]
     ht, wd = disps.shape[1], disps.shape[2]
     dist = torch.empty((K,), dtype=torch.float32, device=poses.device)
-    with torch.cuda.device(poses.device):
-        rc = _lib.load().goslam_frame_distance(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), _lib.ptr(ii), _lib.ptr(jj),
-            _lib.ptr(dist), K, ht, wd, float(beta), _lib.stream_ptr())
-    _lib.check(rc, "frame_distance")
+    _lib.call("frame_distance", poses, disps, intrinsics, ii, jj, dist, K, ht, wd, float(beta))
     return dist
 
 
@@ -124,11 +89,7 @@ def frame_distance_bidirectional(poses, disps, intrinsics, ii, jj, beta):
     K = ii.shape[0]
     ht, wd = disps.shape[1], disps.shape[2]
     dist = torch.empty((K,), dtype=torch.float32, device=poses.device)
-    with torch.cuda.device(poses.device):
-        rc = _lib.load().goslam_frame_distance_bidir(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), _lib.ptr(ii), _lib.ptr(jj),
-            _lib.ptr(dist), K, ht, wd, float(beta), _lib.stream_ptr())
-    _lib.check(rc, "frame_distance_bidir")
+    _lib.call("frame_distance_bidir", poses, disps, intrinsics, ii, jj, dist, K, ht, wd, float(beta))
     return dist
 
 
@@ -144,14 +105,10 @@ def frame_distance_grid(poses, disps, intrinsics, r0, r1, c0, c1, k, beta):
                            % (r0, r1, c0, c1, min(poses.shape[0], disps.shape[0])))
     ht, wd = disps.shape[1], disps.shape[2]
     dist = torch.empty((max(r1 - r0, 0), max(c1 - c0, 0)), dtype=torch.float32, device=poses.device)
-    lib = _lib.load()
-    with torch.cuda.device(poses.device):
-        nbytes = lib.goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1)
-        ws = _workspace(nbytes, poses.device) if nbytes else None
-        rc = lib.goslam_frame_distance_grid(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), r0, r1, c0, c1, int(k), ht, wd, float(beta),
-            _lib.ptr(dist), _lib.ptr(ws), ctypes.c_size_t(0 if ws is None else ws.numel()), _lib.stream_ptr())
-    _lib.check(rc, "frame_distance_grid")
+    nbytes = _lib.load().goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1)
+    ws = _lib.workspace(nbytes, poses.device) if nbytes else None
+    _lib.call("frame_distance_grid", poses, disps, intrinsics, r0, r1, c0, c1, int(k), ht, wd, float(beta), dist, ws,
+              0 if ws is None else ws.numel())
     return dist
 
 
@@ -163,11 +120,7 @@ def projmap(poses, disps, intrinsics, ii, jj):
     ht, wd = disps.shape[1], disps.shape[2]
     coords = torch.empty((K, ht, wd, 3), dtype=torch.float32, device=poses.device)
     valid = torch.empty((K, ht, wd, 1), dtype=torch.float32, device=poses.device)
-    with torch.cuda.device(poses.device):
-        rc = _lib.load().goslam_projmap(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), _lib.ptr(ii), _lib.ptr(jj),
-            _lib.ptr(coords), _lib.ptr(valid), K, ht, wd, _lib.stream_ptr())
-    _lib.check(rc, "projmap")
+    _lib.call("projmap", poses, disps, intrinsics, ii, jj, coords, valid, K, ht, wd)
     return [coords, valid]
 
 
@@ -177,10 +130,7 @@ def iproj(poses, disps, intrinsics):
     _need_cuda(poses, disps, intrinsics)
     num, ht, wd = disps.shape
     points = torch.empty((num, ht, wd, 3), dtype=torch.float32, device=disps.device)
-    with torch.cuda.device(disps.device):
-        rc = _lib.load().goslam_iproj(_lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics),
-                                      _lib.ptr(points), num, ht, wd, _lib.stream_ptr())
-    _lib.check(rc, "iproj")
+    _lib.call("iproj", poses, disps, intrinsics, points, num, ht, wd)
     return points
 
 
@@ -191,11 +141,7 @@ def depth_filter(poses, disps, intrinsics, ix, thresh):
     K = ix.shape[0]
     num, ht, wd = disps.shape
     counter = torch.empty((K, ht, wd), dtype=torch.float32, device=disps.device)
-    with torch.cuda.device(disps.device):
-        rc = _lib.load().goslam_depth_filter(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), _lib.ptr(ix), _lib.ptr(thresh),
-            _lib.ptr(counter), K, num, ht, wd, _lib.stream_ptr())
-    _lib.check(rc, "depth_filter")
+    _lib.call("depth_filter", poses, disps, intrinsics, ix, thresh, counter, K, num, ht, wd)
     return counter
 
 
@@ -208,11 +154,7 @@ def reproject(poses, disps, intrinsics_all, ii, jj, want_valid=True):
     ht, wd = disps.shape[1], disps.shape[2]
     coords = torch.empty((1, K, ht, wd, 2), dtype=torch.float32, device=poses.device)
     valid = torch.empty((1, K, ht, wd, 1), dtype=torch.float32, device=poses.device) if want_valid else None
-    with torch.cuda.device(poses.device):
-        rc = _lib.load().goslam_reproject(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics_all), _lib.ptr(ii), _lib.ptr(jj),
-            _lib.ptr(coords), _lib.ptr(valid), K, ht, wd, _lib.stream_ptr())
-    _lib.check(rc, "reproject")
+    _lib.call("reproject", poses, disps, intrinsics_all, ii, jj, coords, valid, K, ht, wd)
     return coords, valid
 
 
@@ -227,11 +169,7 @@ def reproject_motion(poses, disps, intrinsics_all, ii, jj, target):
         raise RuntimeError("reproject_motion: target must be float32 [1, N, ht, wd, 2]")
     coords = torch.empty((1, K, ht, wd, 2), dtype=torch.float32, device=poses.device)
     motion = torch.empty((1, K, 4, ht, wd), dtype=torch.float32, device=poses.device)
-    with torch.cuda.device(poses.device):
-        rc = _lib.load().goslam_reproject_motion(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics_all), _lib.ptr(ii), _lib.ptr(jj),
-            _lib.ptr(target), _lib.ptr(coords), None, _lib.ptr(motion), K, ht, wd, _lib.stream_ptr())
-    _lib.check(rc, "reproject_motion")
+    _lib.call("reproject_motion", poses, disps, intrinsics_all, ii, jj, target, coords, None, motion, K, ht, wd)
     return coords, motion
 
 
@@ -261,7 +199,6 @@ def ba(poses, disps, intrinsics, disps_sens, targets, weights, eta, ii, jj,
     num, ht, wd = disps.shape
     t0, t1 = int(t0), int(t1)
     P = max(t1 - t0, 0)
-    lib = _lib.load()
     eta_c = None
     eta_rows = 0
     if not motion_only:
@@ -274,19 +211,12 @@ def ba(poses, disps, intrinsics, disps_sens, targets, weights, eta, ii, jj,
     dx = torch.zeros((P, 6), dtype=torch.float32, device=dev)
     dz = None if motion_only else torch.empty((num, ht * wd), dtype=torch.float32, device=dev)
     status = torch.zeros((max(int(iterations), 1),), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        nbytes = lib.goslam_ba_workspace_bytes(N, num, ht, wd, t0, t1)
-        if nbytes == 0:
-            raise RuntimeError("ba: invalid shapes (N=%d num=%d t0=%d t1=%d)" % (N, num, t0, t1))
-        ws = _workspace(nbytes, dev)
-        rc = lib.goslam_ba(
-            _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(intrinsics), _lib.ptr(disps_sens),
-            _lib.ptr(targets), _lib.ptr(weights), _lib.ptr(eta_c), eta_rows,
-            _lib.ptr(ii), _lib.ptr(jj), N, num, ht, wd, t0, t1, int(iterations),
-            float(lm), float(ep), int(bool(motion_only)),
-            _lib.ptr(dx), _lib.ptr(dz), _lib.ptr(status),
-            _lib.ptr(ws), ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-    _lib.check(rc, "ba")
+    nbytes = _lib.load().goslam_ba_workspace_bytes(N, num, ht, wd, t0, t1)
+    if nbytes == 0:
+        raise RuntimeError("ba: invalid shapes (N=%d num=%d t0=%d t1=%d)" % (N, num, t0, t1))
+    ws = _lib.workspace(nbytes, dev)
+    _lib.call("ba", poses, disps, intrinsics, disps_sens, targets, weights, eta_c, eta_rows, ii, jj, N, num, ht, wd,
+              t0, t1, int(iterations), float(lm), float(ep), int(bool(motion_only)), dx, dz, status, ws, ws.numel())
     if return_status:
         return [dx, dz, status]
     return [dx, dz]

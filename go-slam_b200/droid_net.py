@@ -11,18 +11,14 @@ from . import _lib
 
 def cvx_upsample(data, mask):
     """data [b, ht, wd, dim] (dim <= 4), mask [b, 9*8*8, ht, wd] (f16 or f32) -> [b, 8ht, 8wd, dim] f32."""
-    if not data.is_cuda:
-        raise RuntimeError("cvx_upsample: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("cvx_upsample", data)
     batch, ht, wd, dim = data.shape
     d = data.float().contiguous()
     m = mask.reshape(batch, 576, ht, wd).contiguous()
     if m.dtype not in (torch.float16, torch.float32):
         m = m.float()
     out = torch.empty((batch, 8 * ht, 8 * wd, dim), dtype=torch.float32, device=data.device)
-    with torch.cuda.device(data.device):
-        rc = _lib.load().goslam_cvx_upsample(_lib.ptr(d), _lib.ptr(m), 1 if m.dtype == torch.float16 else 0,
-                                             _lib.ptr(out), batch, ht, wd, dim, _lib.stream_ptr())
-    _lib.check(rc, "cvx_upsample")
+    _lib.call("cvx_upsample", d, m, 1 if m.dtype == torch.float16 else 0, out, batch, ht, wd, dim)
     return out
 
 
@@ -111,7 +107,6 @@ class UpdateModule(nn.Module):
 
     def _pack(self):
         """kernel-side weights of every layer (include/goslam_b200.h: goslam_update_weights), cached per parameter version"""
-        from . import _lib
         from .modules.gru import pack_conv
         params = list(self.parameters())
         key = tuple((p.data_ptr(), p._version) for p in params)
@@ -154,11 +149,8 @@ class UpdateModule(nn.Module):
         net', delta [batch, num, h, w, 2], weight [batch, num, h, w, 2] (, eta [batch, M, h, w], upmask [batch, M, 576, h, w]
         when ii is given; M = distinct source frames, sorted) — src/droid_net.py:107-140.  One library call."""
         import ctypes
-        from . import _lib
-        from .droid_backends import _workspace
         batch, num, ch, ht, wd = net.shape
-        if not net.is_cuda:
-            raise RuntimeError("UpdateModule: CUDA tensors required (no CPU fallback)")
+        _lib.need_cuda("UpdateModule", net)
         if batch != 1:
             raise RuntimeError("UpdateModule: batch 1 (as GO-SLAM calls it)")
         dev = net.device
@@ -181,14 +173,9 @@ class UpdateModule(nn.Module):
         weight = torch.empty((1, N, ht, wd, 2), dtype=torch.float32, device=dev)
         eta = torch.empty((1, M, ht, wd), dtype=torch.float32, device=dev) if slot is not None else None
         upmask = torch.empty((1, M, 576, ht, wd), dtype=torch.float16, device=dev) if slot is not None else None
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            ws = _workspace(lib.goslam_update_op_workspace_bytes(N, M, ht, wd), dev)
-            rc = lib.goslam_update_op(ctypes.byref(st), _lib.ptr(net_c), _lib.ptr(inp_c), _lib.ptr(corr_c), _lib.ptr(flow_c),
-                                      _lib.ptr(slot), N, M, ht, wd, _lib.ptr(net_out), _lib.ptr(delta), _lib.ptr(weight),
-                                      _lib.ptr(eta), _lib.ptr(upmask), _lib.ptr(ws), ctypes.c_size_t(ws.numel()),
-                                      _lib.stream_ptr())
-        _lib.check(rc, "update_op")
+        ws = _lib.workspace(_lib.load().goslam_update_op_workspace_bytes(N, M, ht, wd), dev)
+        _lib.call("update_op", ctypes.byref(st), net_c, inp_c, corr_c, flow_c, slot, N, M, ht, wd, net_out, delta, weight,
+                  eta, upmask, ws, ws.numel())
         net_out = net_out.to(net.dtype)
         if slot is None:
             return net_out, delta, weight

@@ -11,13 +11,11 @@ device->host sync per candidate.  It returns the `(ii, jj)` the reference hands 
                                                self.video.stereo, ii1, jj1)
     self.add_factors(ii, jj, remove)
 """
-import ctypes
 import math
 
 import torch
 
 from . import _lib
-from .droid_backends import _workspace
 
 
 def local_edge_count(t0, t, rad, stereo, jfloor=0):
@@ -38,8 +36,7 @@ def backend_edges(dist, t_start, t_end, radius, nms, thresh, max_factors, stereo
 
 def proximity_edges(dist, t0, t1, t, rad, nms, thresh, max_factors, stereo, ii_old, jj_old, dmax=100.0, jfloor=0,
                     loop=False):
-    if not dist.is_cuda:
-        raise RuntimeError("proximity_edges: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("proximity_edges", dist)
     dev = dist.device
     d = dist.reshape(-1).float().contiguous()
     if d.numel() != (t - t0) * (t - t1):
@@ -51,18 +48,12 @@ def proximity_edges(dist, t0, t1, t, rad, nms, thresh, max_factors, stereo, ii_o
     es_i = torch.empty(cap, dtype=torch.int64, device=dev)
     es_j = torch.empty(cap, dtype=torch.int64, device=dev)
     num = torch.zeros(1, dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        nbytes = lib.goslam_proximity_workspace_bytes(int(t0), int(t1), int(t))
-        if nbytes == 0:
-            raise RuntimeError("proximity_edges: empty window (t0=%d t1=%d t=%d)" % (t0, t1, t))
-        ws = _workspace(nbytes, dev)
-        rc = lib.goslam_proximity_edges(_lib.ptr(d), int(t0), int(t1), int(t), int(rad), int(nms), float(thresh),
-                                        float(dmax), int(jfloor), int(bool(loop)), mf,
-                                        int(bool(stereo)), _lib.ptr(io), _lib.ptr(jo), int(io.numel()),
-                                        _lib.ptr(es_i), _lib.ptr(es_j), cap, _lib.ptr(num), _lib.ptr(ws),
-                                        ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-    _lib.check(rc, "proximity_edges")
+    nbytes = _lib.load().goslam_proximity_workspace_bytes(int(t0), int(t1), int(t))
+    if nbytes == 0:
+        raise RuntimeError("proximity_edges: empty window (t0=%d t1=%d t=%d)" % (t0, t1, t))
+    ws = _lib.workspace(nbytes, dev)
+    _lib.call("proximity_edges", d, int(t0), int(t1), int(t), int(rad), int(nms), float(thresh), float(dmax), int(jfloor),
+              int(bool(loop)), mf, int(bool(stereo)), io, jo, int(io.numel()), es_i, es_j, cap, num, ws, ws.numel())
     n = int(num.item())            # the one host sync (the reference builds its edge tensor on the host here)
     return es_i[:n], es_j[:n]
 

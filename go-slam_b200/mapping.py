@@ -116,23 +116,18 @@ def snapshot_frames(video, frames, decay):
     F = len(order)
     if F == 0:
         return Snapshot([], [], torch.empty((0, 4, 4), device=dev), None, H, W)
-    lib = _lib.load()
-    nbytes = int(lib.goslam_mapping_snapshot_workspace_bytes(F, H, W))
+    nbytes = int(_lib.load().goslam_mapping_snapshot_workspace_bytes(F, H, W))
     if nbytes == 0:
         raise RuntimeError("snapshot_frames: invalid size (%d frames of %d x %d)" % (F, H, W))
     ws = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
     counts = torch.empty((F,), dtype=torch.int32, device=dev)
     ids = torch.tensor([order, occ], dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
-    with torch.cuda.device(dev):
-        with video.mapping.get_lock():
-            rc = lib.goslam_mapping_snapshot(
-                _lib.ptr(video.images), _lib.ptr(video.mask_filtered), _lib.ptr(video.disps_filtered),
-                _lib.ptr(video.update_priority), buffer, H, W, _lib.ptr(ids[0]), _lib.ptr(ids[1]), F, float(decay),
-                _lib.ptr(ws), ctypes.c_size_t(nbytes), _lib.ptr(counts), _lib.stream_ptr())
-            _lib.check(rc, "mapping_snapshot")
-            poses = video.poses_filtered.index_select(0, ids[0].long())
-            comp = video.pose_compensate[0:1].clone()
-            n_f = counts.tolist()
+    with video.mapping.get_lock():
+        _lib.call("mapping_snapshot", video.images, video.mask_filtered, video.disps_filtered, video.update_priority,
+                  buffer, H, W, ids[0], ids[1], F, float(decay), ws, nbytes, counts)
+        poses = video.poses_filtered.index_select(0, ids[0].long())
+        comp = video.pose_compensate[0:1].clone()
+        n_f = counts.tolist()
     c2w = (lietorch.SE3(comp) * lietorch.SE3(poses).inv()).matrix().contiguous()
     return Snapshot(order, n_f, c2w, ws, H, W)
 
@@ -163,28 +158,20 @@ def build_ray_batch(snapshot, frame_list, n_rays, intrinsics):
     if plan.R > 0:
         n = len(slots)
         arr = ctypes.c_int * n
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_mapping_rays(
-                _lib.ptr(snapshot.workspace), ctypes.c_size_t(snapshot.workspace.numel()), len(snapshot.frames),
-                snapshot.H, snapshot.W, _lib.ptr(snapshot.c2w), _lib.ptr(draws), plan.n_draws, n, arr(*slots),
-                arr(*counts), arr(*plan.draw), fx, fy, cx, cy, _lib.ptr(rays_o), _lib.ptr(rays_d), _lib.ptr(depth),
-                _lib.ptr(color), plan.R, _lib.stream_ptr())
-        _lib.check(rc, "mapping_rays")
+        _lib.call("mapping_rays", snapshot.workspace, snapshot.workspace.numel(), len(snapshot.frames), snapshot.H,
+                  snapshot.W, snapshot.c2w, draws, plan.n_draws, n, arr(*slots), arr(*counts), arr(*plan.draw), fx, fy,
+                  cx, cy, rays_o, rays_d, depth, color, plan.R)
     return RayBatch(rays_o, rays_d, depth, color, draws)
 
 
 def all_rays(H, W, intrinsics, c2w):
     """build_all_rays(H, W, fx, fy, cx, cy, c2w, nerf_coordinate=False) flattened: rays_o, rays_d [H*W,3]"""
     fx, fy, cx, cy = [float(v) for v in intrinsics]
-    if not c2w.is_cuda:
-        raise RuntimeError("all_rays: c2w must be a CUDA tensor (no CPU fallback)")
+    _lib.need_cuda("all_rays", c2w)
     m = c2w.detach().to(torch.float32).contiguous()
     rays_o = torch.empty((H * W, 3), dtype=torch.float32, device=m.device)
     rays_d = torch.empty((H * W, 3), dtype=torch.float32, device=m.device)
-    with torch.cuda.device(m.device):
-        rc = _lib.load().goslam_mapping_all_rays(_lib.ptr(m), int(H), int(W), fx, fy, cx, cy, _lib.ptr(rays_o),
-                                                 _lib.ptr(rays_d), _lib.stream_ptr())
-    _lib.check(rc, "mapping_all_rays")
+    _lib.call("mapping_all_rays", m, int(H), int(W), fx, fy, cx, cy, rays_o, rays_d)
     return rays_o, rays_d
 
 

@@ -21,14 +21,12 @@ import numpy as np
 import torch
 
 from . import _lib
-from .droid_backends import _workspace
 
 DEPTH_CHUNK_BYTES = 256 << 20          # default bound of the depth scratch of view_masks
 
 
 def _mesh_args(verts, faces):
-    if not verts.is_cuda:
-        raise RuntimeError("mesher: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("mesher", verts)
     verts = verts.detach().to(torch.float64).reshape(-1, 3).contiguous()
     faces = faces.detach().to(device=verts.device, dtype=torch.int64).reshape(-1, 3).contiguous()
     return verts, faces
@@ -47,15 +45,10 @@ def render_depth(verts, faces, c2w, H, W, fx, fy, cx, cy, near=0.001, far=20.0):
     c2w = _poses(c2w, dev)
     K = c2w.shape[0]
     depth = torch.empty((K, int(H), int(W)), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        for k0 in range(0, K, 65535):
-            k1 = min(K, k0 + 65535)
-            rc = lib.goslam_mesh_depth_render(_lib.ptr(verts), verts.shape[0], _lib.ptr(faces), faces.shape[0],
-                                              _lib.ptr(c2w[k0:k1]), k1 - k0, int(H), int(W), float(fx), float(fy),
-                                              float(cx), float(cy), float(near), float(far), _lib.ptr(depth[k0:k1]),
-                                              _lib.stream_ptr())
-            _lib.check(rc, "mesh_depth_render")
+    for k0 in range(0, K, 65535):
+        k1 = min(K, k0 + 65535)
+        _lib.call("mesh_depth_render", verts, verts.shape[0], faces, faces.shape[0], c2w[k0:k1], k1 - k0, int(H), int(W),
+                  float(fx), float(fy), float(cx), float(cy), float(near), float(far), depth[k0:k1])
     return depth
 
 
@@ -72,42 +65,33 @@ def view_masks(verts, faces, c2w, H, W, fx, fy, cx, cy, radius, eps=0.05, chunk=
     chunk = max(1, min(int(chunk), 65535))
     seen = torch.zeros(V, dtype=torch.uint8, device=dev)
     fore = torch.zeros(V, dtype=torch.uint8, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        for k0 in range(0, K, chunk):
-            k1 = min(K, k0 + chunk)
-            depth = render_depth(verts, faces, c2w[k0:k1], H, W, fx, fy, cx, cy, far=20.0)
-            w2c = torch.inverse(c2w[k0:k1]).float().contiguous()      # the reference's call, on the device
-            rc = lib.goslam_mesh_view_masks(_lib.ptr(verts), V, _lib.ptr(w2c), _lib.ptr(depth), k1 - k0, H, W,
-                                            float(fx), float(fy), float(cx), float(cy), float(radius), float(eps),
-                                            _lib.ptr(seen), _lib.ptr(fore), _lib.stream_ptr())
-            _lib.check(rc, "mesh_view_masks")
-            del depth
+    for k0 in range(0, K, chunk):
+        k1 = min(K, k0 + chunk)
+        depth = render_depth(verts, faces, c2w[k0:k1], H, W, fx, fy, cx, cy, far=20.0)
+        w2c = torch.inverse(c2w[k0:k1]).float().contiguous()      # the reference's call, on the device
+        _lib.call("mesh_view_masks", verts, V, w2c, depth, k1 - k0, H, W, float(fx), float(fy), float(cx), float(cy),
+                  float(radius), float(eps), seen, fore)
+        del depth
     return seen.bool(), fore.bool()
 
 
 def _compact(verts, faces, colors, count):
-    """run `count(lib, workspace, counts, stream)` (a cull count entry), then the emit, the kept vertices' ids and the
-    colour gather.  One host synchronisation (the two counts)."""
-    lib = _lib.load()
+    """run `count(workspace, counts)` (a cull count entry), then the emit, the kept vertices' ids and the colour gather.
+    One host synchronisation (the two counts)."""
     nv, nf = verts.shape[0], faces.shape[0]
     dev = verts.device
-    with torch.cuda.device(dev):
-        st = _lib.stream_ptr()
-        ws = torch.empty(lib.goslam_mesh_cull_workspace_bytes(nv, nf), dtype=torch.uint8, device=dev)
-        counts = torch.empty(2, dtype=torch.int64, device=dev)
-        _lib.check(count(lib, ws, counts, st), "mesh cull count")
-        kv, kf = counts.tolist()
-        out_v = torch.empty((kv, 3), dtype=torch.float64, device=dev)
-        out_f = torch.empty((kf, 3), dtype=torch.int64, device=dev)
-        _lib.check(lib.goslam_mesh_cull_emit(_lib.ptr(verts), nv, _lib.ptr(faces), nf, _lib.ptr(ws), ws.numel(),
-                                             _lib.ptr(out_v), kv, _lib.ptr(out_f), kf, st), "mesh_cull_emit")
-        out_c = None
-        if colors is not None:
-            ids = torch.empty(kv, dtype=torch.int64, device=dev)
-            _lib.check(lib.goslam_mesh_cull_vertex_ids(nv, nf, _lib.ptr(ws), ws.numel(), _lib.ptr(ids), kv, st),
-                       "mesh_cull_vertex_ids")
-            out_c = colors.index_select(0, ids)
+    ws = torch.empty(_lib.load().goslam_mesh_cull_workspace_bytes(nv, nf), dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    count(ws, counts)
+    kv, kf = counts.tolist()
+    out_v = torch.empty((kv, 3), dtype=torch.float64, device=dev)
+    out_f = torch.empty((kf, 3), dtype=torch.int64, device=dev)
+    _lib.call("mesh_cull_emit", verts, nv, faces, nf, ws, ws.numel(), out_v, kv, out_f, kf)
+    out_c = None
+    if colors is not None:
+        ids = torch.empty(kv, dtype=torch.int64, device=dev)
+        _lib.call("mesh_cull_vertex_ids", nv, nf, ws, ws.numel(), ids, kv)
+        out_c = colors.index_select(0, ids)
     return out_v, out_f, out_c
 
 
@@ -136,18 +120,17 @@ def keep_faces(verts, faces, face_mask=None, colors=None, vert_mask=None):
     dev = verts.device
     fm, vm = _mask_arg(face_mask, faces.shape[0], dev), _mask_arg(vert_mask, verts.shape[0], dev)
     colors = _colors_arg(colors, verts.shape[0], dev)
-    return _compact(verts, faces, colors, lambda lib, ws, counts, st: lib.goslam_mesh_cull_mask_count(
-        verts.shape[0], _lib.ptr(faces), faces.shape[0], _lib.ptr(fm), _lib.ptr(vm), _lib.ptr(ws), ws.numel(),
-        _lib.ptr(counts), st))
+    return _compact(verts, faces, colors, lambda ws, counts: _lib.call(
+        "mesh_cull_mask_count", verts.shape[0], faces, faces.shape[0], fm, vm, ws, ws.numel(), counts))
 
 
-def _keep_box(verts, faces, lo, hi, colors=None):
-    """the bound cull of neus.cull_mesh (lo <= v <= hi, host float32 thresholds), colours carried along"""
+def keep_box(verts, faces, lo, hi, colors=None):
+    """the bound cull (lo <= v <= hi, host float32 thresholds) as (vertices, faces, colours or None), stable orders"""
+    verts, faces = _mesh_args(verts, faces)
     lo = (ctypes.c_float * 3)(*[float(v) for v in lo])
     hi = (ctypes.c_float * 3)(*[float(v) for v in hi])
-    return _compact(verts, faces, colors, lambda lib, ws, counts, st: lib.goslam_mesh_cull_count(
-        _lib.ptr(verts), verts.shape[0], _lib.ptr(faces), faces.shape[0], lo, hi, _lib.ptr(ws), ws.numel(),
-        _lib.ptr(counts), st))
+    return _compact(verts, faces, colors, lambda ws, counts: _lib.call(
+        "mesh_cull_count", verts, verts.shape[0], faces, faces.shape[0], lo, hi, ws, ws.numel(), counts))
 
 
 def component_mask(verts, faces, threshold, largest=False):
@@ -158,19 +141,16 @@ def component_mask(verts, faces, threshold, largest=False):
     keep = torch.zeros(nf, dtype=torch.uint8, device=dev)
     if nf == 0:
         return keep
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        st = _lib.stream_ptr()
-        nbytes = lib.goslam_mesh_components_workspace_bytes(nv, nf)
-        if nbytes == 0:
-            raise RuntimeError("mesh components: cannot size the workspace for %d faces" % nf)
-        ws = _workspace(nbytes, dev)
-        counts = torch.empty(1, dtype=torch.int64, device=dev)
-        _lib.check(lib.goslam_mesh_components_count(_lib.ptr(verts), nv, _lib.ptr(faces), nf, _lib.ptr(ws), ws.numel(),
-                                                    _lib.ptr(counts), st), "mesh_components_count")
-        n_comp = int(counts.item())
-        _lib.check(lib.goslam_mesh_components_keep(nf, n_comp, float(threshold), int(bool(largest)), _lib.ptr(ws),
-                                                   ws.numel(), _lib.ptr(keep), st), "mesh_components_keep")
+        # CUB sizes its scratch for the current device
+        nbytes = _lib.load().goslam_mesh_components_workspace_bytes(nv, nf)
+    if nbytes == 0:
+        raise RuntimeError("mesh components: cannot size the workspace for %d faces" % nf)
+    ws = _lib.workspace(nbytes, dev)
+    counts = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.call("mesh_components_count", verts, nv, faces, nf, ws, ws.numel(), counts)
+    n_comp = int(counts.item())
+    _lib.call("mesh_components_keep", nf, n_comp, float(threshold), int(bool(largest)), ws, ws.numel(), keep)
     return keep
 
 
@@ -221,7 +201,7 @@ def cull_mesh(self, mesh, estimate_c2w_list, bound, mesh_out_file):
         if bound is not None:
             if isinstance(bound, np.ndarray):
                 eps = 0.001
-                verts, faces, colors = _keep_box(verts, faces, bound[:, 0] - eps, bound[:, 1] + eps, colors)
+                verts, faces, colors = keep_box(verts, faces, bound[:, 0] - eps, bound[:, 1] + eps, colors)
             elif isinstance(bound, OrientedBoundingBox):
                 verts, faces, colors = keep_faces(verts, faces, colors=colors, vert_mask=bound.in_bound(verts))
             else:
@@ -255,8 +235,7 @@ def cull_mesh(self, mesh, estimate_c2w_list, bound, mesh_out_file):
 # ---- reconstruction evaluation (align_mesh / eval_mesh) -----------------------------------------------------------
 def _points(x, what):
     x = torch.as_tensor(x)
-    if not x.is_cuda:
-        raise RuntimeError("%s: CUDA tensors required (no CPU fallback)" % what)
+    _lib.need_cuda(what, x)
     x = x.detach().to(torch.float64).reshape(-1, 3).contiguous()
     if x.shape[0] == 0:
         raise ValueError("%s: no points" % what)
@@ -270,14 +249,13 @@ class NNIndex:
     def __init__(self, points, min_cell=0.0):
         self.points = _points(points, "NNIndex")
         n = self.points.shape[0]
-        lib = _lib.load()
         with torch.cuda.device(self.points.device):
-            nbytes = lib.goslam_nn_index_workspace_bytes(n)
-            if nbytes == 0:
-                raise RuntimeError("NNIndex: cannot index %d points" % n)
-            self.buf = torch.empty(nbytes, dtype=torch.uint8, device=self.points.device)
-            _lib.check(lib.goslam_nn_index_build(_lib.ptr(self.points), n, float(min_cell), _lib.ptr(self.buf), nbytes,
-                                                 _lib.stream_ptr()), "nn_index_build")
+            # CUB sizes its scratch for the current device
+            nbytes = _lib.load().goslam_nn_index_workspace_bytes(n)
+        if nbytes == 0:
+            raise RuntimeError("NNIndex: cannot index %d points" % n)
+        self.buf = torch.empty(nbytes, dtype=torch.uint8, device=self.points.device)
+        _lib.call("nn_index_build", self.points, n, float(min_cell), self.buf, nbytes)
 
     def __len__(self):
         return self.points.shape[0]
@@ -289,10 +267,7 @@ class NNIndex:
             torch.empty((0, 3), dtype=torch.float64, device=self.points.device)
         dist = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
         idx = torch.empty(q.shape[0], dtype=torch.int64, device=q.device)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib.load().goslam_nn_query(_lib.ptr(self.buf), self.buf.numel(), len(self), _lib.ptr(q),
-                                                   q.shape[0], float(max_dist), _lib.ptr(dist), _lib.ptr(idx),
-                                                   _lib.stream_ptr()), "nn_query")
+        _lib.call("nn_query", self.buf, self.buf.numel(), len(self), q, q.shape[0], float(max_dist), dist, idx)
         return dist, idx
 
 
@@ -315,23 +290,20 @@ def sample_surface_from(verts, faces, uniforms):
         raise ValueError("sample_surface: the mesh has no faces")
     u = torch.as_tensor(uniforms).to(verts.device, torch.float64).reshape(-1, 3).contiguous()
     out = torch.empty((u.shape[0], 3), dtype=torch.float64, device=verts.device)
-    lib = _lib.load()
     with torch.cuda.device(verts.device):
-        nbytes = lib.goslam_mesh_sample_workspace_bytes(faces.shape[0])
-        if nbytes == 0:
-            raise RuntimeError("sample_surface: cannot size the workspace for %d faces" % faces.shape[0])
-        ws = _workspace(nbytes, verts.device)
-        _lib.check(lib.goslam_mesh_sample_surface(_lib.ptr(verts), verts.shape[0], _lib.ptr(faces), faces.shape[0],
-                                                  _lib.ptr(u), u.shape[0], _lib.ptr(out), None, _lib.ptr(ws), nbytes,
-                                                  _lib.stream_ptr()), "mesh_sample_surface")
+        # CUB sizes its scratch for the current device
+        nbytes = _lib.load().goslam_mesh_sample_workspace_bytes(faces.shape[0])
+    if nbytes == 0:
+        raise RuntimeError("sample_surface: cannot size the workspace for %d faces" % faces.shape[0])
+    ws = _lib.workspace(nbytes, verts.device)
+    _lib.call("mesh_sample_surface", verts, verts.shape[0], faces, faces.shape[0], u, u.shape[0], out, None, ws, nbytes)
     return out
 
 
 def sample_surface(verts, faces, count, generator=None):
     """[count, 3] f64 area-weighted samples of the mesh's surface, uniforms from torch.rand on the mesh's device"""
     verts = torch.as_tensor(verts)
-    if not verts.is_cuda:
-        raise RuntimeError("sample_surface: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("sample_surface", verts)
     return sample_surface_from(verts, faces, _uniforms(int(count), generator, verts.device))
 
 
@@ -347,17 +319,13 @@ def icp_point_to_point(src, dst, threshold, init=None, max_iteration=30, relativ
     T0 = torch.eye(4, dtype=torch.float64) if init is None else torch.as_tensor(np.asarray(init, np.float64))
     T0 = T0.to(dev, torch.float64).reshape(4, 4).contiguous()
     out = torch.empty(19, dtype=torch.float64, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        nbytes = lib.goslam_icp_workspace_bytes(src.shape[0])
-        if nbytes == 0:
-            raise RuntimeError("icp_point_to_point: cannot size the workspace for %d points" % src.shape[0])
-        ws = _workspace(nbytes, dev)
-        _lib.check(lib.goslam_icp_point_to_point(_lib.ptr(src), src.shape[0], _lib.ptr(index.buf), index.buf.numel(),
-                                                 len(index), float(threshold), _lib.ptr(T0), int(max_iteration),
-                                                 float(relative_fitness), float(relative_rmse), _lib.ptr(out),
-                                                 _lib.ptr(ws), nbytes, _lib.stream_ptr()), "icp_point_to_point")
-        host = out.cpu()
+    nbytes = _lib.load().goslam_icp_workspace_bytes(src.shape[0])
+    if nbytes == 0:
+        raise RuntimeError("icp_point_to_point: cannot size the workspace for %d points" % src.shape[0])
+    ws = _lib.workspace(nbytes, dev)
+    _lib.call("icp_point_to_point", src, src.shape[0], index.buf, index.buf.numel(), len(index), float(threshold), T0,
+              int(max_iteration), float(relative_fitness), float(relative_rmse), out, ws, nbytes)
+    host = out.cpu()
     return host[:16].reshape(4, 4).clone(), float(host[16]), float(host[17]), int(host[18])
 
 
@@ -371,15 +339,11 @@ def mesh_metrics(est_pts, gt_pts, dist_th):
     under dist_th (%) and the F-score, with the reference's dtypes (float64 means, float32 ratios).  One host read."""
     est, gt = _points(est_pts, "mesh_metrics"), _points(gt_pts, "mesh_metrics")
     stats = torch.empty(4, dtype=torch.float64, device=est.device)
-    lib = _lib.load()
-    with torch.cuda.device(est.device):
-        comp, _ = NNIndex(est).query(gt)
-        _lib.check(lib.goslam_nn_distance_stats(_lib.ptr(comp), comp.numel(), float(dist_th), _lib.ptr(stats[0:2]),
-                                                _lib.stream_ptr()), "nn_distance_stats")
-        acc, _ = NNIndex(gt).query(est)
-        _lib.check(lib.goslam_nn_distance_stats(_lib.ptr(acc), acc.numel(), float(dist_th), _lib.ptr(stats[2:4]),
-                                                _lib.stream_ptr()), "nn_distance_stats")
-        s = stats.tolist()
+    comp, _ = NNIndex(est).query(gt)
+    _lib.call("nn_distance_stats", comp, comp.numel(), float(dist_th), stats[0:2])
+    acc, _ = NNIndex(gt).query(est)
+    _lib.call("nn_distance_stats", acc, acc.numel(), float(dist_th), stats[2:4])
+    s = stats.tolist()
     completion = np.float64(s[0]) / gt.shape[0] * 100
     accuracy = np.float64(s[2]) / est.shape[0] * 100
     completion_ratio, accuracy_ratio = _ratio(int(s[1]), gt.shape[0]), _ratio(int(s[3]), est.shape[0])
@@ -453,14 +417,14 @@ def _hull_run(points, what):
     """goslam_hull_vertices on points (CUDA, any float dtype, [n,3]): (points f64, workspace, info [4] on the device)"""
     pts = _points(points, what)
     n = pts.shape[0]
-    lib = _lib.load()
-    nbytes = lib.goslam_hull_workspace_bytes(n)
+    with torch.cuda.device(pts.device):
+        # CUB sizes its scratch for the current device
+        nbytes = _lib.load().goslam_hull_workspace_bytes(n)
     if nbytes == 0:
         raise ValueError("%s: %d points (at most 2^28)" % (what, n))
-    ws = _workspace(nbytes, pts.device)
+    ws = _lib.workspace(nbytes, pts.device)
     info = torch.empty(4, dtype=torch.int64, device=pts.device)
-    _lib.check(lib.goslam_hull_vertices(_lib.ptr(pts), n, _lib.ptr(ws), nbytes, _lib.ptr(info), _lib.stream_ptr()),
-               "hull_vertices")
+    _lib.call("hull_vertices", pts, n, ws, nbytes, info)
     return pts, ws, nbytes, info
 
 
@@ -476,23 +440,19 @@ def hull_vertices(points):
     """sorted int64 ids of the convex-hull vertices of points [n,3] (CUDA): the exact extreme points, so a point on a
     hull face or edge is not one and of equal points only the lowest index can be.  ValueError when the points span
     less than three dimensions.  One host read."""
-    with torch.cuda.device(torch.as_tensor(points).device):
-        pts, ws, nbytes, info = _hull_run(points, "hull_vertices")
-        count = _hull_info(info, "hull_vertices")
-        out = torch.empty(count, dtype=torch.int64, device=pts.device)
-        _lib.check(_lib.load().goslam_hull_vertices_emit(_lib.ptr(ws), nbytes, pts.shape[0], _lib.ptr(out), count,
-                                                         _lib.stream_ptr()), "hull_vertices_emit")
+    pts, ws, nbytes, info = _hull_run(points, "hull_vertices")
+    count = _hull_info(info, "hull_vertices")
+    out = torch.empty(count, dtype=torch.int64, device=pts.device)
+    _lib.call("hull_vertices_emit", ws, nbytes, pts.shape[0], out, count)
     return out
 
 
 def _oriented_box(points, extend):
     """box [15] f64 on the device (center, R row-major, extent + extend).  One host read (the hull's status)."""
-    with torch.cuda.device(torch.as_tensor(points).device):
-        pts, ws, nbytes, info = _hull_run(points, "oriented_box")
-        box = torch.empty(15, dtype=torch.float64, device=pts.device)
-        _lib.check(_lib.load().goslam_obb_from_hull(_lib.ptr(pts), pts.shape[0], _lib.ptr(ws), nbytes, float(extend),
-                                                    _lib.ptr(box), _lib.stream_ptr()), "obb_from_hull")
-        _hull_info(info, "oriented_box")
+    pts, ws, nbytes, info = _hull_run(points, "oriented_box")
+    box = torch.empty(15, dtype=torch.float64, device=pts.device)
+    _lib.call("obb_from_hull", pts, pts.shape[0], ws, nbytes, float(extend), box)
+    _hull_info(info, "oriented_box")
     return box
 
 
@@ -508,17 +468,14 @@ def in_oriented_box(points, center, R, extent):
     """bool [n]: Open3D's get_point_indices_within_bounding_box rule (six plane tests on the box corners) for points
     [n,3] (CUDA).  The box is read on the device."""
     pts = torch.as_tensor(points)
-    if not pts.is_cuda:
-        raise RuntimeError("in_oriented_box: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("in_oriented_box", pts)
     pts = pts.detach().to(torch.float64).reshape(-1, 3).contiguous()
     dev = pts.device
     box = torch.cat([torch.as_tensor(t).to(dev, torch.float64).reshape(-1) for t in (center, R, extent)])
     if box.numel() != 15:
         raise ValueError("in_oriented_box: center [3], R [3,3] and extent [3] expected")
     mask = torch.empty(pts.shape[0], dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().goslam_obb_in_bound(_lib.ptr(box), _lib.ptr(pts), pts.shape[0], _lib.ptr(mask),
-                                                   _lib.stream_ptr()), "obb_in_bound")
+    _lib.call("obb_in_bound", box, pts, pts.shape[0], mask)
     return mask.bool()
 
 
@@ -596,26 +553,22 @@ def mapping_points(video, cur_idx):
     if dev.type != "cuda":
         raise RuntimeError("mapping_points: a CUDA video is required (no CPU fallback)")
     _, ht, wd = video.disps_up.shape
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        nbytes = lib.goslam_mapping_points_workspace_bytes(T, ht, wd)
-        if nbytes == 0:
-            raise ValueError("mapping_points: invalid shape (%d, %d, %d)" % (T, ht, wd))
-        poses = video.poses.detach()[:T].float().contiguous()
-        disps = video.disps_up.detach()[:T].float().contiguous()
-        intr = (video.intrinsics[0].detach() * video.scale_factor).float().contiguous()
-        w2w = lietorch.SE3(video.pose_compensate[0].clone().unsqueeze(dim=0)).to(dev)
-        poses_world = (w2w * lietorch.SE3(poses).inv()).data.float().contiguous()
-        ws = _workspace(nbytes, dev)
-        count = torch.empty(1, dtype=torch.int64, device=dev)
-        st = _lib.stream_ptr()
-        _lib.check(lib.goslam_mapping_points_count(_lib.ptr(poses), _lib.ptr(poses_world), _lib.ptr(disps),
-                                                   _lib.ptr(intr), T, ht, wd, _lib.ptr(ws), nbytes, _lib.ptr(count),
-                                                   st), "mapping_points_count")
-        n = int(count.item())
-        out = torch.empty((n, 3), dtype=torch.float64, device=dev)
-        _lib.check(lib.goslam_mapping_points_emit(_lib.ptr(poses_world), _lib.ptr(disps), _lib.ptr(intr), T, ht, wd,
-                                                  _lib.ptr(ws), nbytes, _lib.ptr(out), n, st), "mapping_points_emit")
+        # CUB sizes its scratch for the current device
+        nbytes = _lib.load().goslam_mapping_points_workspace_bytes(T, ht, wd)
+    if nbytes == 0:
+        raise ValueError("mapping_points: invalid shape (%d, %d, %d)" % (T, ht, wd))
+    poses = video.poses.detach()[:T].float().contiguous()
+    disps = video.disps_up.detach()[:T].float().contiguous()
+    intr = (video.intrinsics[0].detach() * video.scale_factor).float().contiguous()
+    w2w = lietorch.SE3(video.pose_compensate[0].clone().unsqueeze(dim=0)).to(dev)
+    poses_world = (w2w * lietorch.SE3(poses).inv()).data.float().contiguous()
+    ws = _lib.workspace(nbytes, dev)
+    count = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.call("mapping_points_count", poses, poses_world, disps, intr, T, ht, wd, ws, nbytes, count)
+    n = int(count.item())
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    _lib.call("mapping_points_emit", poses_world, disps, intr, T, ht, wd, ws, nbytes, out, n)
     return out
 
 

@@ -12,19 +12,11 @@ AltCorrBlock(fmaps)(coords, ii, jj) -> windowed correlation, all levels in one l
 A pooled pyramid is in the tiled layout, private to the build and lookup kernels; `corr_pyramid` /
 `gather_pyramid()` give the reference's [N, h, w, h>>i, w>>i] levels as a de-tiled copy.
 """
-import ctypes
-
 import torch
 import torch.nn.functional as F
 
 from .. import _lib
-
-
-def _ptr_array(tensors):
-    arr = (ctypes.c_void_p * len(tensors))()
-    for i, t in enumerate(tensors):
-        arr[i] = t.data_ptr()
-    return arr
+from .._lib import ptr_array as _ptr_array
 
 
 class CorrPool:
@@ -139,14 +131,11 @@ class CorrBlock:
             return
         dtype = torch.float16 if fmap1.dtype == torch.float16 else torch.float32
         f1 = fmap1.reshape(N, dim, ht, wd).to(dtype).contiguous()
-        f2 = fmap2.reshape(N, dim, ht, wd).to(dtype).contiguous()   # named: a converted copy must outlive the launch
+        f2 = fmap2.reshape(N, dim, ht, wd).to(dtype).contiguous()
         self._levels = [torch.empty((N, ht, wd, ht >> i, wd >> i), dtype=dtype, device=dev)
                         for i in range(num_levels)]
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_corr_build(
-                _lib.ptr(f1), _lib.ptr(f2), 1 if dtype == torch.float16 else 0, _ptr_array(self._levels),
-                num_levels, N, dim, ht, wd, _lib.stream_ptr())
-        _lib.check(rc, "corr_build")
+        _lib.call("corr_build", f1, f2, 1 if dtype == torch.float16 else 0, _ptr_array(self._levels), num_levels,
+                  N, dim, ht, wd)
 
     @classmethod
     def from_video(cls, fmaps_kmajor, ii, jj, ht, wd, rig=1, num_levels=4, radius=3, pool=None):
@@ -168,12 +157,8 @@ class CorrBlock:
         self.pool = pool
         self._slots_host = pool.alloc(N)
         self.slots = pool.slot_table(self._slots_host)
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_corr_pool_build(
-                _lib.ptr(fmaps_kmajor), int(fmaps_kmajor.shape[0]), int(rig), _lib.ptr(ii), _lib.ptr(jj),
-                _lib.ptr(self.slots), _ptr_array(pool.levels), self.num_levels, N, 128, self.ht, self.wd,
-                _lib.stream_ptr())
-        _lib.check(rc, "corr_pool_build")
+        _lib.call("corr_pool_build", fmaps_kmajor, int(fmaps_kmajor.shape[0]), int(rig), ii, jj, self.slots,
+                  _ptr_array(pool.levels), self.num_levels, N, 128, self.ht, self.wd)
 
     def __call__(self, coords):
         batch, num, ht, wd, _ = coords.shape
@@ -186,12 +171,8 @@ class CorrBlock:
         out = torch.empty((batch, num, self.num_levels * rd * rd, ht, wd), dtype=vol0.dtype,
                           device=vol0.device)
         pyr = [p.contiguous() for p in self._levels]
-        with torch.cuda.device(vol0.device):
-            rc = _lib.load().goslam_corr_pyramid_lookup(
-                _ptr_array(pyr), 1 if vol0.dtype == torch.float16 else 0, self.num_levels,
-                _lib.ptr(coords), _lib.ptr(out), N, ht, wd, vol0.shape[3], vol0.shape[4],
-                int(self.radius), _lib.stream_ptr())
-        _lib.check(rc, "corr_pyramid_lookup")
+        _lib.call("corr_pyramid_lookup", _ptr_array(pyr), 1 if vol0.dtype == torch.float16 else 0, self.num_levels,
+                  coords, out, N, ht, wd, vol0.shape[3], vol0.shape[4], int(self.radius))
         return out
 
     def _call_pooled(self, coords, batch, num, ht, wd):
@@ -200,15 +181,11 @@ class CorrBlock:
             raise RuntimeError("CorrBlock: %d coordinate maps for %d edges" % (N, len(self._slots_host)))
         pool = self.pool
         rd = 2 * self.radius + 1
-        dev = pool.levels[0].device
         coords = coords.reshape(N, ht, wd, 2).contiguous().float()
-        out = torch.empty((batch, num, self.num_levels * rd * rd, ht, wd), dtype=torch.float16, device=dev)
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_corr_pool_lookup(
-                _ptr_array(pool.levels), 1, self.num_levels, _lib.ptr(self.slots), pool.capacity,
-                pool.TILED, _lib.ptr(coords), _lib.ptr(out), N, ht, wd, pool.ht, pool.wd, int(self.radius),
-                _lib.stream_ptr())
-        _lib.check(rc, "corr_pool_lookup")
+        out = torch.empty((batch, num, self.num_levels * rd * rd, ht, wd), dtype=torch.float16,
+                          device=pool.levels[0].device)
+        _lib.call("corr_pool_lookup", _ptr_array(pool.levels), 1, self.num_levels, self.slots, pool.capacity,
+                  pool.TILED, coords, out, N, ht, wd, pool.ht, pool.wd, int(self.radius))
         return out
 
     def cat(self, other):
@@ -292,9 +269,7 @@ def fmaps_to_kmajor(fmaps, out=None):
     F = f.numel() // (128 * h * w)
     if out is None:
         out = torch.empty((F, h * w, 128), dtype=torch.float16, device=f.device)
-    with torch.cuda.device(f.device):
-        rc = _lib.load().goslam_fmaps_to_kmajor(_lib.ptr(f), _lib.ptr(out), F, 128, h, w, _lib.stream_ptr())
-    _lib.check(rc, "fmaps_to_kmajor")
+    _lib.call("fmaps_to_kmajor", f, out, F, 128, h, w)
     return out
 
 
@@ -336,9 +311,5 @@ class AltCorrBlock:
         ii = torch.as_tensor(ii, device=dev).long().contiguous()
         jj = torch.as_tensor(jj, device=dev).long().contiguous()
         c = coords.reshape(N, H, W, 2).float().contiguous()
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_altcorr_pyramid(_ptr_array(pyr), self.num_levels, _lib.ptr(c), _lib.ptr(ii),
-                                                    _lib.ptr(jj), _lib.ptr(out), N, H, W, C, int(self.radius),
-                                                    _lib.stream_ptr())
-        _lib.check(rc, "altcorr_pyramid")
+        _lib.call("altcorr_pyramid", _ptr_array(pyr), self.num_levels, c, ii, jj, out, N, H, W, C, int(self.radius))
         return out

@@ -70,8 +70,7 @@ class EncoderPack:
 def encode(weights, norm_fn, out_dim, image, mean=None, std=None, split=False):
     """image [B, 3, H, W] (CUDA, f32 or f16) -> f16 [B, out_dim, H/8, W/8], or with split (out_dim 256) the pair
     (tanh of channels 0-127, relu of channels 128-255).  mean / std [3] apply (x - mean) / std before the stem."""
-    if not image.is_cuda:
-        raise RuntimeError("BasicEncoder: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("BasicEncoder", image)
     B, C, H, W = image.shape
     if C != 3 or H % 8 or W % 8:
         raise ValueError("BasicEncoder: image must be [B, 3, H, W] with H and W multiples of 8, got %s"
@@ -89,15 +88,9 @@ def encode(weights, norm_fn, out_dim, image, mean=None, std=None, split=False):
     if mean is not None:
         mean = mean.reshape(3).to(dev, torch.float32).contiguous()
         std = std.reshape(3).to(dev, torch.float32).contiguous()
-    from ..droid_backends import _workspace
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        ws = _workspace(lib.goslam_encoder_workspace_bytes(B, H, W, norm), dev)
-        rc = lib.goslam_basic_encoder(ctypes.byref(weights), norm, out_dim, _lib.ptr(image),
-                                      1 if image.dtype == torch.float16 else 0, _lib.ptr(mean), _lib.ptr(std), B, H, W,
-                                      _lib.ptr(out), _lib.ptr(out2), 1 if split else 0, _lib.ptr(ws),
-                                      ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-    _lib.check(rc, "basic_encoder")
+    ws = _lib.workspace(_lib.load().goslam_encoder_workspace_bytes(B, H, W, norm), dev)
+    _lib.call("basic_encoder", ctypes.byref(weights), norm, out_dim, image, 1 if image.dtype == torch.float16 else 0,
+              mean, std, B, H, W, out, out2, 1 if split else 0, ws, ws.numel())
     return (out, out2) if split else out
 
 

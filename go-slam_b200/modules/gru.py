@@ -14,7 +14,6 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..droid_backends import _workspace
 
 
 def to_nhwc(x):
@@ -22,9 +21,7 @@ def to_nhwc(x):
     b, c, h, w = x.shape
     src = x.contiguous() if x.dtype == torch.float16 else x.half().contiguous()
     dst = torch.empty((b, h, w, c), dtype=torch.float16, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = _lib.load().goslam_nchw_to_nhwc_f16(_lib.ptr(src), _lib.ptr(dst), b, c, h * w, _lib.stream_ptr())
-    _lib.check(rc, "nchw_to_nhwc")
+    _lib.call("nchw_to_nhwc_f16", src, dst, b, c, h * w)
     return dst
 
 
@@ -32,9 +29,7 @@ def to_nchw(x):
     """[B, h, w, C] float16 -> [B, C, h, w] float16"""
     b, h, w, c = x.shape
     dst = torch.empty((b, c, h, w), dtype=torch.float16, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = _lib.load().goslam_nhwc_to_nchw_f16(_lib.ptr(x), _lib.ptr(dst), b, c, h * w, _lib.stream_ptr())
-    _lib.check(rc, "nhwc_to_nchw")
+    _lib.call("nhwc_to_nchw_f16", x, dst, b, c, h * w)
     return dst
 
 
@@ -85,12 +80,8 @@ class ConvGRU(nn.Module):
         b, h, w, _ = net.shape
         out = torch.empty_like(net)
         st = self._pack()
-        lib = _lib.load()
-        with torch.cuda.device(net.device):
-            ws = _workspace(lib.goslam_conv_gru_workspace_bytes(b, h, w), net.device)
-            rc = lib.goslam_conv_gru(ctypes.byref(st), _lib.ptr(net), _lib.ptr(inp), _lib.ptr(corr), _lib.ptr(flow),
-                                     _lib.ptr(out), b, h, w, _lib.ptr(ws), ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-        _lib.check(rc, "conv_gru")
+        ws = _lib.workspace(_lib.load().goslam_conv_gru_workspace_bytes(b, h, w), net.device)
+        _lib.call("conv_gru", ctypes.byref(st), net, inp, corr, flow, out, b, h, w, ws, ws.numel())
         return out
 
     @torch.no_grad()
@@ -143,9 +134,7 @@ def conv2d_nhwc(inputs, weight, bias, cout, act=None, out=None, out_f32=False, o
     d.taps, d.cout, d.cout_pad, d.act = taps, cout, cout_pad, ACT[act]
     d.out_scale = float(out_scale)
     d.out, d.out_f32, d.out_stride, d.out_offset = out.data_ptr(), int(out.dtype == torch.float32), out.shape[-1], out_offset
-    with torch.cuda.device(x0.device):
-        rc = _lib.load().goslam_conv2d_nhwc(ctypes.byref(d), B, h, w, _lib.stream_ptr())
-    _lib.check(rc, "conv2d_nhwc")
+    _lib.call("conv2d_nhwc", ctypes.byref(d), B, h, w, device=x0.device)
     return out
 
 
@@ -154,7 +143,5 @@ def to_nhwc_padded(x, cpad):
     b, c, h, w = x.shape
     src = x.contiguous() if x.dtype == torch.float16 else x.half().contiguous()
     dst = torch.empty((b, h, w, cpad), dtype=torch.float16, device=x.device)
-    with torch.cuda.device(x.device):
-        rc = _lib.load().goslam_nchw_to_nhwc_f16_pad(_lib.ptr(src), _lib.ptr(dst), b, c, cpad, h * w, _lib.stream_ptr())
-    _lib.check(rc, "nchw_to_nhwc_pad")
+    _lib.call("nchw_to_nhwc_f16_pad", src, dst, b, c, cpad, h * w)
     return dst

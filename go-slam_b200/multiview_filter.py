@@ -80,10 +80,8 @@ class MultiviewFilter(torch.nn.Module):
         n, ht, wd = v.disps_up.shape
         if T > n:
             raise RuntimeError("MultiviewFilter: counter %d exceeds the video buffer %d" % (T, n))
-        lib = _lib.load()
         dev = b["poses"].device
         with torch.cuda.device(dev):
-            stream = _lib.stream_ptr()
             with v.get_lock():
                 b["poses"][:T].copy_(v.poses[:T])
                 b["disps"][:T].copy_(v.disps_up[:T])
@@ -92,22 +90,15 @@ class MultiviewFilter(torch.nn.Module):
             poses, disps = b["poses"][:T], b["disps"][:T]
             # the reference's iproj argument, with the same SE3 algebra
             poses_world = (lietorch.SE3(b["w2w"]) * lietorch.SE3(poses).inv()).data.contiguous()
-            rc = lib.goslam_mvfilter_compute(
-                _lib.ptr(poses), _lib.ptr(poses_world), _lib.ptr(disps), _lib.ptr(b["intrinsic"]),
-                float(self.filter_thresh), int(self.filter_visible_num), self._kernel_code(), T, ht, wd,
-                _lib.ptr(self._ws), self._ws.numel(), stream)
-            _lib.check(rc, "mvfilter_compute")
-            with v.mapping.get_lock():
-                rc = lib.goslam_mvfilter_commit(
-                    _lib.ptr(poses), _lib.ptr(disps), _lib.ptr(self._ws), self._ws.numel(), T, ht, wd,
-                    _lib.ptr(v.poses_filtered), _lib.ptr(v.disps_filtered), _lib.ptr(v.mask_filtered),
-                    _lib.ptr(v.update_priority), _lib.ptr(v.filtered_id), _lib.ptr(v.bound),
-                    _lib.ptr(b["status"]), stream)
-                _lib.check(rc, "mvfilter_commit")
-                # mapping reads these buffers from another process as soon as the lock is released
-                torch.cuda.current_stream(dev).synchronize()
-                n_mask, _, n_final, committed = b["status"].tolist()
-                bd = v.bound[0].tolist()
+        _lib.call("mvfilter_compute", poses, poses_world, disps, b["intrinsic"], float(self.filter_thresh),
+                  int(self.filter_visible_num), self._kernel_code(), T, ht, wd, self._ws, self._ws.numel())
+        with v.mapping.get_lock():
+            _lib.call("mvfilter_commit", poses, disps, self._ws, self._ws.numel(), T, ht, wd, v.poses_filtered,
+                      v.disps_filtered, v.mask_filtered, v.update_priority, v.filtered_id, v.bound, b["status"])
+            # mapping reads these buffers from another process as soon as the lock is released
+            torch.cuda.current_stream(dev).synchronize()
+            n_mask, _, n_final, committed = b["status"].tolist()
+            bd = v.bound[0].tolist()
         if n_mask < 100:
             return
         if not committed:

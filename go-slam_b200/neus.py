@@ -27,7 +27,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .droid_backends import _workspace
+from .mesher import keep_box
 
 N_LEVELS, N_FEAT = 16, 2
 MLP_IN, MLP_IN_PAD, MLP_HID, MLP_OUT_PAD = 67, 80, 64, 16
@@ -235,8 +235,7 @@ class InstantNeuS(nn.Module):
     @torch.no_grad()
     def _forward_impl(self, rays_o, rays_d, z_vals, dists, debug=False, train=False):
         """the fused marcher; train=True keeps what the backward needs in `self.last_debug`"""
-        if not z_vals.is_cuda:
-            raise RuntimeError("InstantNeuS.forward: CUDA tensors required (no CPU fallback)")
+        _lib.need_cuda("InstantNeuS.forward", z_vals)
         dev = z_vals.device
         R, S = z_vals.shape
         rays_o = rays_o.detach().float().contiguous()
@@ -272,13 +271,8 @@ class InstantNeuS(nn.Module):
             o.mlp_in = self.last_debug['mlp_in'].data_ptr()
             o.enc = self.last_debug['enc'].data_ptr()
             o.fallback = self.last_debug['fallback'].data_ptr()
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            ws = _workspace(lib.goslam_neus_workspace_bytes(R, S), dev)
-            rc = lib.goslam_neus_forward(ctypes.byref(p), _lib.ptr(rays_o), _lib.ptr(rays_d),
-                                         _lib.ptr(z_vals), _lib.ptr(dists), R, S, ctypes.byref(o),
-                                         _lib.ptr(ws), ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-        _lib.check(rc, "neus_forward")
+        ws = _lib.workspace(_lib.load().goslam_neus_workspace_bytes(R, S), dev)
+        _lib.call("neus_forward", ctypes.byref(p), rays_o, rays_d, z_vals, dists, R, S, ctypes.byref(o), ws, ws.numel())
         out['sdf_variance'] = torch.full((R, 1), 1.0 / inv_s, **f32)
         return out
 
@@ -311,10 +305,7 @@ class InstantNeuS(nn.Module):
         for a in range(3):
             p.bound[2 * a], p.bound[2 * a + 1] = float(bound_min[a]), float(bound_max[a])
         u = torch.empty((res, res, res), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_neus_sdf_grid(ctypes.byref(p), _lib.ptr(tabs[:res]), _lib.ptr(tabs[res:2 * res]),
-                                                  _lib.ptr(tabs[2 * res:]), res, res, res, _lib.ptr(u), _lib.stream_ptr())
-        _lib.check(rc, "neus_sdf_grid")
+        _lib.call("neus_sdf_grid", ctypes.byref(p), tabs[:res], tabs[res:2 * res], tabs[2 * res:], res, res, res, u)
         return u
 
     @torch.no_grad()
@@ -332,10 +323,7 @@ class InstantNeuS(nn.Module):
         for i in range(6):
             p.bound[i] = bound[i]
         rgb = torch.empty((verts.shape[0], 3), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = _lib.load().goslam_neus_vertex_color(ctypes.byref(p), _lib.ptr(verts), verts.shape[0], _lib.ptr(rgb),
-                                                      _lib.stream_ptr())
-        _lib.check(rc, "neus_vertex_color")
+        _lib.call("neus_vertex_color", ctypes.byref(p), verts, verts.shape[0], rgb)
         return rgb
 
     @torch.no_grad()
@@ -393,24 +381,19 @@ def marching_cubes(u, iso, bound_min, bound_max):
     """marching cubes of the f32 CUDA field u [nx,ny,nz] at level iso (inside iff u > iso), on the generated tables of
     csrc/mc_tables.cuh: (vertices [V,3] f64 in world coordinates v / (n - 1.0) * (float32)(bound_max - bound_min) +
     bound_min, faces [F,3] i64), CUDA tensors.  Reads the two counts back (one host synchronisation)."""
-    lib = _lib.load()
     u = u.detach().float().contiguous()
     nx, ny, nz = u.shape
     dev = u.device
     i64 = dict(dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.stream_ptr()
-        ws = torch.empty(lib.goslam_mc_workspace_bytes(nx, ny, nz), dtype=torch.uint8, device=dev)
-        counts = torch.empty(2, **i64)
-        _lib.check(lib.goslam_mc_count(_lib.ptr(u), nx, ny, nz, float(iso), _lib.ptr(ws), ws.numel(), _lib.ptr(counts), st),
-                   "mc_count")
-        nv, nf = counts.tolist()
-        verts = torch.empty((nv, 3), dtype=torch.float64, device=dev)
-        faces = torch.empty((nf, 3), **i64)
-        lo = (ctypes.c_float * 3)(*[float(v) for v in bound_min])
-        hi = (ctypes.c_float * 3)(*[float(v) for v in bound_max])
-        _lib.check(lib.goslam_mc_emit(_lib.ptr(u), nx, ny, nz, float(iso), lo, hi, _lib.ptr(ws), ws.numel(),
-                                      _lib.ptr(verts), nv, _lib.ptr(faces), nf, st), "mc_emit")
+    ws = torch.empty(_lib.load().goslam_mc_workspace_bytes(nx, ny, nz), dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, **i64)
+    _lib.call("mc_count", u, nx, ny, nz, float(iso), ws, ws.numel(), counts)
+    nv, nf = counts.tolist()
+    verts = torch.empty((nv, 3), dtype=torch.float64, device=dev)
+    faces = torch.empty((nf, 3), **i64)
+    lo = (ctypes.c_float * 3)(*[float(v) for v in bound_min])
+    hi = (ctypes.c_float * 3)(*[float(v) for v in bound_max])
+    _lib.call("mc_emit", u, nx, ny, nz, float(iso), lo, hi, ws, ws.numel(), verts, nv, faces, nf)
     return verts, faces
 
 
@@ -418,24 +401,7 @@ def cull_mesh(verts, faces, lo, hi):
     """keep the vertices with lo <= v <= hi (lo, hi: 3 float32 values each), the faces whose three vertices are kept,
     then drop unreferenced vertices; stable orders, faces re-indexed (update_faces + remove_unreferenced_vertices).
     CUDA tensors in and out; reads the two counts back (one host synchronisation)."""
-    lib = _lib.load()
-    verts = verts.detach().to(torch.float64).contiguous()
-    faces = faces.detach().to(torch.int64).contiguous()
-    nv, nf = verts.shape[0], faces.shape[0]
-    dev = verts.device
-    with torch.cuda.device(dev):
-        st = _lib.stream_ptr()
-        ws = torch.empty(lib.goslam_mesh_cull_workspace_bytes(nv, nf), dtype=torch.uint8, device=dev)
-        counts = torch.empty(2, dtype=torch.int64, device=dev)
-        lo = (ctypes.c_float * 3)(*[float(v) for v in lo])
-        hi = (ctypes.c_float * 3)(*[float(v) for v in hi])
-        _lib.check(lib.goslam_mesh_cull_count(_lib.ptr(verts), nv, _lib.ptr(faces), nf, lo, hi, _lib.ptr(ws), ws.numel(),
-                                              _lib.ptr(counts), st), "mesh_cull_count")
-        kv, kf = counts.tolist()
-        out_v = torch.empty((kv, 3), dtype=torch.float64, device=dev)
-        out_f = torch.empty((kf, 3), dtype=torch.int64, device=dev)
-        _lib.check(lib.goslam_mesh_cull_emit(_lib.ptr(verts), nv, _lib.ptr(faces), nf, _lib.ptr(ws), ws.numel(),
-                                             _lib.ptr(out_v), kv, _lib.ptr(out_f), kf, st), "mesh_cull_emit")
+    out_v, out_f, _ = keep_box(verts, faces, lo, hi)
     return out_v, out_f
 
 
@@ -480,7 +446,6 @@ class _NeusFunction(torch.autograd.Function):
         p, keep, inv_s = ctx.pstruct
         dev = z_vals.device
         R, S = z_vals.shape
-        lib = _lib.load()
         f32 = dict(dtype=torch.float32, device=dev)
         c = lambda t: None if t is None else t.detach().float().contiguous()
         d_color, d_depth, d_sdf = c(d_color), c(d_depth), c(d_sdf)
@@ -499,55 +464,44 @@ class _NeusFunction(torch.autograd.Function):
         g_B = torch.zeros(3, 33, **f32)
         g_w0 = torch.zeros(35, **f32)
         g_inv_s = torch.zeros(1, **f32)
-        with torch.cuda.device(dev):
-            for r0 in range(0, R, _NeusFunction.CHUNK_RAYS):
-                r1 = min(R, r0 + _NeusFunction.CHUNK_RAYS)
-                n = (r1 - r0) * S
-                sl = slice(r0, r1)
-                ro, rd, zv, ds = rays_o[sl], rays_d[sl], z_vals[sl], dists[sl]
-                d_y = torch.empty(n, 3, **f32); d_s = torch.empty(n, **f32); d_g = torch.empty(n, 3, **f32)
-                dc = None if d_color is None else d_color[sl].contiguous()
-                dd = None if d_depth is None else d_depth[sl].contiguous()
-                dsu = None if d_sdf is None else d_sdf[sl].contiguous()
-                rc = lib.goslam_neus_composite_backward(
-                    ctypes.byref(p), _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(ds), _lib.ptr(alpha[sl]), _lib.ptr(rgb[sl]),
-                    _lib.ptr(sdf[sl]), _lib.ptr(grad[sl]), _lib.ptr(z_mid[sl]),
-                    None if dc is None else _lib.ptr(dc), None if dd is None else _lib.ptr(dd),
-                    None if dsu is None else _lib.ptr(dsu), None if d_gerr is None else _lib.ptr(d_gerr),
-                    _lib.ptr(fallback), ctypes.c_int64(R * S), ctypes.c_int64(r0 * S), r1 - r0, S,
-                    _lib.ptr(d_y), _lib.ptr(d_s), _lib.ptr(d_g), _lib.ptr(g_inv_s), _lib.stream_ptr())
-                _lib.check(rc, "neus_composite_backward")
-                amax = torch.maximum(d_y.abs().max(), d_s.abs().max()).clamp_min(1e-30)
-                sc = torch.exp2(torch.floor(torch.log2(1024.0 / amax))).clamp(max=2.0 ** 40).reshape(1).contiguous()   # device scalar
-                # ---- colour network, row-wise half (one kernel): H1, H2, dH2, dH1, dX and what hangs off dX per sample ----
-                X = mlp_in[sl].reshape(n, MLP_IN_PAD)                                 # half, as the forward built it
-                H1, H2, dH1, dH2 = (torch.empty(n, MLP_HID, **f16) for _ in range(4))
-                dY8, pts_hl = torch.empty(n, 8, **f16), torch.empty(n, 8, **f16)
-                dE, h = torch.empty(n, 40, **f16), torch.empty(n, 40, **f16)
-                d_out = torch.empty(n, 32, **f16)
-                d_gt = torch.empty(n, 3, **f32)
-                mo = _lib.NeusMlpBwdOut()
-                mo.H1, mo.H2, mo.dH1, mo.dH2 = H1.data_ptr(), H2.data_ptr(), dH1.data_ptr(), dH2.data_ptr()
-                mo.dY8, mo.dE, mo.d_out, mo.h = dY8.data_ptr(), dE.data_ptr(), d_out.data_ptr(), h.data_ptr()
-                mo.pts_hl, mo.d_grad_total = pts_hl.data_ptr(), d_gt.data_ptr()
-                rc = lib.goslam_neus_mlp_backward(ctypes.byref(p), _lib.ptr(X), _lib.ptr(enc[sl]), _lib.ptr(pos[sl]), _lib.ptr(d_y),
-                                                  _lib.ptr(d_s), _lib.ptr(d_g), _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(z_mid[sl]),
-                                                  _lib.ptr(sc), r1 - r0, S, ctypes.byref(mo), _lib.stream_ptr())
-                _lib.check(rc, "neus_mlp_backward")
-                # ---- weight gradients: GEMMs over the sample dimension (cuBLAS, fp16 in, fp32 out) ----
-                g_W3[:8] += torch.mm(dY8.t(), H2, out_dtype=torch.float32) / sc
-                g_W2 += torch.mm(dH2.t(), H1, out_dtype=torch.float32) / sc
-                g_W1 += torch.mm(dH1.t(), X, out_dtype=torch.float32) / sc
-                gb = torch.mm(pts_hl.t(), dE, out_dtype=torch.float32)                 # colour embedding sin(pts @ B)
-                g_B += (gb[:3, :33] + gb[3:6, :33]) / sc
-                gs = torch.mm(d_out.t(), h, out_dtype=torch.float32) / sc               # sdf_layer: out = W h + b
-                g_sdf_w += gs[:, :35]
-                g_sdf_b += gs[:, 35]
-                d_enc = torch.mm(d_out, Wsdf_enc, out_dtype=torch.float32)             # [n, 32] f32, still scaled
-                rc = lib.goslam_neus_grid_backward(ctypes.byref(p), _lib.ptr(ro), _lib.ptr(rd), _lib.ptr(zv), _lib.ptr(ds),
-                                                   _lib.ptr(fallback), ctypes.c_int64(r0 * S), r1 - r0, S, _lib.ptr(d_enc), _lib.ptr(sc), _lib.ptr(d_gt), _lib.ptr(g_grid),
-                                                   _lib.ptr(g_w0), _lib.stream_ptr())
-                _lib.check(rc, "neus_grid_backward")
+        for r0 in range(0, R, _NeusFunction.CHUNK_RAYS):
+            r1 = min(R, r0 + _NeusFunction.CHUNK_RAYS)
+            n = (r1 - r0) * S
+            sl = slice(r0, r1)
+            ro, rd, zv, ds = rays_o[sl], rays_d[sl], z_vals[sl], dists[sl]
+            d_y = torch.empty(n, 3, **f32); d_s = torch.empty(n, **f32); d_g = torch.empty(n, 3, **f32)
+            dc = None if d_color is None else d_color[sl].contiguous()
+            dd = None if d_depth is None else d_depth[sl].contiguous()
+            dsu = None if d_sdf is None else d_sdf[sl].contiguous()
+            _lib.call("neus_composite_backward", ctypes.byref(p), ro, rd, ds, alpha[sl], rgb[sl], sdf[sl], grad[sl],
+                      z_mid[sl], dc, dd, dsu, d_gerr, fallback, R * S, r0 * S, r1 - r0, S, d_y, d_s, d_g, g_inv_s)
+            amax = torch.maximum(d_y.abs().max(), d_s.abs().max()).clamp_min(1e-30)
+            sc = torch.exp2(torch.floor(torch.log2(1024.0 / amax))).clamp(max=2.0 ** 40).reshape(1).contiguous()   # device scalar
+            # ---- colour network, row-wise half (one kernel): H1, H2, dH2, dH1, dX and what hangs off dX per sample ----
+            X = mlp_in[sl].reshape(n, MLP_IN_PAD)                                 # half, as the forward built it
+            H1, H2, dH1, dH2 = (torch.empty(n, MLP_HID, **f16) for _ in range(4))
+            dY8, pts_hl = torch.empty(n, 8, **f16), torch.empty(n, 8, **f16)
+            dE, h = torch.empty(n, 40, **f16), torch.empty(n, 40, **f16)
+            d_out = torch.empty(n, 32, **f16)
+            d_gt = torch.empty(n, 3, **f32)
+            mo = _lib.NeusMlpBwdOut()
+            mo.H1, mo.H2, mo.dH1, mo.dH2 = H1.data_ptr(), H2.data_ptr(), dH1.data_ptr(), dH2.data_ptr()
+            mo.dY8, mo.dE, mo.d_out, mo.h = dY8.data_ptr(), dE.data_ptr(), d_out.data_ptr(), h.data_ptr()
+            mo.pts_hl, mo.d_grad_total = pts_hl.data_ptr(), d_gt.data_ptr()
+            _lib.call("neus_mlp_backward", ctypes.byref(p), X, enc[sl], pos[sl], d_y, d_s, d_g, ro, rd, z_mid[sl], sc,
+                      r1 - r0, S, ctypes.byref(mo))
+            # ---- weight gradients: GEMMs over the sample dimension (cuBLAS, fp16 in, fp32 out) ----
+            g_W3[:8] += torch.mm(dY8.t(), H2, out_dtype=torch.float32) / sc
+            g_W2 += torch.mm(dH2.t(), H1, out_dtype=torch.float32) / sc
+            g_W1 += torch.mm(dH1.t(), X, out_dtype=torch.float32) / sc
+            gb = torch.mm(pts_hl.t(), dE, out_dtype=torch.float32)                 # colour embedding sin(pts @ B)
+            g_B += (gb[:3, :33] + gb[3:6, :33]) / sc
+            gs = torch.mm(d_out.t(), h, out_dtype=torch.float32) / sc               # sdf_layer: out = W h + b
+            g_sdf_w += gs[:, :35]
+            g_sdf_b += gs[:, 35]
+            d_enc = torch.mm(d_out, Wsdf_enc, out_dtype=torch.float32)             # [n, 32] f32, still scaled
+            _lib.call("neus_grid_backward", ctypes.byref(p), ro, rd, zv, ds, fallback, r0 * S, r1 - r0, S, d_enc, sc,
+                      d_gt, g_grid, g_w0)
         g_sdf_w[0] += g_w0
         # samples the forward kept out of the network (outside the real-time bound and not among the first 100 of a
         # nothing-in-bound call): rgb = 0, alpha = 0, the kernels return zeros for them, so the GEMMs above see zero rows.

@@ -64,39 +64,28 @@ class CudaBackend:
         return self._ws
 
     def phase1(self, targets, weights, eta_by_frame, ii, jj, motion_only):
-        lib = self._lib.load()
         self.N = int(ii.shape[0])
         ws = self._workspace(self.N)
-        n_sys = lib.goslam_ba_system_doubles(self.t0, self.t1)
+        n_sys = self._lib.load().goslam_ba_system_doubles(self.t0, self.t1)
         system = torch.empty(n_sys, dtype=torch.float64, device=self.poses.device)
         # eta is FRAME-indexed here ([num, ht, wd]; eta_rows == num selects that form in the kernel),
         # so every rank reads the rows of its own frames whatever its local slot order is
         eta = eta_by_frame.reshape(self.num, -1)
         if not eta.is_contiguous() or eta.dtype != torch.float32:
             eta = eta.float().contiguous()
-        with torch.cuda.device(self.poses.device):
-            rc = lib.goslam_ba_phase1(
-                self._lib.ptr(self.poses), self._lib.ptr(self.disps), self._lib.ptr(self.intr), self._lib.ptr(self.sens),
-                self._lib.ptr(targets), self._lib.ptr(weights), self._lib.ptr(eta), -int(eta.shape[0]),
-                self._lib.ptr(ii), self._lib.ptr(jj), self.N, self.num, self.ht, self.wd, self.t0, self.t1,
-                int(bool(motion_only)), self._lib.ptr(system), self._lib.ptr(ws), ctypes.c_size_t(ws.numel()),
-                self._lib.stream_ptr())
-        self._lib.check(rc, "ba_phase1")
+        self._lib.call("ba_phase1", self.poses, self.disps, self.intr, self.sens, targets, weights, eta, -int(eta.shape[0]),
+                       ii, jj, self.N, self.num, self.ht, self.wd, self.t0, self.t1, int(bool(motion_only)), system, ws,
+                       ws.numel())
         return system
 
     def phase2(self, system, lm, ep, motion_only, owner_lo, owner_hi, return_status=False):
-        lib = self._lib.load()
         ws = self._workspace(self.N)
         dev = self.poses.device
         dx = torch.empty((self.t1 - self.t0, 6), dtype=torch.float32, device=dev)
         status = torch.zeros(1, dtype=torch.int32, device=dev) if return_status else None
-        with torch.cuda.device(dev):
-            rc = lib.goslam_ba_phase2(
-                self._lib.ptr(self.poses), self._lib.ptr(self.disps), self._lib.ptr(system), self.N, self.num,
-                self.ht, self.wd, self.t0, self.t1, float(lm), float(ep), int(bool(motion_only)),
-                int(owner_lo), int(owner_hi), self._lib.ptr(dx), None, self._lib.ptr(status),
-                self._lib.ptr(ws), ctypes.c_size_t(ws.numel()), self._lib.stream_ptr())
-        self._lib.check(rc, "ba_phase2")
+        self._lib.call("ba_phase2", self.poses, self.disps, system, self.N, self.num, self.ht, self.wd, self.t0, self.t1,
+                       float(lm), float(ep), int(bool(motion_only)), int(owner_lo), int(owner_hi), dx, None, status, ws,
+                       ws.numel())
         return (dx, status) if return_status else dx
 
 
@@ -109,8 +98,7 @@ class _PeerBuffer:
         self.shape, self.dtype = tuple(int(x) for x in shape), dtype
         nbytes = max(1, int(torch.empty((), dtype=dtype).element_size() * int(torch.Size(self.shape).numel())))
         ptr, handle = ctypes.c_void_p(), (ctypes.c_ubyte * 64)()
-        with torch.cuda.device(device):
-            lib_mod.check(lib_mod.load().goslam_peer_alloc(ctypes.c_size_t(nbytes), ctypes.byref(ptr), handle), "peer_alloc")
+        lib_mod.call("peer_alloc", nbytes, ctypes.byref(ptr), handle, device=device)
         self.ptr, self.handle, self.nbytes = int(ptr.value), bytes(handle), nbytes
         typestr = {torch.float32: "<f4", torch.float64: "<f8", torch.int32: "<i4", torch.uint8: "|u1"}[dtype]
         self.__cuda_array_interface__ = {"shape": self.shape, "typestr": typestr, "data": (self.ptr, False), "version": 2}
@@ -118,7 +106,7 @@ class _PeerBuffer:
 
     def __del__(self):
         try:
-            self._lib.load().goslam_peer_free(ctypes.c_void_p(self.ptr))
+            self._lib.call("peer_free", self.ptr)
         except Exception:
             pass
 
@@ -147,17 +135,15 @@ class PeerLink:
         dist.all_gather_object(handles, mine, group=group)
         self._mapped = []
         self.ptrs = {k: [0] * self.world for k in mine}
-        lib = _lib.load()
-        with torch.cuda.device(dev):
-            for r in range(self.world):
-                for k in mine:
-                    if r == self.rank:
-                        self.ptrs[k][r] = getattr(self, k).ptr
-                    else:
-                        q = ctypes.c_void_p()
-                        _lib.check(lib.goslam_ipc_open(handles[r][k], ctypes.byref(q)), "ipc_open")
-                        self.ptrs[k][r] = int(q.value)
-                        self._mapped.append(int(q.value))
+        for r in range(self.world):
+            for k in mine:
+                if r == self.rank:
+                    self.ptrs[k][r] = getattr(self, k).ptr
+                else:
+                    q = ctypes.c_void_p()
+                    _lib.call("ipc_open", handles[r][k], ctypes.byref(q), device=dev)
+                    self.ptrs[k][r] = int(q.value)
+                    self._mapped.append(int(q.value))
         self.epoch = 0
         torch.cuda.synchronize(dev)
         dist.barrier(group=group)                 # every rank's buffers are zeroed and mapped before the first signal
@@ -176,16 +162,13 @@ class PeerLink:
     def wait_idle(self):
         """stream-ordered: every rank has finished the last iteration (call before touching `disps.tensor` by hand)"""
         if self.epoch > 0 and self.world > 1:
-            peers = self.struct()
-            with torch.cuda.device(self.timeout.device):
-                self._lib.check(self._lib.load().goslam_ba_peers_wait(ctypes.byref(peers), self._lib.stream_ptr()), "ba_peers_wait")
+            self._lib.call("ba_peers_wait", ctypes.byref(self.struct()), device=self.timeout.device)
 
     def close(self):
-        lib = self._lib.load()
         torch.cuda.synchronize(self.timeout.device)
         dist.barrier(group=self.group)            # nobody still reads my buffers
         for q in self._mapped:
-            lib.goslam_ipc_close(ctypes.c_void_p(q))
+            self._lib.call("ipc_close", q)
         self._mapped = []
 
 
@@ -198,7 +181,6 @@ class PeerBackend(CudaBackend):
         self.link = link
 
     def iteration(self, targets, weights, eta_by_frame, ii, jj, lm, ep, motion_only, owner_lo, owner_hi):
-        lib = self._lib.load()
         self.N = int(ii.shape[0])
         ws = self._workspace(self.N)
         eta = eta_by_frame.reshape(self.num, -1)
@@ -208,18 +190,12 @@ class PeerBackend(CudaBackend):
         peers = self.link.struct()
         dev = self.poses.device
         dx = torch.empty((self.t1 - self.t0, 6), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.goslam_ba_phase1_peers(
-                self._lib.ptr(self.poses), self._lib.ptr(self.intr), self._lib.ptr(self.sens), self._lib.ptr(targets),
-                self._lib.ptr(weights), self._lib.ptr(eta), -int(eta.shape[0]), self._lib.ptr(ii), self._lib.ptr(jj), self.N,
-                self.num, self.ht, self.wd, self.t0, self.t1, int(bool(motion_only)), ctypes.byref(peers), self._lib.ptr(ws),
-                ctypes.c_size_t(ws.numel()), self._lib.stream_ptr())
-            self._lib.check(rc, "ba_phase1_peers")
-            rc = lib.goslam_ba_phase2_peers(
-                self._lib.ptr(self.poses), self.N, self.num, self.ht, self.wd, self.t0, self.t1, float(lm), float(ep),
-                int(bool(motion_only)), int(owner_lo), int(owner_hi), ctypes.byref(peers), self._lib.ptr(dx), None, None,
-                self._lib.ptr(ws), ctypes.c_size_t(ws.numel()), self._lib.stream_ptr())
-            self._lib.check(rc, "ba_phase2_peers")
+        self._lib.call("ba_phase1_peers", self.poses, self.intr, self.sens, targets, weights, eta, -int(eta.shape[0]), ii,
+                       jj, self.N, self.num, self.ht, self.wd, self.t0, self.t1, int(bool(motion_only)),
+                       ctypes.byref(peers), ws, ws.numel())
+        self._lib.call("ba_phase2_peers", self.poses, self.N, self.num, self.ht, self.wd, self.t0, self.t1, float(lm),
+                       float(ep), int(bool(motion_only)), int(owner_lo), int(owner_hi), ctypes.byref(peers), dx, None, None,
+                       ws, ws.numel())
         return dx
 
 

@@ -7,12 +7,9 @@ eager [R,S] kernels and a torch.sort).  The two linspace tables and the shared
 `perturb_rand[N_samples]` (src/render.py:159) still come from torch, so the RNG stream advances
 exactly as in the reference and z_vals are bit-identical to it for the same RNG state.
 """
-import ctypes
-
 import torch
 
 from . import _lib
-from .droid_backends import _workspace
 from .mapping import all_rays
 
 _tables = {}
@@ -30,8 +27,7 @@ def _linspace_tables(n_samples, n_surface, device):
 def sample_z(rays_o, rays_d, bound, gt_depth, n_samples, n_surface, perturb=1.0, lindisp=False):
     """Returns z_vals [R, S], dists [R, S] with S = n_samples (+ n_surface when gt_depth is given)."""
     device = rays_o.device
-    if not rays_o.is_cuda:
-        raise RuntimeError("sample_z: CUDA tensors required (no CPU fallback)")
+    _lib.need_cuda("sample_z", rays_o)
     R = int(rays_o.shape[0])
     if gt_depth is None:
         n_surface = 0
@@ -44,13 +40,9 @@ def sample_z(rays_o, rays_d, bound, gt_depth, n_samples, n_surface, perturb=1.0,
     gd = gt_depth.reshape(-1).float().contiguous() if gt_depth is not None else None
     z_vals = torch.empty((R, S), dtype=torch.float32, device=device)
     dists = torch.empty((R, S), dtype=torch.float32, device=device)
-    ws = _workspace(256, device)
-    with torch.cuda.device(device):
-        rc = _lib.load().goslam_sample_z(_lib.ptr(ro), _lib.ptr(rd), _lib.ptr(bd), _lib.ptr(gd), _lib.ptr(tv),
-                                         _lib.ptr(ts), _lib.ptr(rand), R, n_samples, n_surface, int(bool(lindisp)),
-                                         _lib.ptr(z_vals), _lib.ptr(dists), _lib.ptr(ws),
-                                         ctypes.c_size_t(ws.numel()), _lib.stream_ptr())
-    _lib.check(rc, "sample_z")
+    ws = _lib.workspace(256, device)
+    _lib.call("sample_z", ro, rd, bd, gd, tv, ts, rand, R, n_samples, n_surface, int(bool(lindisp)), z_vals, dists, ws,
+              ws.numel())
     return z_vals, dists
 
 

@@ -86,17 +86,14 @@ def ape(ref_poses, est_positions):
     dev = ref.device
     ref = ref.to(torch.float64).contiguous()
     est = est.to(torch.float64).contiguous()
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        nbytes = lib.goslam_ape_workspace_bytes(n)
-        if nbytes == 0:
-            raise ValueError("ape: %d poses is more than the library takes" % n)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        out = torch.empty(OUT, dtype=torch.float64, device=dev)
-        errors = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
-        _lib.check(lib.goslam_ape_sim3(_lib.ptr(est), _lib.ptr(ref), n, _lib.ptr(ws), nbytes, _lib.ptr(out),
-                                       _lib.ptr(errors), _lib.stream_ptr()), "ape_sim3")
-        host = out.cpu().numpy()
+    nbytes = _lib.load().goslam_ape_workspace_bytes(n)
+    if nbytes == 0:
+        raise ValueError("ape: %d poses is more than the library takes" % n)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    out = torch.empty(OUT, dtype=torch.float64, device=dev)
+    errors = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
+    _lib.call("ape_sim3", est, ref, n, ws, nbytes, out, errors)
+    host = out.cpu().numpy()
     status = int(host[0])
     if status != 0:
         raise ValueError(MESSAGES.get(status, "APE: status %d" % status))

@@ -46,12 +46,8 @@ def fill_interpolate(video, N, tt, intrinsics, depths=None):
     depths = depths.to(dev, torch.float32).contiguous() if depths is not None else None
     t0 = torch.empty(M, dtype=torch.long, device=dev)
     t1 = torch.empty(M, dtype=torch.long, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().goslam_fill_interpolate(
-            _lib.ptr(video.timestamp), _lib.ptr(video.poses), _lib.ptr(video.intrinsics), _lib.ptr(video.disps),
-            _lib.ptr(video.disps_sens), N, M, _lib.ptr(tt), _lib.ptr(intrinsics), _lib.ptr(depths), H, W,
-            _lib.ptr(t0), _lib.ptr(t1), _lib.stream_ptr())
-    _lib.check(rc, "fill_interpolate")
+    _lib.call("fill_interpolate", video.timestamp, video.poses, video.intrinsics, video.disps, video.disps_sens, N, M, tt,
+              intrinsics, depths, H, W, t0, t1)
     return t0, t1
 
 

@@ -27,6 +27,123 @@ def test_header_symbols_exported(lib):
     assert sorted(_lib.SIGNATURES) == names, "binding declares symbols the header does not"
 
 
+P = ctypes.c_void_p
+_C_STRUCTS = {"goslam_neus_params": "NeusParams", "goslam_neus_out": "NeusOut", "goslam_neus_mlp_bwd_out": "NeusMlpBwdOut",
+              "goslam_ba_peers": "BaPeers", "goslam_gru_weights": "GruWeights", "goslam_update_weights": "UpdateWeights",
+              "goslam_conv_desc": "ConvDesc", "goslam_encoder_conv": "EncoderConv",
+              "goslam_encoder_weights": "EncoderWeights"}
+
+
+def _prototypes():
+    """(return type, name, [parameter declarations]) of every prototype: a line-anchored scan of the header"""
+    src = open(os.path.join(ROOT, "include", "goslam_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    out = []
+    for m in re.finditer(r"^(int|size_t|int64_t|const char\*) (goslam_[a-z0-9_]+)\((.*?)\);", src, flags=re.M | re.S):
+        params = [" ".join(p.split()) for p in m.group(3).split(",")]
+        out.append((m.group(1), m.group(2), [] if params == ["void"] else params))
+    return out
+
+
+def _expected_type(decl):
+    from goslam_b200 import _lib
+    words = decl.replace("*", " * ").split()
+    if decl in ("int", "size_t", "int64_t", "const char*"):          # return types
+        words = words + ["_"]
+    words = [w for w in words[:-1] if w != "const"]
+    if "*" not in words:
+        return {"int": ctypes.c_int, "unsigned": ctypes.c_uint, "float": ctypes.c_float, "double": ctypes.c_double,
+                "size_t": ctypes.c_size_t, "int64_t": ctypes.c_int64, "long long": ctypes.c_int64}[" ".join(words)]
+    if words == ["char", "*"]:
+        return ctypes.c_char_p
+    if words[0] in _C_STRUCTS and words[1:] == ["*"]:
+        return ctypes.POINTER(getattr(_lib, _C_STRUCTS[words[0]]))
+    return P
+
+
+def test_every_prototype_is_bound_with_its_header_types(lib):
+    protos = _prototypes()
+    assert len(protos) == len(_declared_symbols())
+    for ret, name, params in protos:
+        fn = getattr(lib, name)
+        assert fn.restype == _expected_type(ret), name
+        assert fn.argtypes == [_expected_type(p) for p in params], name
+
+
+def test_derived_signatures_written_out():
+    from goslam_b200 import _lib
+    sigs = _lib.parse_header(open(_lib.HEADER).read())
+    i, f, d, z, i64 = ctypes.c_int, ctypes.c_float, ctypes.c_double, ctypes.c_size_t, ctypes.c_int64
+    assert sigs["goslam_ba"] == (i, [P] * 7 + [i] + [P] * 2 + [i] * 7 + [f, f, i] + [P] * 3 + [P, z, P], True)
+    assert sigs["goslam_neus_forward"] == (i, [ctypes.POINTER(_lib.NeusParams)] + [P] * 4 + [i, i] +
+                                           [ctypes.POINTER(_lib.NeusOut), P, z, P], True)
+    assert sigs["goslam_mapping_rays"] == (i, [P, z, i, i, i, P, P, i64, i, P, P, P, d, d, d, d, P, P, P, P, i64, P],
+                                           True)
+    assert sigs["goslam_ape_sim3"] == (i, [P, P, i64, P, z, P, P, P], True)
+    assert sigs["goslam_neus_composite_backward"][1][14:18] == [i64, i64, i, i]          # long long
+    assert sigs["goslam_strerror"] == (ctypes.c_char_p, [i], False)
+    assert sigs["goslam_ape_workspace_bytes"] == (z, [i64], False)
+    assert sigs["goslam_peer_alloc"] == (i, [z, P, P], False)
+
+
+def test_unknown_c_type_is_an_error():
+    from goslam_b200 import _lib
+    with pytest.raises(ValueError, match="goslam_probe"):
+        _lib.parse_header("int goslam_probe(const float* x, struct unknown u, void* stream);")
+    with pytest.raises(ValueError, match="goslam_probe_ret"):
+        _lib.parse_header("half goslam_probe_ret(int n);")
+
+
+def test_structures_match_the_c_layout(tmp_path):
+    """sizeof and every field's offsetof of each C struct, from a C99 program compiled against the header"""
+    import shutil
+    import subprocess
+    from goslam_b200 import _lib
+    gcc = shutil.which("gcc")
+    if gcc is None:
+        pytest.skip("gcc is missing")
+    lines = ["#include <stdio.h>", "#include <stddef.h>", '#include "goslam_b200.h"', "int main(void) {"]
+    for cname, pyname in _C_STRUCTS.items():
+        lines.append('  printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
+        for field, _ in getattr(_lib, pyname)._fields_:
+            cfield = "in" if field == "inp" else field
+            lines.append('  printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (cname, field, cname, cfield))
+    lines += ["  return 0;", "}"]
+    src, exe = tmp_path / "layout.c", str(tmp_path / "layout")
+    src.write_text("\n".join(lines) + "\n")
+    subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-pedantic", "-I", os.path.join(ROOT, "include"), str(src),
+                    "-o", exe], check=True)
+    got = dict(line.split() for line in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.splitlines())
+    want = {}
+    for cname, pyname in _C_STRUCTS.items():
+        cls = getattr(_lib, pyname)
+        want[cname] = str(ctypes.sizeof(cls))
+        for field, _ in cls._fields_:
+            want["%s.%s" % (cname, field)] = str(getattr(cls, field).offset)
+    assert got == want
+    assert {c: int(got[c]) for c in _C_STRUCTS} == {
+        "goslam_neus_params": 96, "goslam_neus_out": 120, "goslam_neus_mlp_bwd_out": 80, "goslam_ba_peers": 216,
+        "goslam_gru_weights": 64, "goslam_update_weights": 240, "goslam_conv_desc": 168, "goslam_encoder_conv": 16,
+        "goslam_encoder_weights": 320}
+
+
+def test_call_rejects_a_cpu_tensor_before_the_library(monkeypatch):
+    import torch
+    from goslam_b200 import _lib
+
+    class Unreachable:
+        def __getattr__(self, name):
+            def fn(*args):
+                raise AssertionError("%s reached the library" % name)
+            return fn
+    monkeypatch.setattr(_lib, "_LIB", Unreachable())
+    cpu = torch.zeros(4, 7)
+    with pytest.raises(RuntimeError, match="no CPU fallback"):
+        _lib.call("iproj", cpu, cpu, cpu, cpu, 1, 1, 1)
+    with pytest.raises(RuntimeError, match="CUDA"):
+        _lib.call("frame_distance", None, None, None, None, None, cpu, 0, 4, 4, 0.3)
+
+
 def test_identification(lib):
     assert lib.goslam_version() == 100
     assert lib.goslam_sm_arch() == 90
