@@ -822,6 +822,7 @@ struct CompBwdArgs {
   float* d_sdf_out;                  // [R,S]
   float* d_grad;                     // [R,S,3]
   float* d_inv_s;                    // [1], accumulated
+  float* d_true_cos;                 // [R,S] dL/d(rays_d . normal) through get_alpha, or null
   int R, S;
 };
 
@@ -895,7 +896,7 @@ __global__ void __launch_bounds__(256) neus_composite_bwd_kernel(const CompBwdAr
 #pragma unroll
         for (int k = 0; k < 3; ++k) pt[k] = __fadd_rn(o[k], __fmul_rn(dir[k], zm));
         const bool inb = sample_in_bound(pt, a.p.rt_bound, a.sample0 + (long long)gi, forced);
-        float dx[3] = {0.f, 0.f, 0.f}, dsdf = 0.f, dg[3] = {0.f, 0.f, 0.f};
+        float dx[3] = {0.f, 0.f, 0.f}, dsdf = 0.f, dg[3] = {0.f, 0.f, 0.f}, dtc = 0.f;
         if (inb) {
           const float d_alpha = G[c] * T[c] - suffix / (1.0f - al[c] + 1e-7f);
 #pragma unroll
@@ -922,6 +923,7 @@ __global__ void __launch_bounds__(256) neus_composite_bwd_kernel(const CompBwdAr
             const float d_tc = d_ic * ((r0 > 0.f ? 0.5f * (1.0f - car) : 0.f) + (r1 > 0.f ? car : 0.f));
 #pragma unroll
             for (int k = 0; k < 3; ++k) dg[k] = d_tc * dir[k];
+            dtc = d_tc;
           }
           if (a.d_sdf) dsdf += a.d_sdf[gi];
           // ---- eikonal term: gradient_error = mean_n((|g| - 1)^2 * mask) ----
@@ -933,6 +935,7 @@ __global__ void __launch_bounds__(256) neus_composite_bwd_kernel(const CompBwdAr
           }
         }
         a.d_sdf_out[gi] = dsdf;
+        if (a.d_true_cos) a.d_true_cos[gi] = dtc;
 #pragma unroll
         for (int k = 0; k < 3; ++k) { a.d_mlp_out[gi * 3 + k] = dx[k]; a.d_grad[gi * 3 + k] = dg[k]; }
       }
@@ -1092,6 +1095,171 @@ __global__ void __launch_bounds__(256) neus_grid_bwd_kernel(const GridBwdArgs a)
   }
 }
 
+
+// ------------------------------------------------------------------------------------------------------
+// neus_ray_bwd_kernel — dL/d rays_o and dL/d rays_d (camera refinement, src/mapping.py:173-194 with mapping.BA).  A sample
+// at p = o + z d (z = z_mid, which carries no gradient) that went through the network reaches the loss through
+//   (1) sdf_layer's include_xyz columns:  dL/dx d_xyz, x = clamp((p - b0)/(b1 - b0) 2 - 1, -1, 1)
+//   (2) the hash-grid encoding, first order: dL/d enc . d enc/d u, u = (x + 1)/2, per level times its scale
+//   (3) the analytic normal n = d sdf/d p, second order: dL/dn . d n/d p — inside a cell the trilinear interpolant's
+//       only second derivatives are the mixed partials d2/du_a du_b (a != b), scaled 0.25 (2/(b1-b0))_a (2/(b1-b0))_b
+//   (4) the colour embedding sin(p B) in world p:  dE B^T
+// and the direction also enters get_alpha through true_cos = d . n.  Per ray:
+//   dL/d o = sum_s dL/dp_s,   dL/d d = sum_s z_s dL/dp_s + sum_s (dL/d true_cos_s) n_s.
+// One warp per ray, lane per sample in steps of 32, the per-ray sums by a fixed butterfly: no atomics, the result does
+// not depend on how the caller chunks the rays.  A separate kernel rather than a variant of neus_grid_bwd_kernel: that
+// one is thread per sample across rays and its scatter aggregation wants runs of lanes in one cell, this one reduces
+// per ray.
+// ------------------------------------------------------------------------------------------------------
+struct RayBwdArgs {
+  goslam_neus_params p;
+  const float* rays_o; const float* rays_d; const float* z_vals; const float* dists;
+  const float* d_enc;                // [n,32] dL/d(encoding), times *scale
+  const float* d_xyz;                // [n,3]  dL/d x through sdf_layer's include_xyz columns, times *scale
+  const __half* dE;                  // [n,40] dL/d(p . B_j), 33 columns used, times *scale
+  const float* scale;                // device scalar or null (1)
+  const float* d_grad;               // [n,3]  dL/d normal (all paths), unscaled
+  const float* d_true_cos;           // [n]    dL/d true_cos through get_alpha, unscaled
+  const int* fallback;               // the forward's nothing-in-bound flag (device, may be null = 0)
+  long long sample0;                 // index of this call's first sample within the forward call
+  float* d_rays_o; float* d_rays_d;  // [R,3]
+  int R, S;
+};
+
+// gradient of the trilinear interpolant of the corner field f (corner q = x bit 0, y bit 1, z bit 2) w.r.t. the cell
+// coordinates, at the weights w*[0] = 1 - fraction, w*[1] = fraction
+__device__ __forceinline__ void trilinear_grad(const float (&f)[8], const float (&wx)[2], const float (&wy)[2],
+                                               const float (&wz)[2], float (&g)[3]) {
+  g[0] = wz[0] * fmaf(wy[1], f[3] - f[2], wy[0] * (f[1] - f[0])) + wz[1] * fmaf(wy[1], f[7] - f[6], wy[0] * (f[5] - f[4]));
+  g[1] = wz[0] * fmaf(wx[1], f[3] - f[1], wx[0] * (f[2] - f[0])) + wz[1] * fmaf(wx[1], f[7] - f[5], wx[0] * (f[6] - f[4]));
+  g[2] = wy[0] * fmaf(wx[1], f[5] - f[1], wx[0] * (f[4] - f[0])) + wy[1] * fmaf(wx[1], f[7] - f[3], wx[0] * (f[6] - f[2]));
+}
+
+__global__ void __launch_bounds__(256, 2) neus_ray_bwd_kernel(const RayBwdArgs a) {
+  __shared__ float colB[99];
+  for (int i = threadIdx.x; i < 99; i += blockDim.x) colB[i] = a.p.color_B[i];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= a.R) return;
+  const int S = a.S;
+  float o[3], dir[3], w0[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    o[c] = a.rays_o[(size_t)r * 3 + c];
+    dir[c] = a.rays_d[(size_t)r * 3 + c];
+    w0[c] = __ldg(a.p.sdf_w + c);
+  }
+  const bool forced = a.fallback && __ldg(a.fallback) != 0;
+  const float inv_sc = a.scale ? 1.0f / __ldg(a.scale) : 1.0f;
+  const __half2* table = reinterpret_cast<const __half2*>(a.p.grid);
+  float acc_o[3] = {0.f, 0.f, 0.f}, acc_d[3] = {0.f, 0.f, 0.f};
+  for (int s = lane; s < S; s += 32) {
+    const size_t gi = (size_t)r * S + s;
+    const float zm = __fadd_rn(a.z_vals[gi], a.dists[gi] / 2.0f);
+    float pt[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pt[c] = __fadd_rn(o[c], __fmul_rn(dir[c], zm));
+    if (!sample_in_bound(pt, a.p.rt_bound, a.sample0 + (long long)gi, forced)) continue;
+    float xn[3], dscale[3], x01[3], q[3];
+    float g1[3] = {0.f, 0.f, 0.f}, g2[3] = {0.f, 0.f, 0.f}, genc[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      normalise_coord(pt[c], a.p.bound[2 * c], a.p.bound[2 * c + 1], xn[c], dscale[c], x01[c]);
+      q[c] = 0.5f * dscale[c] * a.d_grad[gi * 3 + c];            // dL/d genc_c (normal_c = (W0[c] + 0.5 genc_c) dscale_c)
+    }
+#pragma unroll 2
+    for (int l = 0; l < kLevels; ++l) {
+      const LevelConst L = c_lvl[l];
+      unsigned pg[3];
+      float fr[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float pos = fmaf(L.scale, x01[c], 0.5f);
+        const float fl = floorf(pos);
+        pg[c] = (unsigned)fl; fr[c] = pos - fl;
+      }
+      float2 vf[8];
+#pragma unroll
+      for (int c8 = 0; c8 < 8; ++c8) {
+        const int bx = c8 & 1, by = (c8 >> 1) & 1, bz = (c8 >> 2) & 1;
+        unsigned ix;
+        if (l >= kDenseLevels) {
+          ix = ((pg[0] + bx) ^ ((pg[1] + by) * 2654435761u) ^ ((pg[2] + bz) * 805459861u)) & 0x7FFFFu;
+        } else {
+          ix = (pg[0] + bx) + (pg[1] + by) * L.res + (pg[2] + bz) * L.res2;
+          ix = ix >= L.size ? ix - L.size : ix;
+        }
+        vf[c8] = __half22float2(__ldg(table + L.offset + ix));
+      }
+      const float2 de = __ldg(reinterpret_cast<const float2*>(a.d_enc + gi * 32 + 2 * l));
+      // what the forward contracts this level's features with for the normal: W0[3:] rounded to half (tcnn's dL/dy)
+      const float gy0 = __half2float(__float2half_rn(__ldg(a.p.sdf_w + 3 + 2 * l)));
+      const float gy1 = __half2float(__float2half_rn(__ldg(a.p.sdf_w + 4 + 2 * l)));
+      float cg[8], cd[8];
+#pragma unroll
+      for (int c8 = 0; c8 < 8; ++c8) {
+        cg[c8] = fmaf(vf[c8].y, gy1, vf[c8].x * gy0);
+        cd[c8] = fmaf(vf[c8].y, de.y, vf[c8].x * de.x);
+      }
+      const float wx[2] = {1.f - fr[0], fr[0]}, wy[2] = {1.f - fr[1], fr[1]}, wz[2] = {1.f - fr[2], fr[2]};
+      float gg[3], gd[3];
+      trilinear_grad(cg, wx, wy, wz, gg);
+      trilinear_grad(cd, wx, wy, wz, gd);
+      // mixed second partials of the normal's field
+      const float hxy = wz[0] * ((cg[3] - cg[2]) - (cg[1] - cg[0])) + wz[1] * ((cg[7] - cg[6]) - (cg[5] - cg[4]));
+      const float hxz = wy[0] * ((cg[5] - cg[4]) - (cg[1] - cg[0])) + wy[1] * ((cg[7] - cg[6]) - (cg[3] - cg[2]));
+      const float hyz = wx[0] * ((cg[6] - cg[4]) - (cg[2] - cg[0])) + wx[1] * ((cg[7] - cg[5]) - (cg[3] - cg[1]));
+      const float s2 = L.scale * L.scale;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        genc[c] = fmaf(L.scale, gg[c], genc[c]);
+        g1[c] = fmaf(L.scale, gd[c], g1[c]);
+      }
+      g2[0] = fmaf(s2, fmaf(q[1], hxy, q[2] * hxz), g2[0]);
+      g2[1] = fmaf(s2, fmaf(q[0], hxy, q[2] * hyz), g2[1]);
+      g2[2] = fmaf(s2, fmaf(q[0], hxz, q[1] * hyz), g2[2]);
+    }
+    // colour embedding: dL/dp += sum_j dE_j B[:, j]
+    float emb[3] = {0.f, 0.f, 0.f};
+    {
+      const uint4* er = reinterpret_cast<const uint4*>(a.dE + gi * 40);
+#pragma unroll
+      for (int v = 0; v < 5; ++v) {
+        const uint4 u = __ldg(er + v);
+        const unsigned w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 e2 = make_float2(__half2float(__ushort_as_half((unsigned short)(w4[k] & 0xFFFFu))),
+                                        __half2float(__ushort_as_half((unsigned short)(w4[k] >> 16))));
+          const int j = 8 * v + 2 * k;
+          if (j < 33) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) emb[c] = fmaf(e2.x, colB[33 * c + j], emb[c]);
+          }
+          if (j + 1 < 33) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) emb[c] = fmaf(e2.y, colB[33 * c + j + 1], emb[c]);
+          }
+        }
+      }
+    }
+    const float dtc = a.d_true_cos[gi];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float dxn = __ldg(a.d_xyz + gi * 3 + c) + 0.5f * g1[c];            // scaled units
+      const float dp = dscale[c] * fmaf(dxn, inv_sc, 0.5f * g2[c]) + emb[c] * inv_sc;
+      const float nrm = fmaf(0.5f, genc[c], w0[c]) * dscale[c];
+      acc_o[c] += dp;
+      acc_d[c] = fmaf(dtc, nrm, fmaf(zm, dp, acc_d[c]));
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float vo = gs_warp_sum(acc_o[c]), vd = gs_warp_sum(acc_d[c]);
+    if (lane == 0) { a.d_rays_o[(size_t)r * 3 + c] = vo; a.d_rays_d[(size_t)r * 3 + c] = vd; }
+  }
+}
 
 // ------------------------------------------------------------------------------------------------------
 // neus_mlp_bwd_kernel — the row-wise half of the colour network's backward in ONE pass per 32-sample warp tile:
@@ -1396,12 +1564,12 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, c
   return GOSLAM_OK;
 }
 
-int goslam_neus_composite_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
-                                   const float* dists, const float* alpha, const float* rgb, const float* sdf,
-                                   const float* grad, const float* z_mid, const float* d_color, const float* d_depth,
-                                   const float* d_sdf, const float* d_gradient_error, const int* fallback,
-                                   long long total_samples, long long sample0, int R, int S,
-                                   float* d_mlp_out, float* d_sdf_out, float* d_grad, float* d_inv_s, void* stream) {
+int goslam_neus_composite_backward_ex(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
+                                      const float* dists, const float* alpha, const float* rgb, const float* sdf,
+                                      const float* grad, const float* z_mid, const float* d_color, const float* d_depth,
+                                      const float* d_sdf, const float* d_gradient_error, const int* fallback,
+                                      long long total_samples, long long sample0, int R, int S, float* d_mlp_out,
+                                      float* d_sdf_out, float* d_grad, float* d_inv_s, float* d_true_cos, void* stream) {
   if (!params || !rays_o || !rays_d || !dists || !alpha || !rgb || !sdf || !grad || !z_mid || !d_mlp_out || !d_sdf_out ||
       !d_grad || !d_inv_s || R < 0 || S <= 0 || S > 32 * kCompChunks || sample0 < 0 ||
       total_samples < sample0 + (long long)R * S)
@@ -1413,11 +1581,22 @@ int goslam_neus_composite_backward(const goslam_neus_params* params, const float
   a.d_color = d_color; a.d_depth = d_depth; a.d_sdf = d_sdf; a.d_gerr = d_gradient_error;
   a.fallback = fallback; a.sample0 = sample0;
   a.gerr_norm = total_samples > 0 ? (float)(1.0 / (double)total_samples) : 0.f;
-  a.d_mlp_out = d_mlp_out; a.d_sdf_out = d_sdf_out; a.d_grad = d_grad; a.d_inv_s = d_inv_s;
+  a.d_mlp_out = d_mlp_out; a.d_sdf_out = d_sdf_out; a.d_grad = d_grad; a.d_inv_s = d_inv_s; a.d_true_cos = d_true_cos;
   a.R = R; a.S = S;
   neus_composite_bwd_kernel<<<gs_cdiv(R, 8), 256, 0, (cudaStream_t)stream>>>(a);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
+}
+
+int goslam_neus_composite_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
+                                   const float* dists, const float* alpha, const float* rgb, const float* sdf,
+                                   const float* grad, const float* z_mid, const float* d_color, const float* d_depth,
+                                   const float* d_sdf, const float* d_gradient_error, const int* fallback,
+                                   long long total_samples, long long sample0, int R, int S,
+                                   float* d_mlp_out, float* d_sdf_out, float* d_grad, float* d_inv_s, void* stream) {
+  return goslam_neus_composite_backward_ex(params, rays_o, rays_d, dists, alpha, rgb, sdf, grad, z_mid, d_color, d_depth,
+                                           d_sdf, d_gradient_error, fallback, total_samples, sample0, R, S, d_mlp_out,
+                                           d_sdf_out, d_grad, d_inv_s, nullptr, stream);
 }
 
 int goslam_neus_mlp_backward(const goslam_neus_params* params, const void* mlp_in, const void* enc, const float* pos,
@@ -1464,6 +1643,26 @@ int goslam_neus_grid_backward(const goslam_neus_params* params, const float* ray
   const long long blocks = (a.n + 255) / 256;
   if (blocks > 0x7fffffffLL) return GOSLAM_EINVAL;
   neus_grid_bwd_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(a);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
+}
+
+int goslam_neus_ray_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
+                             const float* z_vals, const float* dists, const int* fallback, long long sample0, int R, int S,
+                             const float* d_enc, const float* d_xyz, const void* dE, const float* scale, const float* d_grad,
+                             const float* d_true_cos, float* d_rays_o, float* d_rays_d, void* stream) {
+  if (!params || !rays_o || !rays_d || !z_vals || !dists || !d_enc || !d_xyz || !dE || !d_grad || !d_true_cos || !d_rays_o ||
+      !d_rays_d || R < 0 || S <= 0 || S > 32 * kCompChunks || sample0 < 0)
+    return GOSLAM_EINVAL;
+  if (R == 0) return GOSLAM_OK;
+  { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
+  RayBwdArgs a{};
+  a.p = *params; a.rays_o = rays_o; a.rays_d = rays_d; a.z_vals = z_vals; a.dists = dists;
+  a.d_enc = d_enc; a.d_xyz = d_xyz; a.dE = reinterpret_cast<const __half*>(dE); a.scale = scale; a.d_grad = d_grad;
+  a.d_true_cos = d_true_cos; a.fallback = fallback; a.sample0 = sample0;
+  a.d_rays_o = d_rays_o; a.d_rays_d = d_rays_d;
+  a.R = R; a.S = S;
+  neus_ray_bwd_kernel<<<gs_cdiv(R, 8), 256, 0, (cudaStream_t)stream>>>(a);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

@@ -19,6 +19,8 @@ returned tensors carry a grad_fn: `loss.backward()` runs goslam_neus_composite_b
 weight-gradient GEMMs (cuBLAS) and goslam_neus_grid_backward, and fills `.grad` of the hash grid, sdf_layer, colour `_B`, colour
 network and variance parameters (SURVEY 8f-3).  Differentiable outputs: color, depth, sdf, gradient_error; the other
 keys are returned detached (the reference's losses use depth_variance detached and never read normal / weight_sum).
+When rays_o or rays_d requires grad (camera refinement: rays built from a pose leaf), the backward also runs
+goslam_neus_ray_backward and returns dL/d rays_o, dL/d rays_d in the rays' dtype; the parameter gradients are the same.
 """
 import ctypes
 import math
@@ -222,12 +224,14 @@ class InstantNeuS(nn.Module):
 
     def forward(self, rays_o, rays_d, z_vals, dists, render_params: dict = None, debug=False):
         """debug=True (tests only): additionally keeps the per-sample NeuS alpha [R,S] and SDF normal [R,S,3]
-        in `self.last_debug`.  With grad enabled and any trainable parameter requiring grad: differentiable."""
+        in `self.last_debug`.  With grad enabled and any trainable parameter, rays_o or rays_d requiring grad:
+        differentiable, also w.r.t. the rays (camera refinement, src/mapping.py:173-194).  z_vals and dists are sampled
+        from detached rays and carry no gradient."""
         params = self.trainable_tensors()
-        if torch.is_grad_enabled() and not debug and any(p.requires_grad for p in params):
-            if any(t.requires_grad for t in (rays_o, rays_d, z_vals, dists)):
-                raise RuntimeError("InstantNeuS.forward: gradients w.r.t. rays / depths are not implemented "
-                                   "(the mapping step optimises the scene representation only)")
+        if torch.is_grad_enabled() and not debug and any(t.requires_grad for t in params + (rays_o, rays_d)):
+            if z_vals.requires_grad or dists.requires_grad:
+                raise RuntimeError("InstantNeuS.forward: gradients w.r.t. z_vals / dists are not implemented "
+                                   "(the renderer samples them from detached rays)")
             vals = _NeusFunction.apply(self, rays_o, rays_d, z_vals, dists, *params)
             return dict(zip(_NeusFunction.KEYS, vals))
         return self._forward_impl(rays_o, rays_d, z_vals, dists, debug=debug)
@@ -411,8 +415,9 @@ class _NeusFunction(torch.autograd.Function):
     forward : the fused marcher with its per-sample intermediates kept.
     backward: goslam_neus_composite_backward -> goslam_neus_mlp_backward (row-wise colour-network backward on mma.sync)
               -> weight-gradient GEMMs over the sample dimension (cuBLAS, fp16 in / fp32 out, loss scale)
-              -> goslam_neus_grid_backward (hash-grid scatter + the second-order path through the analytic normal).
-              Chunked over rays to bound the activations."""
+              -> goslam_neus_grid_backward (hash-grid scatter + the second-order path through the analytic normal)
+              -> goslam_neus_ray_backward when rays_o or rays_d needs a gradient (composite_backward_ex then also keeps
+              dL/d true_cos).  Chunked over rays to bound the activations."""
     CHUNK_RAYS = 1 << 16
     MAX_SAMPLES = 128            # goslam_neus_composite_backward keeps up to 4 chunks of 32 samples of a ray in registers
     KEYS = ('color', 'depth', 'sdf', 'gradient_error', 'depth_variance', 'normal', 'weight_sum', 'z_vals', 'sdf_variance')
@@ -424,6 +429,7 @@ class _NeusFunction(torch.autograd.Function):
                                "got %d (the forward alone, under torch.no_grad(), takes up to 288)"
                                % (_NeusFunction.MAX_SAMPLES, z_vals.shape[1]))
         ctx.set_materialize_grads(False)
+        ctx.ray_dtypes = (rays_o.dtype, rays_d.dtype)
         rays_o, rays_d = rays_o.detach().float().contiguous(), rays_d.detach().float().contiguous()
         z_vals, dists = z_vals.detach().float().contiguous(), dists.detach().float().contiguous()
         out = net._forward_impl(rays_o, rays_d, z_vals, dists, train=True)
@@ -464,6 +470,10 @@ class _NeusFunction(torch.autograd.Function):
         g_B = torch.zeros(3, 33, **f32)
         g_w0 = torch.zeros(35, **f32)
         g_inv_s = torch.zeros(1, **f32)
+        ray_grad = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        if ray_grad:
+            g_ro, g_rd = torch.empty(R, 3, **f32), torch.empty(R, 3, **f32)
+            Wsdf_xyz = sdf_w.float()[:, :3].contiguous()                         # [32, 3]
         for r0 in range(0, R, _NeusFunction.CHUNK_RAYS):
             r1 = min(R, r0 + _NeusFunction.CHUNK_RAYS)
             n = (r1 - r0) * S
@@ -473,8 +483,13 @@ class _NeusFunction(torch.autograd.Function):
             dc = None if d_color is None else d_color[sl].contiguous()
             dd = None if d_depth is None else d_depth[sl].contiguous()
             dsu = None if d_sdf is None else d_sdf[sl].contiguous()
-            _lib.call("neus_composite_backward", ctypes.byref(p), ro, rd, ds, alpha[sl], rgb[sl], sdf[sl], grad[sl],
-                      z_mid[sl], dc, dd, dsu, d_gerr, fallback, R * S, r0 * S, r1 - r0, S, d_y, d_s, d_g, g_inv_s)
+            if ray_grad:
+                d_tc = torch.empty(n, **f32)
+                _lib.call("neus_composite_backward_ex", ctypes.byref(p), ro, rd, ds, alpha[sl], rgb[sl], sdf[sl], grad[sl],
+                          z_mid[sl], dc, dd, dsu, d_gerr, fallback, R * S, r0 * S, r1 - r0, S, d_y, d_s, d_g, g_inv_s, d_tc)
+            else:
+                _lib.call("neus_composite_backward", ctypes.byref(p), ro, rd, ds, alpha[sl], rgb[sl], sdf[sl], grad[sl],
+                          z_mid[sl], dc, dd, dsu, d_gerr, fallback, R * S, r0 * S, r1 - r0, S, d_y, d_s, d_g, g_inv_s)
             amax = torch.maximum(d_y.abs().max(), d_s.abs().max()).clamp_min(1e-30)
             sc = torch.exp2(torch.floor(torch.log2(1024.0 / amax))).clamp(max=2.0 ** 40).reshape(1).contiguous()   # device scalar
             # ---- colour network, row-wise half (one kernel): H1, H2, dH2, dH1, dX and what hangs off dX per sample ----
@@ -502,6 +517,10 @@ class _NeusFunction(torch.autograd.Function):
             d_enc = torch.mm(d_out, Wsdf_enc, out_dtype=torch.float32)             # [n, 32] f32, still scaled
             _lib.call("neus_grid_backward", ctypes.byref(p), ro, rd, zv, ds, fallback, r0 * S, r1 - r0, S, d_enc, sc,
                       d_gt, g_grid, g_w0)
+            if ray_grad:
+                d_xyz = torch.mm(d_out.float(), Wsdf_xyz)                         # [n, 3] f32, still scaled
+                _lib.call("neus_ray_backward", ctypes.byref(p), ro, rd, zv, ds, fallback, r0 * S, r1 - r0, S, d_enc, d_xyz,
+                          dE, sc, d_gt, d_tc, g_ro[sl], g_rd[sl])
         g_sdf_w[0] += g_w0
         # samples the forward kept out of the network (outside the real-time bound and not among the first 100 of a
         # nothing-in-bound call): rgb = 0, alpha = 0, the kernels return zeros for them, so the GEMMs above see zero rows.
@@ -509,4 +528,6 @@ class _NeusFunction(torch.autograd.Function):
         raw = float(torch.exp(net.variance_network.variance.detach().float() * sf))
         g_var = (g_inv_s[0] * inv_s * sf) if 1e-6 <= raw <= 1e6 else torch.zeros((), **f32)
         g_mlp = torch.cat([g_W1.reshape(-1), g_W2.reshape(-1), g_W3.reshape(-1)])
-        return (None, None, None, None, None, g_grid, g_mlp, g_sdf_w, g_sdf_b, g_B, g_var.reshape(()))
+        g_ro = g_ro.to(ctx.ray_dtypes[0]) if ctx.needs_input_grad[1] else None
+        g_rd = g_rd.to(ctx.ray_dtypes[1]) if ctx.needs_input_grad[2] else None
+        return (None, g_ro, g_rd, None, None, g_grid, g_mlp, g_sdf_w, g_sdf_b, g_B, g_var.reshape(()))

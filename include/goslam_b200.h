@@ -378,6 +378,32 @@ int goslam_neus_grid_backward(const goslam_neus_params* params, const float* ray
                               const float* z_vals, const float* dists, const int* fallback, long long sample0, int R, int S,
                               const float* d_enc, const float* d_enc_scale, const float* d_grad, float* grid_grad,
                               float* d_w0, void* stream);
+/* goslam_neus_composite_backward_ex — goslam_neus_composite_backward with one more optional output: d_true_cos [R,S]
+ *   (NULL = not written) = dL/d true_cos, true_cos = rays_d . normal, through get_alpha alone (0 for samples kept out of
+ *   the network and where the clip stops the gradient).  Every other output is the same, bit for bit.  The ray backward
+ *   takes it for the direction's direct path.
+ *
+ * goslam_neus_ray_backward — per ray: dL/d rays_o [R,3] and dL/d rays_d [R,3] (WRITTEN, not accumulated) of the rays of
+ *   the call, for camera refinement (src/mapping.py:173-194 with mapping.BA).  For a sample at p = o + z d (z = z_vals +
+ *   dists/2 carries no gradient) that went through the network, dL/dp sums four paths: sdf_layer's include_xyz columns
+ *   (d_xyz [R*S,3] = d_out W_sdf[:,:3] w.r.t. the normalised position, zero on clamped axes), the hash-grid encoding to first
+ *   order (d_enc [R*S,32]), the analytic normal to second order (d_grad [R*S,3] = dL/d normal, mixed partials of the
+ *   trilinear interpolant on the f16 table) and the colour embedding sin(p B) (dE [R*S,40] f16, 33 columns used, as
+ *   goslam_neus_mlp_backward writes it).  d_enc, d_xyz and dE are in units of *scale (NULL = 1); d_grad and d_true_cos
+ *   [R*S] (from goslam_neus_composite_backward_ex) are unscaled.  Then dL/d o = sum_s dL/dp_s and dL/d d =
+ *   sum_s z_s dL/dp_s + sum_s d_true_cos_s normal_s.  The per-ray sums run in a fixed order without atomics: the result is
+ *   deterministic and does not depend on how the caller splits the rays.  In bound / fallback / sample0 as for the other
+ *   backward entries.  S <= 128. */
+int goslam_neus_composite_backward_ex(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
+                                      const float* dists, const float* alpha, const float* rgb, const float* sdf,
+                                      const float* grad, const float* z_mid, const float* d_color, const float* d_depth,
+                                      const float* d_sdf, const float* d_gradient_error, const int* fallback,
+                                      long long total_samples, long long sample0, int R, int S, float* d_mlp_out,
+                                      float* d_sdf_out, float* d_grad, float* d_inv_s, float* d_true_cos, void* stream);
+int goslam_neus_ray_backward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
+                             const float* z_vals, const float* dists, const int* fallback, long long sample0, int R, int S,
+                             const float* d_enc, const float* d_xyz, const void* dE, const float* scale, const float* d_grad,
+                             const float* d_true_cos, float* d_rays_o, float* d_rays_d, void* stream);
 /* goslam_neus_mlp_backward — the row-wise half of the colour network's backward (tcnn FullyFusedMLP 80->64->64->16, no
  * biases, ReLU, fp16) in one pass per 32-sample warp tile on mma.sync: recomputes H1, H2 from the kept input rows,
  * dH2 = (dY W3).[H2>0], dH1 = (dH2 W2).[H1>0], dX = dH1 W1, and from dX per sample: dE = dX[:33] cos(p B) (embedding),
