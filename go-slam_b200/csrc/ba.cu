@@ -73,10 +73,10 @@ struct BaDims {
   int N, num, ht, wd, hw, t0, t1, P, n;
 };
 
-size_t ba_layout(const BaDims& d, void* base, size_t cap, BaWs* ws) {
-  GsArena a(base, cap);
+size_t ba_layout(const BaDims& d, void* base, BaWs* ws) {
+  GsArena a(base);
   const int ntiles = gs_cdiv(d.hw, kTP);
-  BaWs w{};
+  BaWs& w = *ws;
   w.slot_of_frame = a.take<int>(d.num);
   w.kx = a.take<int>(d.num);
   w.counts = a.take<int>(8);
@@ -97,8 +97,8 @@ size_t ba_layout(const BaDims& d, void* base, size_t cap, BaWs* ws) {
   w.rhs = a.take<double>(d.n > 0 ? d.n : 1);
   w.dx = a.take<float>((size_t)(d.P > 0 ? d.P : 1) * 6);
   w.ntiles = ntiles;
-  if (ws) *ws = w;
-  return a.off;
+  // the reported size keeps 256 bytes of slack past the carve, which the entry points do not require
+  return base ? a.off : a.off + 256;
 }
 
 // ------------------------------------------------------------------------------------
@@ -1698,7 +1698,8 @@ extern "C" {
 size_t goslam_ba_workspace_bytes(int N, int num, int ht, int wd, int t0, int t1) {
   BaDims d;
   if (!make_dims(N, num, ht, wd, t0, t1, &d)) return 0;
-  return ba_layout(d, nullptr, 0, nullptr) + 256;
+  BaWs ws;
+  return ba_layout(d, nullptr, &ws);
 }
 
 size_t goslam_ba_system_doubles(int t0, int t1) {
@@ -1717,8 +1718,7 @@ int goslam_ba(float* poses, float* disps, const float* intrinsics, const float* 
   if (!motion_only && (eta == nullptr || eta_rows == 0)) return GOSLAM_EINVAL;
   if (d.P == 0 || iterations <= 0) return GOSLAM_OK;
   BaWs ws;
-  const size_t need = ba_layout(d, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ba_layout(d, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
 #ifdef GOSLAM_BA_FORCE_MULTIKERNEL      // build-time A/B switch (tools/), never in the shipped library
   constexpr bool multi_kernel = true;
@@ -1772,8 +1772,7 @@ int goslam_ba_phase1(const float* poses, const float* disps, const float* intrin
   if (!make_dims(N, num, ht, wd, t0, t1, &d)) return GOSLAM_EINVAL;
   if (d.P == 0) return GOSLAM_OK;
   BaWs ws;
-  const size_t need = ba_layout(d, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ba_layout(d, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   int rc = launch_phase1(poses, disps, intrinsics, disps_sens, targets, weights, eta, eta_rows, ii,
                          jj, d, ws, motion_only, true, st);
@@ -1791,8 +1790,7 @@ int goslam_ba_phase2(float* poses, float* disps, const double* system, int N, in
   if (!make_dims(N, num, ht, wd, t0, t1, &d)) return GOSLAM_EINVAL;
   if (d.P == 0) return GOSLAM_OK;
   BaWs ws;
-  const size_t need = ba_layout(d, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ba_layout(d, workspace, &ws)) return GOSLAM_EWORKSPACE;
   SysSrc local{};
   local.p[0] = system; local.n = 1;
   return launch_phase2(poses, disps, local, d, ws, lm, ep, motion_only, owner_lo, owner_hi, dx_out,
@@ -1814,8 +1812,7 @@ int goslam_ba_phase1_peers(const float* poses, const float* intrinsics, const fl
   if (!make_dims(N, num, ht, wd, t0, t1, &d) || !peers_ok(peers)) return GOSLAM_EINVAL;
   if (d.P == 0) return GOSLAM_OK;
   BaWs ws;
-  const size_t need = ba_layout(d, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ba_layout(d, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int W = peers->world, me = peers->rank;
   // (1) every rank has written the inverse-depth rows of the previous iteration into my replica, and has finished
@@ -1848,8 +1845,7 @@ int goslam_ba_phase2_peers(float* poses, int N, int num, int ht, int wd, int t0,
   if (!make_dims(N, num, ht, wd, t0, t1, &d) || !peers_ok(peers)) return GOSLAM_EINVAL;
   if (d.P == 0) return GOSLAM_OK;
   BaWs ws;
-  const size_t need = ba_layout(d, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ba_layout(d, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int W = peers->world, me = peers->rank;
   SysSrc src{};

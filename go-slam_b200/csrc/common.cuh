@@ -97,17 +97,18 @@ __host__ __device__ static inline int gs_cdiv(int a, int b) { return (a + b - 1)
 #define gs_cdiv_dev gs_cdiv
 static inline size_t gs_align(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
-// Bump allocator over a caller-provided workspace.
+// Bump allocator over a caller-provided workspace: take<T>(n) hands out the next 256-byte aligned block of n Ts, and
+// off is the bytes taken so far.  Each workspace has one layout function, xxx_layout(shape..., base, &carve), that
+// takes its blocks in order and returns off: with a null base the arena only counts (every pointer is null), which
+// is how the matching goslam_*_workspace_bytes sizes the workspace; with the caller's base it carves it.
 struct GsArena {
-  char* base; size_t cap; size_t off;
-  GsArena(void* p, size_t c) : base((char*)p), cap(c), off(0) {}
+  char* base; size_t off = 0;
+  explicit GsArena(const void* p) : base((char*)p) {}
   template <typename T> T* take(size_t n) {
-    size_t bytes = gs_align(n * sizeof(T));
-    T* r = (T*)(base + off);
-    off += bytes;
+    T* r = base ? (T*)(base + off) : nullptr;
+    off += gs_align(n * sizeof(T));
     return r;
   }
-  bool ok() const { return off <= cap && (base != nullptr || off == 0); }
 };
 
 // a / b for 0 <= a < 2^51 and b >= 1 through the double reciprocal inv_b = 1.0 / b: the product is within one of the

@@ -630,15 +630,16 @@ struct GruWs {
   __half* z;        // [B,h,w,128]
   __half* rnet;     // [B,h,w,128]
 };
-size_t gru_layout(int B, int h, int w, void* base, size_t cap, GruWs* ws) {
-  GsArena a(base, cap);
-  GruWs g{};
+size_t gru_layout(int B, int h, int w, void* base, GruWs* ws) {
+  if (B <= 0 || h <= 0 || w <= 0) return 256;   // what the size function has always reported for an invalid shape
+  GsArena a(base);
+  GruWs& g = *ws;
   g.glo_sum = a.take<float>((size_t)B * gs_cdiv(h, kPY) * gs_cdiv(w, kPX) * kConsumerWarps * 128);
   g.glo = a.take<float>((size_t)B * 384);
   g.z = a.take<__half>((size_t)B * h * w * 128);
   g.rnet = a.take<__half>((size_t)B * h * w * 128);
-  if (ws) *ws = g;
-  return a.off;
+  // the reported size keeps 256 bytes of slack past the carve, which the entry point does not require
+  return base ? a.off : a.off + 256;
 }
 
 }  // namespace
@@ -720,8 +721,8 @@ int goslam_nchw_to_nhwc_f16_pad(const void* src, void* dst, int B, int C, int Cp
 }
 
 size_t goslam_conv_gru_workspace_bytes(int B, int h, int w) {
-  if (B <= 0 || h <= 0 || w <= 0) return 256;
-  return gru_layout(B, h, w, nullptr, 0, nullptr) + 256;
+  GruWs ws;
+  return gru_layout(B, h, w, nullptr, &ws);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -733,19 +734,21 @@ struct OpWs {
   void* gru;
   size_t gru_bytes;
 };
-static size_t op_layout(int N, int M, int h, int w, void* base, size_t cap, OpWs* out) {
-  GsArena a(base, cap);
-  OpWs o{};
+static size_t op_layout(int N, int M, int h, int w, void* base, OpWs* out) {
+  if (N <= 0 || h <= 0 || w <= 0) return 256;   // what the size function has always reported for an invalid shape
+  GsArena a(base);
+  OpWs& o = *out;
   const size_t px = (size_t)N * h * w, pm = (size_t)(M > 0 ? M : 1) * h * w;
   o.corr256 = a.take<__half>(px * 256); o.c1 = a.take<__half>(px * 128); o.c2 = a.take<__half>(px * 128);
   o.f1 = a.take<__half>(px * 128); o.f2 = a.take<__half>(px * 64);
   o.net = a.take<__half>(px * 128); o.inp = a.take<__half>(px * 128); o.state = a.take<__half>(px * 128);
   o.hid = a.take<__half>(px * 256); o.a1 = a.take<__half>(px * 128);
   o.mean = a.take<__half>(pm * 128); o.a2 = a.take<__half>(pm * 128); o.up = a.take<__half>(pm * 576);
-  o.gru_bytes = goslam_conv_gru_workspace_bytes(N, h, w);
+  GruWs gru;
+  o.gru_bytes = gru_layout(N, h, w, nullptr, &gru);   // the GRU's reported size, slack included
   o.gru = a.take<char>(o.gru_bytes);
-  if (out) *out = o;
-  return a.off;
+  // the reported size keeps 256 bytes of slack past the carve, which the entry point does not require
+  return base ? a.off : a.off + 256;
 }
 
 static int layer(const void* in, int cin, int cin_off, int cin_stride, const void* wgt, const float* bias, int taps, int cout,
@@ -758,8 +761,8 @@ static int layer(const void* in, int cin, int cin_off, int cin_stride, const voi
 }
 
 size_t goslam_update_op_workspace_bytes(int N, int M, int h, int w) {
-  if (N <= 0 || h <= 0 || w <= 0) return 256;
-  return op_layout(N, M, h, w, nullptr, 0, nullptr) + 256;
+  OpWs ws;
+  return op_layout(N, M, h, w, nullptr, &ws);
 }
 
 int goslam_update_op(const goslam_update_weights* W, const void* net, const void* inp, const void* corr,
@@ -769,8 +772,7 @@ int goslam_update_op(const goslam_update_weights* W, const void* net, const void
   if (!W || N < 0 || h <= 0 || w <= 0 || (frame_slot && M <= 0)) return GOSLAM_EINVAL;
   if (N == 0) return GOSLAM_OK;
   OpWs ws;
-  const size_t need = op_layout(N, frame_slot ? M : 0, h, w, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < op_layout(N, frame_slot ? M : 0, h, w, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int hw = h * w;
   int rc;
@@ -831,8 +833,7 @@ int goslam_conv_gru(const goslam_gru_weights* wts, const void* net, const void* 
   if (!wts || B < 0 || h <= 0 || w <= 0) return GOSLAM_EINVAL;
   if (B == 0) return GOSLAM_OK;
   GruWs ws;
-  const size_t need = gru_layout(B, h, w, workspace, workspace_bytes, &ws);
-  if (workspace == nullptr || need > workspace_bytes) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < gru_layout(B, h, w, workspace, &ws)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   ConvMaps m{};
   ConvParams p{};

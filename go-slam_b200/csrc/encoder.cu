@@ -345,7 +345,6 @@ struct Layout {
   __half* act[4];
   float* part[3];
   float* stats[4];
-  size_t bytes;
 };
 
 int tiles_of(int hw) { return gs_cdiv(hw, kBM); }
@@ -355,19 +354,17 @@ bool shape_ok(int B, int H, int W) {
          (long long)B * H * W * 8 < (1LL << 40);
 }
 
-Layout layout(int B, int H, int W, int norm, void* base) {
-  Layout L;
+size_t encoder_layout(int B, int H, int W, int norm, void* base, Layout* L) {
   const size_t act = (size_t)B * (H / 2) * (W / 2) * 32;     // the largest activation (stem / layer1)
   size_t part = 0;
   const int hw[3] = {(H / 2) * (W / 2), (H / 4) * (W / 4), (H / 8) * (W / 8)};
   for (int l = 0; l < 3; ++l) part = part > (size_t)tiles_of(hw[l]) * (32 << l) ? part : (size_t)tiles_of(hw[l]) * (32 << l);
   part *= (size_t)B * 2;
-  GsArena ar(base, ~(size_t)0);
-  for (int i = 0; i < 4; ++i) L.act[i] = ar.take<__half>(act);
-  for (int i = 0; i < 3; ++i) L.part[i] = norm ? ar.take<float>(part) : nullptr;
-  for (int i = 0; i < 4; ++i) L.stats[i] = norm ? ar.take<float>((size_t)B * kMaxC * 2) : nullptr;
-  L.bytes = ar.off;
-  return L;
+  GsArena ar(base);
+  for (int i = 0; i < 4; ++i) L->act[i] = ar.take<__half>(act);
+  for (int i = 0; i < 3; ++i) L->part[i] = norm ? ar.take<float>(part) : nullptr;
+  for (int i = 0; i < 4; ++i) L->stats[i] = norm ? ar.take<float>((size_t)B * kMaxC * 2) : nullptr;
+  return ar.off;
 }
 
 ConvArgs conv_args(const goslam_encoder_conv& cw, const __half* in, int Hi, int Wi, int Cin, int Cout, int ksize,
@@ -407,7 +404,8 @@ bool conv_ok(const goslam_encoder_conv& c) { return c.w != nullptr && c.b != nul
 
 extern "C" size_t goslam_encoder_workspace_bytes(int B, int H, int W, int norm) {
   if (!shape_ok(B, H, W) || (norm != GOSLAM_NORM_NONE && norm != GOSLAM_NORM_INSTANCE)) return 0;
-  return layout(B, H, W, norm, nullptr).bytes;
+  Layout L;
+  return encoder_layout(B, H, W, norm, nullptr, &L);
 }
 
 extern "C" int goslam_basic_encoder(const goslam_encoder_weights* wt, int norm, int out_dim, const void* image,
@@ -423,8 +421,8 @@ extern "C" int goslam_basic_encoder(const goslam_encoder_weights* wt, int norm, 
     if (!conv_ok(wt->block[i][0]) || !conv_ok(wt->block[i][1])) return GOSLAM_EINVAL;
     if ((i == 2 || i == 4) && !conv_ok(wt->block[i][2])) return GOSLAM_EINVAL;
   }
-  const Layout L = layout(B, H, W, norm, workspace);
-  if (workspace == nullptr || workspace_bytes < L.bytes) return GOSLAM_EWORKSPACE;
+  Layout L;
+  if (!workspace || workspace_bytes < encoder_layout(B, H, W, norm, workspace, &L)) return GOSLAM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   const bool inst = norm == GOSLAM_NORM_INSTANCE;
 

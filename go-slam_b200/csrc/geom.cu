@@ -387,20 +387,16 @@ struct MvState {
   int mn2[3], mx2[3];                 // second bound (final points)
   unsigned long long n1, n_ext, n_fin;
 };
-constexpr size_t kMvStateBytes = 256;
-static_assert(sizeof(MvState) <= kMvStateBytes, "MvState");
+struct MvWork { MvState* st; float* mean; unsigned char* mask1; unsigned char* fin; };   // mean [T], masks [T, hw]
 
-__host__ __device__ constexpr size_t mv_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-struct MvLayout {
-  size_t mean, mask1, fin, total;
-  __host__ __device__ MvLayout(int T, size_t hw) {
-    mean = kMvStateBytes;
-    mask1 = mean + mv_align((size_t)T * sizeof(float));
-    fin = mask1 + mv_align((size_t)T * hw);
-    total = fin + mv_align((size_t)T * hw);
-  }
-};
+size_t mv_layout(int T, size_t hw, const void* base, MvWork* w) {
+  GsArena ar(base);
+  w->st = ar.take<MvState>(1);
+  w->mean = ar.take<float>(T);
+  w->mask1 = ar.take<unsigned char>((size_t)T * hw);
+  w->fin = ar.take<unsigned char>((size_t)T * hw);
+  return ar.off;
+}
 
 // float -> int with the same order (-0 sorts below +0); the map is its own inverse
 __device__ __forceinline__ int mv_ord(float f) {
@@ -666,17 +662,6 @@ mv_commit_kernel(const float* __restrict__ poses, const float* __restrict__ disp
 // frame's mean, i.e. mask1 of the multiview filter with visible_num = 3.  mv_mean_kernel + mv_vote_kernel count them
 // (MvState::n1); the emit is an ordered CUB select of iproj_point over mask1, [b, h, w] row-major, widened to f64.
 // ---------------------------------------------------------------------------------
-struct MapLayout {
-  size_t mean, mask1, nsel, tmp, total;
-  MapLayout(int T, size_t hw, size_t tmp_bytes) {
-    mean = kMvStateBytes;
-    mask1 = mean + mv_align((size_t)T * sizeof(float));
-    nsel = mask1 + mv_align((size_t)T * hw);
-    tmp = nsel + 256;
-    total = tmp + mv_align(tmp_bytes);
-  }
-};
-
 struct MapPoint3 {
   double x, y, z;
 };
@@ -696,12 +681,32 @@ struct MapPointOp {
 
 using MapIter = cub::TransformInputIterator<MapPoint3, MapPointOp, cub::CountingInputIterator<long long>>;
 
-// a failed size query is reported by the select call itself (GS_CUDA)
-size_t map_select_tmp(long long n) {
+struct MapWork { MvState* st; float* mean; unsigned char* mask1; long long* nsel; void* tmp; size_t tmp_bytes; };
+
+size_t map_layout(int T, size_t hw, void* base, MapWork* w) {
+  GsArena ar(base);
+  w->st = ar.take<MvState>(1);
+  w->mean = ar.take<float>(T);
+  w->mask1 = ar.take<unsigned char>((size_t)T * hw);
+  w->nsel = ar.take<long long>(1);
+  // a failed size query is reported by the select call itself (GS_CUDA)
   size_t t = 0;
   cub::DeviceSelect::Flagged(nullptr, t, MapIter(cub::CountingInputIterator<long long>(0), MapPointOp{}),
-                             (const unsigned char*)nullptr, (MapPoint3*)nullptr, (long long*)nullptr, n);
-  return std::max<size_t>(t, 1);
+                             (const unsigned char*)nullptr, (MapPoint3*)nullptr, (long long*)nullptr,
+                             (long long)(T * hw));
+  w->tmp_bytes = std::max<size_t>(t, 1);
+  w->tmp = ar.take<char>(w->tmp_bytes);
+  return ar.off;
+}
+
+struct GridWork { float* poses; size_t pose_bytes; };   // the poses [max(r1, c1), 7] the grid kernel reads
+
+size_t grid_layout(int r1, int c1, void* base, GridWork* w) {
+  const size_t n = (size_t)7 * std::max(r1, c1);
+  GsArena ar(base);
+  w->poses = ar.take<float>(n);
+  w->pose_bytes = n * sizeof(float);
+  return ar.off;
 }
 
 constexpr float kMapThresh = 0.01f;          // src/mesher.py:252-253
@@ -735,7 +740,8 @@ int goslam_frame_distance_bidir(const float* poses, const float* disps, const fl
 
 size_t goslam_frame_distance_grid_workspace_bytes(int r0, int r1, int c0, int c1) {
   if (r0 < 0 || c0 < 0 || r1 <= r0 || c1 <= c0) return 0;
-  return gs_align((size_t)7 * std::max(r1, c1) * sizeof(float));
+  GridWork w;
+  return grid_layout(r1, c1, nullptr, &w);
 }
 
 int goslam_frame_distance_grid(const float* poses, const float* disps, const float* intrinsics, int r0, int r1, int c0,
@@ -745,13 +751,12 @@ int goslam_frame_distance_grid(const float* poses, const float* disps, const flo
   if ((long long)(r1 - r0) * (c1 - c0) > (long long)INT_MAX) return GOSLAM_EINVAL;
   if (r1 == r0 || c1 == c0) return GOSLAM_OK;
   if (poses == nullptr || disps == nullptr || intrinsics == nullptr || dist == nullptr) return GOSLAM_EINVAL;
-  const size_t need = goslam_frame_distance_grid_workspace_bytes(r0, r1, c0, c1);
-  if (workspace == nullptr || workspace_bytes < need) return GOSLAM_EWORKSPACE;
+  GridWork w;
+  if (!workspace || workspace_bytes < grid_layout(r1, c1, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   // the poses of frames [0, max(r1, c1)) as they are when this call reaches the stream: other processes write the
   // shared pose buffer while a backend pass runs, and every pair must see one consistent set
-  float* snap = static_cast<float*>(workspace);
-  GS_CUDA(cudaMemcpyAsync(snap, poses, (size_t)7 * std::max(r1, c1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  GS_CUDA(cudaMemcpyAsync(w.poses, poses, w.pose_bytes, cudaMemcpyDeviceToDevice, s));
   // band size S(r1) on the host (same closed form as GridBand::start)
   const long long W = c1 - c0, a = (long long)k + 1 - c0;
   auto tri = [W](long long m) -> long long {
@@ -763,7 +768,7 @@ int goslam_frame_distance_grid(const float* poses, const float* disps, const flo
   const long long n_all = (long long)(r1 - r0) * W;
   const int fill_blocks = n_band == n_all ? 0 : (int)std::min<long long>((n_all + 4 * kThreads - 1) / (4 * kThreads), 1024);
   const GridBand band{r0, r1, c0, c1, k};
-  frame_distance_grid_kernel<<<(unsigned)(n_band + fill_blocks), kThreads, 0, s>>>(snap, disps, intrinsics, band, n_band,
+  frame_distance_grid_kernel<<<(unsigned)(n_band + fill_blocks), kThreads, 0, s>>>(w.poses, disps, intrinsics, band, n_band,
                                                                                   fill_blocks, dist, ht, wd, beta);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
@@ -830,7 +835,8 @@ int goslam_depth_filter(const float* poses, const float* disps, const float* int
 
 size_t goslam_mvfilter_workspace_bytes(int T, int ht, int wd) {
   if (T < 0 || T > 65535 || ht <= 0 || wd <= 0) return 0;
-  return MvLayout(T, (size_t)ht * wd).total;
+  MvWork w;
+  return mv_layout(T, (size_t)ht * wd, nullptr, &w);
 }
 
 int goslam_mvfilter_compute(const float* poses, const float* poses_world, const float* disps,
@@ -841,22 +847,17 @@ int goslam_mvfilter_compute(const float* poses, const float* poses_world, const 
   const int radius = kernel_size == 0 ? -1 : (kernel_size < 2 ? 0 : kernel_size / 2);
   if (radius > kMvMaxRadius) return GOSLAM_EINVAL;
   const int hw = ht * wd;
-  const MvLayout L(T, (size_t)hw);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
-  char* ws = static_cast<char*>(workspace);
-  MvState* st = reinterpret_cast<MvState*>(ws);
-  float* mean = reinterpret_cast<float*>(ws + L.mean);
-  unsigned char* mask1 = reinterpret_cast<unsigned char*>(ws + L.mask1);
-  unsigned char* fin = reinterpret_cast<unsigned char*>(ws + L.fin);
+  MvWork w;
+  if (!workspace || workspace_bytes < mv_layout(T, (size_t)hw, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
-  mv_mean_kernel<<<T > 0 ? T : 1, kMvMeanThreads, 0, s>>>(disps, mean, st, T, hw);
+  mv_mean_kernel<<<T > 0 ? T : 1, kMvMeanThreads, 0, s>>>(disps, w.mean, w.st, T, hw);
   GS_CHECK_LAUNCH();
   if (T == 0) return GOSLAM_OK;
   const dim3 grid(gs_cdiv(hw, kMvTile), T);
-  mv_vote_kernel<<<grid, kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, mean, filter_thresh,
-                                           (float)visible_num, mask1, st, T, ht, wd);
+  mv_vote_kernel<<<grid, kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, w.mean, filter_thresh,
+                                           (float)visible_num, w.mask1, w.st, T, ht, wd);
   GS_CHECK_LAUNCH();
-  mv_extend_kernel<<<grid, kThreads, 0, s>>>(poses_world, disps, intrinsic, mask1, fin, st, radius, ht, wd);
+  mv_extend_kernel<<<grid, kThreads, 0, s>>>(poses_world, disps, intrinsic, w.mask1, w.fin, w.st, radius, ht, wd);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }
@@ -866,23 +867,22 @@ int goslam_mvfilter_commit(const float* poses, const float* disps, const void* w
                            float* update_priority, int* filtered_id, float* bound, int64_t* status, void* stream) {
   if (T < 0 || T > 65535 || ht <= 0 || wd <= 0) return GOSLAM_EINVAL;
   if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
-  const MvLayout L(T, (size_t)ht * wd);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
-  const char* ws = static_cast<const char*>(workspace);
+  MvWork w;
+  if (!workspace || workspace_bytes < mv_layout(T, (size_t)ht * wd, workspace, &w)) return GOSLAM_EWORKSPACE;
   const size_t n = (size_t)T * ht * wd;
   const size_t want = std::max<size_t>((n / 4 + kThreads - 1) / kThreads, (size_t)gs_cdiv(T, kThreads));
   const int blocks = (int)std::min<size_t>(std::max<size_t>(want, 1), 4096);
   mv_commit_kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
-      poses, disps, reinterpret_cast<const unsigned char*>(ws + L.fin), reinterpret_cast<const MvState*>(ws), T, n,
-      poses_filtered, disps_filtered, mask_filtered, update_priority, filtered_id, bound, status);
+      poses, disps, w.fin, w.st, T, n, poses_filtered, disps_filtered, mask_filtered, update_priority, filtered_id,
+      bound, status);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }
 
 size_t goslam_mapping_points_workspace_bytes(int T, int ht, int wd) {
   if (T < 1 || T > 65535 || ht <= 0 || wd <= 0 || (size_t)ht * wd > (size_t)INT_MAX / 2) return 0;
-  const size_t hw = (size_t)ht * wd;
-  return MapLayout(T, hw, map_select_tmp((long long)T * (long long)hw)).total;
+  MapWork w;
+  return map_layout(T, (size_t)ht * wd, nullptr, &w);
 }
 
 int goslam_mapping_points_count(const float* poses, const float* poses_world, const float* disps,
@@ -891,19 +891,15 @@ int goslam_mapping_points_count(const float* poses, const float* poses_world, co
   if (T < 1 || T > 65535 || ht <= 0 || wd <= 0 || count == nullptr) return GOSLAM_EINVAL;
   if ((size_t)ht * wd > (size_t)INT_MAX / 2) return GOSLAM_EINVAL;
   const int hw = ht * wd;
-  const MapLayout L(T, (size_t)hw, map_select_tmp((long long)T * hw));
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
-  char* ws = static_cast<char*>(workspace);
-  MvState* st = reinterpret_cast<MvState*>(ws);
-  float* mean = reinterpret_cast<float*>(ws + L.mean);
-  unsigned char* mask1 = reinterpret_cast<unsigned char*>(ws + L.mask1);
+  MapWork w;
+  if (!workspace || workspace_bytes < map_layout(T, (size_t)hw, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
-  mv_mean_kernel<<<T, kMvMeanThreads, 0, s>>>(disps, mean, st, T, hw);
+  mv_mean_kernel<<<T, kMvMeanThreads, 0, s>>>(disps, w.mean, w.st, T, hw);
   GS_CHECK_LAUNCH();
-  mv_vote_kernel<<<dim3(gs_cdiv(hw, kMvTile), T), kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, mean,
-                                                                     kMapThresh, kMapVisible, mask1, st, T, ht, wd);
+  mv_vote_kernel<<<dim3(gs_cdiv(hw, kMvTile), T), kThreads, 0, s>>>(poses, poses_world, disps, intrinsic, w.mean,
+                                                                     kMapThresh, kMapVisible, w.mask1, w.st, T, ht, wd);
   GS_CHECK_LAUNCH();
-  GS_CUDA(cudaMemcpyAsync(count, &st->n1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
+  GS_CUDA(cudaMemcpyAsync(count, &w.st->n1, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
   return GOSLAM_OK;
 }
 
@@ -916,16 +912,13 @@ int goslam_mapping_points_emit(const float* poses_world, const float* disps, con
   const int hw = ht * wd;
   const long long n = (long long)T * hw;
   if (n_points > n) return GOSLAM_EINVAL;
-  const size_t tmp_bytes = map_select_tmp(n);
-  const MapLayout L(T, (size_t)hw, tmp_bytes);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  MapWork w;
+  if (!workspace || workspace_bytes < map_layout(T, (size_t)hw, workspace, &w)) return GOSLAM_EWORKSPACE;
   if (n_points == 0) return GOSLAM_OK;
-  char* ws = static_cast<char*>(workspace);
-  size_t tb = tmp_bytes;
+  size_t tb = w.tmp_bytes;
   const MapIter it(cub::CountingInputIterator<long long>(0), MapPointOp{poses_world, disps, intrinsic, hw, wd});
-  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, it, reinterpret_cast<const unsigned char*>(ws + L.mask1),
-                                     reinterpret_cast<MapPoint3*>(points), reinterpret_cast<long long*>(ws + L.nsel), n,
-                                     (cudaStream_t)stream));
+  GS_CUDA(cub::DeviceSelect::Flagged(w.tmp, tb, it, (const unsigned char*)w.mask1, reinterpret_cast<MapPoint3*>(points),
+                                     w.nsel, n, (cudaStream_t)stream));
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

@@ -163,16 +163,27 @@ __global__ void __launch_bounds__(kGT) proximity_kernel(const ProxArgs a) {
   }
 }
 
+// the distance matrix of the window, its candidate keys (a power of two of them, for the sort) and two counters
+size_t prox_layout(int t0, int t1, int t, void* base, ProxArgs* a) {
+  GsArena ar(base);
+  const size_t n = (size_t)(t - t0) * (t - t1);
+  size_t p2 = 1;
+  while (p2 < n) p2 <<= 1;
+  a->dm = ar.take<float>(n);
+  a->keys = ar.take<unsigned long long>(p2);
+  a->counters = ar.take<int>(2);
+  a->nkeys_cap = (int)p2;
+  return ar.off;
+}
+
 }  // namespace
 
 extern "C" {
 
 size_t goslam_proximity_workspace_bytes(int t0, int t1, int t) {
   if (t <= t0 || t <= t1 || t0 < 0 || t1 < 0) return 0;
-  const size_t n = (size_t)(t - t0) * (t - t1);
-  size_t p2 = 1;
-  while (p2 < n) p2 <<= 1;
-  return gs_align(n * sizeof(float)) + gs_align(p2 * sizeof(unsigned long long)) + 256;
+  ProxArgs a;
+  return prox_layout(t0, t1, t, nullptr, &a);
 }
 
 int goslam_proximity_edges(const float* dist, int t0, int t1, int t, int rad, int nms, float thresh,
@@ -188,20 +199,12 @@ int goslam_proximity_edges(const float* dist, int t0, int t1, int t, int rad, in
   const int jmin = (t0 - rad > jfloor ? t0 - rad : jfloor);
   if (rad > 0 && jmin - t1 < -jlen) return GOSLAM_EINVAL;
   if (stereo && t0 - t1 < -jlen) return GOSLAM_EINVAL;
-  const size_t need = goslam_proximity_workspace_bytes(t0, t1, t);
-  if (workspace == nullptr || workspace_bytes < need) return GOSLAM_EWORKSPACE;
-  const size_t n = (size_t)ilen * jlen;
-  size_t p2 = 1;
-  while (p2 < n) p2 <<= 1;
   ProxArgs a{};
+  if (!workspace || workspace_bytes < prox_layout(t0, t1, t, workspace, &a)) return GOSLAM_EWORKSPACE;
   a.dist = dist; a.ii_old = ii_old; a.jj_old = jj_old; a.n_old = n_old;
   a.t0 = t0; a.t1 = t1; a.t = t; a.rad = rad; a.nms = nms; a.max_factors = max_factors; a.stereo = stereo ? 1 : 0;
   a.thresh = thresh; a.dmax = dmax; a.jfloor = jfloor; a.loop = loop ? 1 : 0;
-  char* w = reinterpret_cast<char*>(workspace);
-  a.dm = reinterpret_cast<float*>(w);
-  a.keys = reinterpret_cast<unsigned long long*>(w + gs_align(n * sizeof(float)));
-  a.counters = reinterpret_cast<int*>(w + gs_align(n * sizeof(float)) + gs_align(p2 * sizeof(unsigned long long)));
-  a.es_i = es_i; a.es_j = es_j; a.cap = cap; a.nkeys_cap = (int)p2;
+  a.es_i = es_i; a.es_j = es_j; a.cap = cap;
   proximity_kernel<<<1, kGT, 0, (cudaStream_t)stream>>>(a);
   GS_CHECK_LAUNCH();
   if (num_edges)

@@ -29,15 +29,14 @@ struct SnapWork {
 
 int num_tiles(long long hw) { return (int)((hw + kTile - 1) / kTile); }
 
-size_t snap_layout(int F, long long hw, void* base, SnapWork* w) {
+size_t snap_layout(int F, long long hw, const void* base, SnapWork* w) {
   const size_t ft = (size_t)F * num_tiles(hw), fp = (size_t)F * hw;
-  size_t off = 0;
-  char* b = (char*)base;
-  w->tile_count = (int*)(b + off); off += gs_align(ft * sizeof(int));
-  w->tile_off = (int*)(b + off);   off += gs_align(ft * sizeof(int));
-  w->pix = (int*)(b + off);        off += gs_align(fp * sizeof(int));
-  w->rec = (float4*)(b + off);     off += gs_align(fp * sizeof(float4));
-  return off;
+  GsArena ar(base);
+  w->tile_count = ar.take<int>(ft);
+  w->tile_off = ar.take<int>(ft);
+  w->pix = ar.take<int>(fp);
+  w->rec = ar.take<float4>(fp);
+  return ar.off;
 }
 
 bool snap_shape_ok(int F, int H, int W) {
@@ -237,10 +236,9 @@ int goslam_mapping_snapshot(const float* images, const float* mask, const float*
   if (!snap_shape_ok(F, H, W) || buffer <= 0) return GOSLAM_EINVAL;
   if (F == 0) return GOSLAM_OK;
   if (!images || !mask || !disps || !update_priority || !frames || !occurrences || !counts) return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
   const long long hw = (long long)H * W;
   SnapWork w;
-  if (workspace_bytes < snap_layout(F, hw, workspace, &w)) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < snap_layout(F, hw, workspace, &w)) return GOSLAM_EWORKSPACE;
   const int T = num_tiles(hw);
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(T, F);
@@ -272,9 +270,8 @@ int goslam_mapping_rays(const void* workspace, size_t workspace_bytes, int F, in
   if (R > max_rays || D > n_draws || R > INT32_MAX) return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
   if (!c2w || !rays_o || !rays_d || !depth || !color || (D > 0 && !draws)) return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
   SnapWork w;
-  if (workspace_bytes < snap_layout(F, hw, const_cast<void*>(workspace), &w)) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < snap_layout(F, hw, workspace, &w)) return GOSLAM_EWORKSPACE;
   const Intr in = make_intr(fx, fy, cx, cy);
   cudaStream_t st = (cudaStream_t)stream;
   long long out = 0, rnd = 0;

@@ -158,8 +158,8 @@ struct McWork {
 };
 
 // one layout for the count and the emit pass; returns the bytes it needs
-size_t mc_layout(const Lattice& g, void* base, McWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+size_t mc_layout(const Lattice& g, const void* base, McWork* w) {
+  GsArena ar(base);
   w->nwords = 3 * cdiv64(g.npts, 32);
   w->ncb = cdiv64(g.ncell, kCellsPerBlock);
   w->words = ar.take<unsigned>(w->nwords);
@@ -311,8 +311,8 @@ struct CullWork {
   u64* tiles;
 };
 
-size_t cull_layout(long long nv, long long nf, void* base, CullWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+size_t cull_layout(long long nv, long long nf, const void* base, CullWork* w) {
+  GsArena ar(base);
   w->vref = ar.take<unsigned>(nv > 0 ? nv : 1);
   w->voff = ar.take<u64>(nv > 0 ? nv : 1);
   w->fkeep = ar.take<unsigned>(nf > 0 ? nf : 1);
@@ -433,7 +433,7 @@ int goslam_mc_emit(const float* u, int nx, int ny, int nz, double iso, const flo
     return GOSLAM_EINVAL;
   const Lattice g = make_lattice(u, nx, ny, nz, iso);
   McWork w;
-  if (!workspace || workspace_bytes < mc_layout(g, const_cast<void*>(workspace), &w)) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < mc_layout(g, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   WorldMap m;
   const int n[3] = {nx, ny, nz};
@@ -486,8 +486,7 @@ int goslam_mesh_cull_emit(const double* verts, int64_t n_verts, const int64_t* f
       (n_faces > 0 && !faces) || (max_out_verts > 0 && !out_verts) || (max_out_faces > 0 && !out_faces))
     return GOSLAM_EINVAL;
   CullWork w;
-  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, const_cast<void*>(workspace), &w))
-    return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   if (n_verts > 0 && max_out_verts > 0) {
     cull_vertex_emit_kernel<<<blocks_for(n_verts, 256), 256, 0, st>>>(verts, n_verts, w.vref, w.voff, out_verts, max_out_verts);
@@ -523,8 +522,7 @@ int goslam_mesh_cull_vertex_ids(int64_t n_verts, int64_t n_faces, const void* wo
                                 int64_t max_ids, void* stream) {
   if (n_verts < 0 || n_faces < 0 || max_ids < 0 || (max_ids > 0 && !ids)) return GOSLAM_EINVAL;
   CullWork w;
-  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, const_cast<void*>(workspace), &w))
-    return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < cull_layout(n_verts, n_faces, workspace, &w)) return GOSLAM_EWORKSPACE;
   if (n_verts > 0 && max_ids > 0) {
     cull_vertex_ids_kernel<<<blocks_for(n_verts, 256), 256, 0, (cudaStream_t)stream>>>(n_verts, w.vref, w.voff,
                                                                                        (long long*)ids, max_ids);

@@ -84,7 +84,7 @@ int sample_cub_bytes(long long nf, size_t* b) {
 struct SampleWork { double* area; double* cum; void* cub_tmp; size_t cub_bytes; };
 
 size_t sample_layout(long long nf, size_t cub_bytes, void* base, SampleWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+  GsArena ar(base);
   w->area = ar.take<double>(nf);
   w->cum = ar.take<double>(nf);
   w->cub_tmp = ar.take<unsigned char>(cub_bytes);
@@ -128,7 +128,7 @@ int nn_cub_bytes(long long n, size_t* b) {
 }
 
 size_t nn_layout(long long n, size_t cub_bytes, const void* base, NnIndex* x) {
-  GsArena ar(const_cast<void*>(base), ~size_t(0) >> 1);
+  GsArena ar(base);
   x->params = ar.take<NnParams>(1);
   x->cell_start = ar.take<unsigned>(max_cells(n) + 1);
   for (int i = 0; i < 2; ++i) {
@@ -368,7 +368,7 @@ struct IcpState {
 struct IcpWork { IcpState* state; double* work; int* corr; double* part; };
 
 size_t icp_layout(long long n, void* base, IcpWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+  GsArena ar(base);
   w->state = ar.take<IcpState>(1);
   w->work = ar.take<double>(3 * n);
   w->corr = ar.take<int>(n);
@@ -565,7 +565,7 @@ int goslam_mesh_sample_surface(const double* verts, int64_t n_verts, const int64
   if (n_verts < 1 || n_faces < 1 || n_faces > kMaxFaces || count < 0 || !verts || !faces ||
       (count > 0 && (!uniforms || !samples)))
     return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
+  if (!workspace) return GOSLAM_EWORKSPACE;     // refused before the CUB size query, which needs a device
   size_t cb = 0;
   if (const int rc = sample_cub_bytes(n_faces, &cb)) return rc;
   SampleWork w;
@@ -594,7 +594,7 @@ int goslam_nn_index_build(const double* points, int64_t n_points, double min_cel
                           void* stream) {
   if (n_points < 1 || n_points > kMaxPoints || !points || !(min_cell >= 0.0) || !(min_cell < INFINITY))
     return GOSLAM_EINVAL;
-  if (!index) return GOSLAM_EWORKSPACE;
+  if (!index) return GOSLAM_EWORKSPACE;     // refused before the CUB size query, which needs a device
   size_t cb = 0;
   if (const int rc = nn_cub_bytes(n_points, &cb)) return rc;
   NnIndex x;
@@ -623,7 +623,7 @@ int goslam_nn_query(const void* index, size_t index_bytes, int64_t n_points, con
   if (n_points < 1 || n_points > kMaxPoints || n_query < 0 || (n_query > 0 && (!query || (!dist && !idx))) ||
       !(max_dist > 0.0))
     return GOSLAM_EINVAL;
-  if (!index) return GOSLAM_EWORKSPACE;
+  if (!index) return GOSLAM_EWORKSPACE;     // refused before the CUB size query, which needs a device
   size_t cb = 0;
   if (const int rc = nn_cub_bytes(n_points, &cb)) return rc;
   NnIndex x;
@@ -658,7 +658,7 @@ int goslam_icp_point_to_point(const double* source, int64_t n_source, const void
       !(threshold > 0.0) || !(threshold < INFINITY) || max_iteration < 0 || relative_fitness != relative_fitness ||
       relative_rmse != relative_rmse)
     return GOSLAM_EINVAL;
-  if (!index || !workspace) return GOSLAM_EWORKSPACE;
+  if (!index || !workspace) return GOSLAM_EWORKSPACE;     // refused before the CUB size query, which needs a device
   size_t cb = 0;
   if (const int rc = nn_cub_bytes(n_target, &cb)) return rc;
   NnIndex x;

@@ -277,7 +277,7 @@ int comp_cub_bytes(long long nf, size_t* bytes) {
 }
 
 size_t comp_layout(long long nf, size_t cub_bytes, void* base, CompWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+  GsArena ar(base);
   const long long ne = 3 * nf > 0 ? 3 * nf : 1, n = nf > 0 ? nf : 1;
   for (int i = 0; i < 2; ++i) {
     w->keys[i] = ar.take<u64>(ne);
@@ -451,7 +451,7 @@ int goslam_mesh_components_count(const double* verts, int64_t n_verts, const int
                                  size_t workspace_bytes, int64_t* counts, void* stream) {
   if (n_verts < 0 || n_faces < 0 || n_faces > kMaxCompFaces || (n_verts > 0 && !verts) || (n_faces > 0 && !faces) || !counts)
     return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
+  if (!workspace) return GOSLAM_EWORKSPACE;     // refused before the empty-input return and the CUB size query
   cudaStream_t st = (cudaStream_t)stream;
   if (n_faces == 0) {
     GS_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t), st));
@@ -498,7 +498,7 @@ int goslam_mesh_components_keep(int64_t n_faces, int64_t n_components, double th
   if (n_faces < 0 || n_faces > kMaxCompFaces || n_components < 0 || n_components > n_faces || (n_faces > 0 && !face_keep) ||
       (n_faces > 0 && n_components == 0) || threshold != threshold)
     return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
+  if (!workspace) return GOSLAM_EWORKSPACE;     // refused before the empty-input return and the CUB size query
   if (n_faces == 0) return GOSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
   size_t cb = 0;

@@ -1505,6 +1505,15 @@ int neus_device_init(int) {
   return GOSLAM_OK;
 }
 
+// the forward's per-block partials and its fallback flag; the same for every R and S
+size_t neus_layout(void* base, NeusArgs* a) {
+  GsArena ar(base);
+  a->blk_gerr = ar.take<float>(kNumSms * 4);
+  a->blk_count = ar.take<unsigned>(kNumSms * 4);
+  a->flag = ar.take<int>(1);
+  return ar.off;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1523,7 +1532,8 @@ int64_t goslam_hashgrid_layout(int64_t* offsets, int* resolutions, float* scales
 
 size_t goslam_neus_workspace_bytes(int R, int S) {
   (void)R; (void)S;
-  return gs_align(kNumSms * 4 * sizeof(float)) + gs_align(kNumSms * 4 * sizeof(unsigned)) + 256;
+  NeusArgs a;
+  return neus_layout(nullptr, &a);
 }
 
 int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, const float* rays_d,
@@ -1532,19 +1542,14 @@ int goslam_neus_forward(const goslam_neus_params* params, const float* rays_o, c
                         void* stream) {
   if (!params || !out || R < 0 || S <= 0 || S > kMaxGroup) return GOSLAM_EINVAL;
   if (R == 0) return GOSLAM_OK;
-  if (workspace == nullptr || workspace_bytes < goslam_neus_workspace_bytes(R, S))
-    return GOSLAM_EWORKSPACE;
+  NeusArgs a{};
+  if (!workspace || workspace_bytes < neus_layout(workspace, &a)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   { const int rc = gs_device_setup<neus_device_init>(); if (rc != GOSLAM_OK) return rc; }
-  GsArena ar(workspace, workspace_bytes);
-  NeusArgs a{};
   a.p = *params; a.o = *out;
   a.rays_o = rays_o; a.rays_d = rays_d; a.z_vals = z_vals; a.dists = dists;
   a.R = R; a.S = S;
   const int grid = kNumSms;
-  a.blk_gerr = ar.take<float>(kNumSms * 4);
-  a.blk_count = ar.take<unsigned>(kNumSms * 4);
-  a.flag = reinterpret_cast<int*>(ar.take<int>(1));
   if (out->fallback) a.flag = out->fallback;      // the backward reads the decision from there
   // rays per warp work item: make G*S a multiple of 32 when that fits the slab, else pad
   int G = 32 / std::__gcd(S, 32);

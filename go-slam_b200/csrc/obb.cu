@@ -179,32 +179,39 @@ struct Dirs {
 
 int facet_cap(long long n) { return (int)std::min<long long>(4 * n + 64, kMaxFacets); }
 
-struct ObbLayout {
-  size_t state, win, main, keep, vflag, surv, apt, aown, adist, out, tmp, tmp_bytes, total;
-  // what hull_mem carves: per facet slot 1 / |normal|, 12 ints (fv, fn, fstamp, freestk, visl, newl, nstart, nend)
-  // and the alive byte; then 256 bytes of alignment slack
-  static size_t hull_bytes(int cap) { return gs_align((size_t)cap * (sizeof(double) + 12 * sizeof(int) + 1) + 256); }
-  explicit ObbLayout(long long n) {
-    size_t o = 0;
-    auto take = [&](size_t b) { const size_t r = o; o += gs_align(b); return r; };
-    state = take(sizeof(ObbState));
-    win = take(hull_bytes(kWinCap) + (size_t)kDirs * (2 * sizeof(int) + sizeof(float)));
-    main = take(hull_bytes(facet_cap(n)));
-    keep = take((size_t)n);
-    vflag = take((size_t)n);
-    surv = take((size_t)n * sizeof(int));
-    apt = take((size_t)n * sizeof(int));
-    aown = take((size_t)n * sizeof(int));
-    adist = take((size_t)n * sizeof(float));
-    out = take((size_t)n * sizeof(int));
-    size_t t1 = 0;   // a failed size query is reported by the select calls themselves (GS_CUDA)
-    cub::DeviceSelect::Flagged(nullptr, t1, cub::CountingInputIterator<int>(0), (const unsigned char*)nullptr,
-                               (int*)nullptr, (long long*)nullptr, (int)std::max<long long>(n, 1));
-    tmp_bytes = std::max<size_t>(t1, 1);
-    tmp = take(tmp_bytes);
-    total = o;
-  }
+// what hull_mem carves: per facet slot 1 / |normal|, 12 ints (fv, fn, fstamp, freestk, visl, newl, nstart, nend)
+// and the alive byte; then 256 bytes of alignment slack
+size_t hull_bytes(int cap) { return gs_align((size_t)cap * (sizeof(double) + 12 * sizeof(int) + 1) + 256); }
+
+struct ObbWork {
+  ObbState* state;
+  char *win, *main;                 // hull_mem's regions: the winners' hull with its active list, the survivors' hull
+  unsigned char *keep, *vflag;      // [n]
+  int *surv, *apt, *aown, *out;     // [n]; apt, aown, adist: the survivors' hull's active list; out: its vertices
+  float* adist;                     // [n]
+  char* tmp;                        // CUB's select storage
+  size_t tmp_bytes;
 };
+
+size_t obb_layout(long long n, const void* base, ObbWork* w) {
+  GsArena ar(base);
+  w->state = ar.take<ObbState>(1);
+  w->win = ar.take<char>(hull_bytes(kWinCap) + (size_t)kDirs * (2 * sizeof(int) + sizeof(float)));
+  w->main = ar.take<char>(hull_bytes(facet_cap(n)));
+  w->keep = ar.take<unsigned char>(n);
+  w->vflag = ar.take<unsigned char>(n);
+  w->surv = ar.take<int>(n);
+  w->apt = ar.take<int>(n);
+  w->aown = ar.take<int>(n);
+  w->adist = ar.take<float>(n);
+  w->out = ar.take<int>(n);
+  size_t t1 = 0;   // a failed size query is reported by the select calls themselves (GS_CUDA)
+  cub::DeviceSelect::Flagged(nullptr, t1, cub::CountingInputIterator<int>(0), (const unsigned char*)nullptr,
+                             (int*)nullptr, (long long*)nullptr, (int)std::max<long long>(n, 1));
+  w->tmp_bytes = std::max<size_t>(t1, 1);
+  w->tmp = ar.take<char>(w->tmp_bytes);
+  return ar.off;
+}
 
 HullMem hull_mem(char* base, int cap, int act_cap, HullState* st, int* apt, int* aown, float* adist) {
   HullMem h;
@@ -940,43 +947,36 @@ extern "C" {
 
 size_t goslam_hull_workspace_bytes(int64_t n) {
   if (n < 1 || n > kMaxPoints) return 0;
-  return ObbLayout(n).total;
+  ObbWork w;
+  return obb_layout(n, nullptr, &w);
 }
 
 int goslam_hull_vertices(const double* points, int64_t n, void* workspace, size_t workspace_bytes, int64_t* info,
                          void* stream) {
   if (points == nullptr || info == nullptr || n < 1 || n > kMaxPoints) return GOSLAM_EINVAL;
-  const ObbLayout L(n);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
-  char* ws = static_cast<char*>(workspace);
+  ObbWork w;
+  if (!workspace || workspace_bytes < obb_layout(n, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
-  ObbState* gs = reinterpret_cast<ObbState*>(ws + L.state);
-  int* apt = reinterpret_cast<int*>(ws + L.apt);
-  int* aown = reinterpret_cast<int*>(ws + L.aown);
-  float* adist = reinterpret_cast<float*>(ws + L.adist);
-  int* surv = reinterpret_cast<int*>(ws + L.surv);
-  unsigned char* keep = reinterpret_cast<unsigned char*>(ws + L.keep);
-  unsigned char* vflag = reinterpret_cast<unsigned char*>(ws + L.vflag);
-  int* out = reinterpret_cast<int*>(ws + L.out);
-  const HullMem wh = hull_mem(ws + L.win, kWinCap, kDirs, &gs->wh, nullptr, nullptr, nullptr);
-  const HullMem mh = hull_mem(ws + L.main, facet_cap(n), 0, &gs->mh, apt, aown, adist);
+  ObbState* gs = w.state;
+  const HullMem wh = hull_mem(w.win, kWinCap, kDirs, &gs->wh, nullptr, nullptr, nullptr);
+  const HullMem mh = hull_mem(w.main, facet_cap(n), 0, &gs->mh, w.apt, w.aown, w.adist);
   GS_CUDA(cudaMemsetAsync(gs, 0, sizeof(ObbState), s));
-  GS_CUDA(cudaMemsetAsync(vflag, 0, (size_t)n, s));
+  GS_CUDA(cudaMemsetAsync(w.vflag, 0, (size_t)n, s));
   extremes_kernel<<<grid_for(n), kThreads, 0, s>>>(points, n, make_dirs(), gs);
   GS_CHECK_LAUNCH();
   winners_kernel<<<1, 32, 0, s>>>(gs);
   GS_CHECK_LAUNCH();
   hull_kernel<<<1, kHullThreads, 0, s>>>(points, gs->win, &gs->n_win, wh, &gs->nonfinite, nullptr, nullptr);
   GS_CHECK_LAUNCH();
-  cull_kernel<<<grid_for(n), kThreads, 0, s>>>(points, n, wh, gs, keep);
+  cull_kernel<<<grid_for(n), kThreads, 0, s>>>(points, n, wh, gs, w.keep);
   GS_CHECK_LAUNCH();
-  size_t tb = L.tmp_bytes;
-  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), keep, surv, &gs->n_surv, (int)n,
+  size_t tb = w.tmp_bytes;
+  GS_CUDA(cub::DeviceSelect::Flagged(w.tmp, tb, cub::CountingInputIterator<int>(0), w.keep, w.surv, &gs->n_surv, (int)n,
                                      s));
-  hull_kernel<<<1, kHullThreads, 0, s>>>(points, surv, &gs->n_surv, mh, &gs->nonfinite, surv, vflag);
+  hull_kernel<<<1, kHullThreads, 0, s>>>(points, w.surv, &gs->n_surv, mh, &gs->nonfinite, w.surv, w.vflag);
   GS_CHECK_LAUNCH();
-  tb = L.tmp_bytes;
-  GS_CUDA(cub::DeviceSelect::Flagged(ws + L.tmp, tb, cub::CountingInputIterator<int>(0), vflag, out, &gs->n_vert, (int)n,
+  tb = w.tmp_bytes;
+  GS_CUDA(cub::DeviceSelect::Flagged(w.tmp, tb, cub::CountingInputIterator<int>(0), w.vflag, w.out, &gs->n_vert, (int)n,
                                      s));
   info_kernel<<<1, 1, 0, s>>>(gs, info);
   GS_CHECK_LAUNCH();
@@ -986,11 +986,10 @@ int goslam_hull_vertices(const double* points, int64_t n, void* workspace, size_
 int goslam_hull_vertices_emit(const void* workspace, size_t workspace_bytes, int64_t n, int64_t* out, int64_t count,
                               void* stream) {
   if (n < 1 || n > kMaxPoints || count < 0 || count > n || (count > 0 && out == nullptr)) return GOSLAM_EINVAL;
-  const ObbLayout L(n);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
+  ObbWork w;
+  if (!workspace || workspace_bytes < obb_layout(n, workspace, &w)) return GOSLAM_EWORKSPACE;
   if (count == 0) return GOSLAM_OK;
-  const int* src = reinterpret_cast<const int*>(static_cast<const char*>(workspace) + L.out);
-  widen_kernel<<<grid_for(count), kThreads, 0, (cudaStream_t)stream>>>(src, out, count);
+  widen_kernel<<<grid_for(count), kThreads, 0, (cudaStream_t)stream>>>(w.out, out, count);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }
@@ -998,11 +997,9 @@ int goslam_hull_vertices_emit(const void* workspace, size_t workspace_bytes, int
 int goslam_obb_from_hull(const double* points, int64_t n, const void* workspace, size_t workspace_bytes, double extend,
                          double* box, void* stream) {
   if (points == nullptr || box == nullptr || n < 1 || n > kMaxPoints) return GOSLAM_EINVAL;
-  const ObbLayout L(n);
-  if (workspace == nullptr || workspace_bytes < L.total) return GOSLAM_EWORKSPACE;
-  const char* ws = static_cast<const char*>(workspace);
-  box_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(points, reinterpret_cast<const int*>(ws + L.out),
-                                                        reinterpret_cast<const ObbState*>(ws + L.state), extend, box);
+  ObbWork w;
+  if (!workspace || workspace_bytes < obb_layout(n, workspace, &w)) return GOSLAM_EWORKSPACE;
+  box_kernel<<<1, kThreads, 0, (cudaStream_t)stream>>>(points, w.out, w.state, extend, box);
   GS_CHECK_LAUNCH();
   return GOSLAM_OK;
 }

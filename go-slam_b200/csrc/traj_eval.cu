@@ -67,7 +67,7 @@ size_t cub_bytes(long long n) {
 }
 
 size_t ape_layout(long long n, void* base, ApeWork* w) {
-  GsArena ar(base, ~size_t(0) >> 1);
+  GsArena ar(base);
   const size_t rows = (size_t)std::max<long long>(n, 1);
   w->state = ar.take<ApeState>(1);
   w->flag = ar.take<unsigned char>(rows);
@@ -328,9 +328,8 @@ size_t goslam_ape_workspace_bytes(int64_t n) {
 int goslam_ape_sim3(const double* est, const double* ref, int64_t n, void* workspace, size_t workspace_bytes,
                     double* out, double* errors, void* stream) {
   if (n < 0 || n > kMaxRows || !out || (n > 0 && (!est || !ref || !errors))) return GOSLAM_EINVAL;
-  if (!workspace) return GOSLAM_EWORKSPACE;
   ApeWork w;
-  if (workspace_bytes < ape_layout(n, workspace, &w)) return GOSLAM_EWORKSPACE;
+  if (!workspace || workspace_bytes < ape_layout(n, workspace, &w)) return GOSLAM_EWORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int nb = partial_blocks(n);
   ape_init_kernel<<<1, 32, 0, st>>>(w.state);

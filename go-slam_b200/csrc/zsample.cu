@@ -171,6 +171,13 @@ __global__ void __launch_bounds__(kZWarps * 32) zs_sample_kernel(const ZArgs a) 
   }
 }
 
+// one 256-byte block: the batch's largest sensor depth, as order-preserving bits
+size_t zs_layout(void* base, unsigned** scal) {
+  GsArena ar(base);
+  *scal = ar.take<unsigned>(1);
+  return ar.off;
+}
+
 }  // namespace
 
 extern "C" {
@@ -182,10 +189,10 @@ int goslam_sample_z(const float* rays_o, const float* rays_d, const float* bound
   if (R < 0 || n_samples < 1 || n_surface < 0 || n_samples + n_surface > kZMaxS) return GOSLAM_EINVAL;
   if (gt_depth == nullptr) n_surface = 0;                 // src/render.py:99-101
   if (n_surface > 0 && t_surface == nullptr) return GOSLAM_EINVAL;
-  if (workspace == nullptr || workspace_bytes < 256) return GOSLAM_EWORKSPACE;
+  unsigned* scal;
+  if (!workspace || workspace_bytes < zs_layout(workspace, &scal)) return GOSLAM_EWORKSPACE;
   if (R == 0) return GOSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  unsigned* scal = reinterpret_cast<unsigned*>(workspace);
   if (gt_depth) {
     GS_CUDA(cudaMemsetAsync(scal, 0, sizeof(unsigned), st));
     const int blocks = gs_cdiv(R, 256 * 8) < kNumSms ? gs_cdiv(R, 256 * 8) : kNumSms;
