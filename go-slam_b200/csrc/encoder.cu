@@ -400,10 +400,17 @@ void launch_stats(const ConvArgs& a, int B, float* stats, cudaStream_t s) {
 
 bool conv_ok(const goslam_encoder_conv& c) { return c.w != nullptr && c.b != nullptr; }
 
+// instance norm needs more than one pixel per channel at 1/8 resolution: F.instance_norm raises for a 1x1 input, where
+// the biased variance is 0 and the normalised output would be 0 everywhere
+bool args_ok(int B, int H, int W, int norm) {
+  if (!shape_ok(B, H, W) || (norm != GOSLAM_NORM_NONE && norm != GOSLAM_NORM_INSTANCE)) return false;
+  return norm != GOSLAM_NORM_INSTANCE || (H / 8) * (W / 8) > 1;
+}
+
 }  // namespace
 
 extern "C" size_t goslam_encoder_workspace_bytes(int B, int H, int W, int norm) {
-  if (!shape_ok(B, H, W) || (norm != GOSLAM_NORM_NONE && norm != GOSLAM_NORM_INSTANCE)) return 0;
+  if (!args_ok(B, H, W, norm)) return 0;
   Layout L;
   return encoder_layout(B, H, W, norm, nullptr, &L);
 }
@@ -411,8 +418,7 @@ extern "C" size_t goslam_encoder_workspace_bytes(int B, int H, int W, int norm) 
 extern "C" int goslam_basic_encoder(const goslam_encoder_weights* wt, int norm, int out_dim, const void* image,
                                     int image_is_f16, const float* mean, const float* stdv, int B, int H, int W, void* out,
                                     void* out2, int split, void* workspace, size_t workspace_bytes, void* stream) {
-  if (wt == nullptr || !shape_ok(B, H, W) || (norm != GOSLAM_NORM_NONE && norm != GOSLAM_NORM_INSTANCE))
-    return GOSLAM_EINVAL;
+  if (wt == nullptr || !args_ok(B, H, W, norm)) return GOSLAM_EINVAL;
   if (out_dim <= 0 || out_dim % 32 != 0 || (split && (out_dim != 256 || out2 == nullptr)) || image == nullptr ||
       out == nullptr || (mean == nullptr) != (stdv == nullptr))
     return GOSLAM_EINVAL;

@@ -75,6 +75,9 @@ def encode(weights, norm_fn, out_dim, image, mean=None, std=None, split=False):
     if C != 3 or H % 8 or W % 8:
         raise ValueError("BasicEncoder: image must be [B, 3, H, W] with H and W multiples of 8, got %s"
                          % (tuple(image.shape),))
+    if norm_fn == "instance" and (H // 8) * (W // 8) == 1:
+        raise ValueError("BasicEncoder: instance norm of a %dx%d image has one pixel per channel at 1/8 resolution; "
+                         "F.instance_norm rejects it (Expected more than 1 spatial element)" % (H, W))
     if image.dtype not in (torch.float16, torch.float32):
         image = image.float()
     image = image.contiguous()

@@ -702,7 +702,8 @@ int goslam_mapping_all_rays(const float* c2w, int H, int W, double fx, double fy
  *   reads (x - mean[c]) / stdv[c] in f32 (rounded to f16 after each op for an f16 image), then rounds to f16.
  *   out_dim % 32 == 0.  Output f16 NCHW: out [B,out_dim,H/8,W/8]; with split (out_dim == 256) out = tanh of channels
  *   0-127 and out2 = relu of channels 128-255, each [B,128,H/8,W/8], both from the f16-rounded conv output.
- *   H and W must be multiples of 8 (H*W <= 2^24), B >= 1; otherwise GOSLAM_EINVAL.  About 40 launches on `stream`, no
+ *   H and W must be multiples of 8 (H*W <= 2^24), B >= 1, and with instance norm (H/8)*(W/8) > 1 (F.instance_norm
+ *   rejects a 1x1 input); otherwise GOSLAM_EINVAL.  About 40 launches on `stream`, no
  *   host synchronisation; deterministic (instance statistics are merged per tile in a fixed order).
  *   Workspace: goslam_encoder_workspace_bytes(B, H, W, norm) (0 for an invalid shape or norm).
  * ---------------------------------------------------------------------------------- */

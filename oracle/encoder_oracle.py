@@ -1,9 +1,18 @@
 """BasicEncoder (src/modules/extractor.py) restated with torch.nn.functional, and the pieces of a MotionFilter replay.
 
-Two modes of `basic_encoder`:
+Three modes of `basic_encoder`:
   float64      every op in f64 (the yardstick);
   autocast     the same functional graph under torch.autocast("cuda") with f32 weights: every op gets the dtype and
-               rounding point the reference's nn modules get when DroidNet runs them (MotionFilter's autocast).
+               rounding point the reference's nn modules get when DroidNet runs them (MotionFilter's autocast);
+  round16      float64 arithmetic, rounded to f16 exactly where goslam_basic_encoder (csrc/encoder.cu) stores f16:
+    stem input   (x - mean) / std in f32, then f16; an f16 image is rounded after the subtract and after the divide
+    weights      f16; biases exact
+    conv output  accumulator + bias, then f16; norm 'none': ReLU of the f16 value, and conv2's relu(y + res) in f16
+    instance     mean and biased variance (eps 1e-5) of the f16 conv output; the layer that reads it normalises on
+                 load, applies the ReLU and rounds to f16; the residual tail relu(relu(n2(y)) + x') is rounded once
+                 (x' = relu(n1(stem)) of layer1.0, n3(downsample) of a stride-2 block, unrounded)
+    output       conv2 in f16; split applies tanh / relu to the f16 value and rounds again
+  What is left between round16 and the kernels is the order of their fp32 accumulations and fp32 statistics.
 Weights are a state_dict with the reference's key names (`conv1.weight`, `layer2.0.downsample.0.bias`, ...).
 """
 import numpy as np
@@ -14,43 +23,102 @@ MEAN = (0.485, 0.456, 0.406)
 STDV = (0.229, 0.224, 0.225)
 
 
-def _norm(x, inst):
-    return F.instance_norm(x, eps=1e-5) if inst else x
+def _round16(x):
+    return x.to(torch.float16).to(torch.float64)
 
 
-def _block(sd, p, x, inst, stride):
-    y = F.relu(_norm(F.conv2d(x, sd[p + "conv1.weight"], sd[p + "conv1.bias"], stride, 1), inst))
-    y = F.relu(_norm(F.conv2d(y, sd[p + "conv2.weight"], sd[p + "conv2.bias"], 1, 1), inst))
+def _keep(x):
+    return x
+
+
+def _instance16(x, stats=None):
+    """instance norm (biased variance, eps 1e-5) of f16-valued x in float64.  stats: a list that collects the
+    per-(image, channel) mean, rstd, min and max of x, [B, C] each"""
+    if x.shape[2] * x.shape[3] == 1:
+        raise ValueError("Expected more than 1 spatial element when training, got input size %s" % (x.shape,))
+    mean = x.mean(dim=(2, 3), keepdim=True)
+    rstd = 1.0 / torch.sqrt((x - mean).pow(2).mean(dim=(2, 3), keepdim=True) + 1e-5)
+    if stats is not None:
+        stats.append((mean[..., 0, 0], rstd[..., 0, 0], x.amin(dim=(2, 3)), x.amax(dim=(2, 3))))
+    return (x - mean) * rstd
+
+
+class _Ops:
+    """the graph's convolutions, normalisation and f16 rounding points: identities and F.instance_norm for the float64
+    and autocast modes, so that those run the reference's op sequence unchanged"""
+
+    def __init__(self, sd, inst, round16, trace=None):
+        self.sd, self.inst, self.trace = sd, inst, trace
+        self.r = _round16 if round16 else _keep
+        stats = trace.setdefault("norm", []) if trace is not None else None
+        self.n = (lambda x: _instance16(x, stats)) if round16 else (lambda x: F.instance_norm(x, eps=1e-5))
+
+    def conv(self, x, name, stride, pad):
+        return self.r(F.conv2d(x, self.r(self.sd[name + ".weight"]), self.sd[name + ".bias"], stride, pad))
+
+    def norm(self, x):
+        return self.n(x) if self.inst else x
+
+
+def _block(o, p, x, x_in, stride):
+    """x: the block's input as conv1 reads it; x_in: as the residual adds it"""
+    r, relu = o.r, F.relu
+    y = r(relu(o.norm(o.conv(x, p + "conv1", stride, 1))))
+    y = relu(o.norm(o.conv(y, p + "conv2", 1, 1)))
     if stride > 1:
-        x = _norm(F.conv2d(x, sd[p + "downsample.0.weight"], sd[p + "downsample.0.bias"], stride), inst)
-    return F.relu(x + y)
+        x_in = o.norm(o.conv(x, p + "downsample.0", stride, 0))
+    return r(relu(x_in + y))
 
 
-def _graph(sd, x, inst):
-    x = F.relu(_norm(F.conv2d(x, sd["conv1.weight"], sd["conv1.bias"], 2, 3), inst))
+def _graph(o, x):
+    x_in = F.relu(o.norm(o.conv(x, "conv1", 2, 3)))
+    x = o.r(x_in)
     for layer, stride in ((1, 1), (2, 2), (3, 2)):
-        x = _block(sd, "layer%d.0." % layer, x, inst, stride)
-        x = _block(sd, "layer%d.1." % layer, x, inst, 1)
-    return F.conv2d(x, sd["conv2.weight"], sd["conv2.bias"])
+        x = x_in = _block(o, "layer%d.0." % layer, x, x_in, stride)
+        x = x_in = _block(o, "layer%d.1." % layer, x, x_in, 1)
+    if o.trace is not None:
+        o.trace["head"] = x
+    return o.conv(x, "conv2", 1, 0)
 
 
-def basic_encoder(sd, norm_fn, x, mean=None, std=None, autocast=False):
+def _stem_input16(x, mean, std):
+    """the stem's operand: (x - mean) / std in f32 (after each op in f16 for an f16 image), rounded to f16"""
+    if mean is not None:
+        mu = torch.tensor(mean, dtype=torch.float32, device=x.device)[:, None, None]
+        sd = torch.tensor(std, dtype=torch.float32, device=x.device)[:, None, None]
+        if x.dtype == torch.float16:
+            x = ((x.float() - mu).half().float() / sd).half()
+        else:
+            x = (x.float() - mu) / sd
+    return _round16(x)
+
+
+def basic_encoder(sd, norm_fn, x, mean=None, std=None, autocast=False, round16=False, trace=None):
     """x [B, 3, H, W] -> [B, out_dim, H/8, W/8].  mean / std: (x - mean) / std first, in f32 (autocast) or f64.
-    float64 mode returns f64; autocast mode returns what the reference's autocast graph returns (f16)."""
+    float64 mode returns f64; autocast mode returns what the reference's autocast graph returns (f16); round16 returns
+    f64 holding the f16 values goslam_basic_encoder writes, for an f32 or f16 x.  trace: a dict that receives, in
+    round16 mode, "norm": each instance norm's statistics in graph order (see _instance16) and "head": the output
+    conv's input."""
     if norm_fn not in ("instance", "none"):
         raise NotImplementedError(norm_fn)
+    if autocast and round16:
+        raise ValueError("autocast and round16 are exclusive")
     inst = norm_fn == "instance"
     dt = torch.float32 if autocast else torch.float64
     sd = {k: v.detach().to(x.device, dt) for k, v in sd.items()}
-    x = x.to(dt)
-    if mean is not None:
-        x = (x - torch.tensor(mean, dtype=dt, device=x.device)[:, None, None]) / \
-            torch.tensor(std, dtype=dt, device=x.device)[:, None, None]
+    if round16:
+        x = _stem_input16(x, mean, std)
+    else:
+        x = x.to(dt)
+        if mean is not None:
+            x = (x - torch.tensor(mean, dtype=dt, device=x.device)[:, None, None]) / \
+                torch.tensor(std, dtype=dt, device=x.device)[:, None, None]
+    o = _Ops(sd, inst, round16, trace if round16 else None)
     with torch.no_grad():
         if not autocast:
-            return _graph(sd, x, inst)
+            return _graph(o, x)
         with torch.autocast("cuda"):
-            return _graph(sd, x, inst)
+            return _graph(o, x)
 
 
 def context_split(out):
