@@ -30,12 +30,13 @@ def install(force=True):
 
 def __getattr__(name):
     """goslam_b200.FactorGraph / DepthVideo / Frontend / Backend / MultiviewFilter / MotionFilter /
-    PoseTrajectoryFiller / CorrBlock / AltCorrBlock / BasicEncoder / InstantNeuS, imported on first use"""
+    PoseTrajectoryFiller / CorrBlock / AltCorrBlock / BasicEncoder / InstantNeuS / RefiningMapper, imported on first use"""
     import importlib
     where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video", "Frontend": ".frontend", "Backend": ".backend",
              "MultiviewFilter": ".multiview_filter", "MotionFilter": ".motion_filter",
              "PoseTrajectoryFiller": ".trajectory_filler", "CorrBlock": ".modules.corr",
-             "AltCorrBlock": ".modules.corr", "BasicEncoder": ".modules.extractor", "InstantNeuS": ".neus"}
+             "AltCorrBlock": ".modules.corr", "BasicEncoder": ".modules.extractor", "InstantNeuS": ".neus",
+             "RefiningMapper": ".mapping"}
     if name in where:
         return getattr(importlib.import_module(where[name], __name__), name)
     raise AttributeError("module %r has no attribute %r" % (__name__, name))

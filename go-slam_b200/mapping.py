@@ -11,8 +11,8 @@ torch.cat.  Here:
 The training step (`optimize_map`) is the reference's, on this library's renderer and InstantNeuS.
 
 Documented differences:
-  - cfg['mapping']['BA'] true raises NotImplementedError at construction (camera refinement needs gradients with
-    respect to the rays; every shipped config sets it false).
+  - cfg['mapping']['BA'] true raises NotImplementedError at construction; `RefiningMapper` (below) is the same process
+    with the reference's camera refinement.  Every shipped config sets it false.
   - importing this module does not turn on torch.autograd.set_detect_anomaly(True) process-wide.
   - the snapshot takes the video's mapping lock once per call, where the reference takes it once per frame.
 There is no CPU path: the video buffers must live on a CUDA device.
@@ -135,22 +135,29 @@ def snapshot_frames(video, frames, decay):
 RayBatch = namedtuple("RayBatch", "rays_o rays_d depth color draws")
 
 
+def _draw_batch(snapshot, frame_list, n_rays):
+    """(slots, counts, plan, draws) of one batch: the reference's torch.randint(N_f, (n_rays,)) per random-branch entry
+    in list order on the current CUDA generator, into slices of one buffer"""
+    slots = [snapshot.slot[int(f)] for f in frame_list]
+    counts = [snapshot.counts[s] for s in slots]
+    plan = plan_batch(counts, n_rays)
+    draws = torch.empty((plan.n_draws,), dtype=torch.int64, device=snapshot.c2w.device)
+    at = 0
+    for n, d in zip(counts, plan.draw):
+        if d > 0:
+            draws[at:at + d].random_(0, n)                     # == torch.randint(n, (d,)): the same Philox consumption
+            at += d
+    return slots, counts, plan, draws
+
+
 def build_ray_batch(snapshot, frame_list, n_rays, intrinsics):
     """build_rays(0, H, 0, W, n_rays, ..., nerf_coordinate=False, mask=mask) for every entry of frame_list (repeats
     allowed), concatenated: rays_o, rays_d, color [R,3], depth [R] f32 and the drawn record indices `draws`.
     intrinsics = (fx, fy, cx, cy).  The random draws are the reference's torch.randint(N_f, (n_rays,)) per
     random-branch entry in list order on the current CUDA generator; no host synchronisation."""
     fx, fy, cx, cy = [float(v) for v in intrinsics]
-    slots = [snapshot.slot[int(f)] for f in frame_list]
-    counts = [snapshot.counts[s] for s in slots]
-    plan = plan_batch(counts, n_rays)
+    slots, counts, plan, draws = _draw_batch(snapshot, frame_list, n_rays)
     dev = snapshot.c2w.device
-    draws = torch.empty((plan.n_draws,), dtype=torch.int64, device=dev)
-    at = 0
-    for n, d in zip(counts, plan.draw):
-        if d > 0:
-            draws[at:at + d].random_(0, n)                     # == torch.randint(n, (d,)): the same Philox consumption
-            at += d
     rays_o = torch.empty((plan.R, 3), dtype=torch.float32, device=dev)
     rays_d = torch.empty((plan.R, 3), dtype=torch.float32, device=dev)
     color = torch.empty((plan.R, 3), dtype=torch.float32, device=dev)
@@ -161,6 +168,67 @@ def build_ray_batch(snapshot, frame_list, n_rays, intrinsics):
         _lib.call("mapping_rays", snapshot.workspace, snapshot.workspace.numel(), len(snapshot.frames), snapshot.H,
                   snapshot.W, snapshot.c2w, draws, plan.n_draws, n, arr(*slots), arr(*counts), arr(*plan.draw), fx, fy,
                   cx, cy, rays_o, rays_d, depth, color, plan.R)
+    return RayBatch(rays_o, rays_d, depth, color, draws)
+
+
+def c2w_to_quadt(c2w):
+    """Rt_to_quaternion(c2w, Tquad=False) (src/nerf_func.py:69-88) for c2w [n,4,4] or [4,4] on the device, one launch:
+    (w, x, y, z, tx, ty, tz) f32, the unit quaternion by Shepperd's method in double with w >= 0.  The reference's sign
+    comes from mathutils; either sign gives the same rotation and, under AdamW, the negated trajectory."""
+    _lib.need_cuda("c2w_to_quadt", c2w)
+    m = c2w.detach().to(torch.float32).contiguous()
+    out = torch.empty(m.shape[:-2] + (7,), dtype=torch.float32, device=m.device)
+    n = out.numel() // 7
+    if n > 0:
+        _lib.call("mapping_c2w_to_quadt", m, n, out)
+    return out
+
+
+class _PoseRays(torch.autograd.Function):
+    """rays_o, rays_d of one batch from per-entry leaves quadt [n,7]; backward: d quadt (csrc/mapping.cu)"""
+
+    @staticmethod
+    def forward(ctx, quadt, snapshot, table, draws, intrinsics, R):
+        q = quadt.detach().to(torch.float32).contiguous()
+        dev = q.device
+        rays_o = torch.empty((R, 3), dtype=torch.float32, device=dev)
+        rays_d = torch.empty((R, 3), dtype=torch.float32, device=dev)
+        color = torch.empty((R, 3), dtype=torch.float32, device=dev)
+        depth = torch.empty((R,), dtype=torch.float32, device=dev)
+        if R > 0:
+            _lib.call("mapping_pose_rays", snapshot.workspace, snapshot.workspace.numel(), len(snapshot.frames),
+                      snapshot.H, snapshot.W, q, draws, draws.numel(), *table, *intrinsics, rays_o, rays_d, depth,
+                      color, R)
+        ctx.args = (q, quadt.dtype, snapshot, table, draws, intrinsics, R)
+        ctx.mark_non_differentiable(depth, color)
+        return rays_o, rays_d, depth, color
+
+    @staticmethod
+    def backward(ctx, g_o, g_d, _g_depth, _g_color):
+        q, dtype, snapshot, table, draws, intrinsics, R = ctx.args
+        z = None if g_o is not None and g_d is not None else torch.zeros((R, 3), dtype=torch.float32, device=q.device)
+        g_o = z if g_o is None else g_o.to(torch.float32).contiguous()
+        g_d = z if g_d is None else g_d.to(torch.float32).contiguous()
+        d_q = torch.empty_like(q)
+        _lib.call("mapping_pose_rays_backward", snapshot.workspace, snapshot.workspace.numel(), len(snapshot.frames),
+                  snapshot.H, snapshot.W, q, draws, draws.numel(), *table, *intrinsics, g_o, g_d, R, d_q)
+        return d_q.to(dtype), None, None, None, None, None
+
+
+def build_pose_ray_batch(snapshot, frame_list, n_rays, intrinsics, quadt):
+    """build_ray_batch with entry e's pose quaternion_to_Rt(quadt[e]) (src/nerf_func.py:44-112) in place of its
+    frame's c2w: quadt [len(frame_list),7], one row per entry (a frame listed twice has two rows).  rays_o and rays_d
+    are differentiable with respect to quadt (goslam_mapping_pose_rays_backward); depth, color and the draws are
+    build_ray_batch's, on the same generator, so the random stream does not depend on refinement."""
+    if quadt.dim() != 2 or quadt.shape != (len(frame_list), 7):
+        raise ValueError("build_pose_ray_batch: quadt must be [%d, 7], got %s" % (len(frame_list), tuple(quadt.shape)))
+    _lib.need_cuda("build_pose_ray_batch", quadt)
+    intr = tuple(float(v) for v in intrinsics)
+    slots, counts, plan, draws = _draw_batch(snapshot, frame_list, n_rays)
+    n = len(slots)
+    arr = ctypes.c_int * n
+    table = (n, arr(*slots), arr(*counts), arr(*plan.draw))
+    rays_o, rays_d, depth, color = _PoseRays.apply(quadt, snapshot, table, draws, intr, plan.R)
     return RayBatch(rays_o, rays_d, depth, color, draws)
 
 
@@ -192,6 +260,8 @@ class _TextLogger:
 
 
 class Mapper(object):
+    _refines_cameras = False          # RefiningMapper: mapping.BA is accepted
+
     def __init__(self, cfg, args, slam):
         self.cfg = cfg
         self.args = args
@@ -214,7 +284,7 @@ class Mapper(object):
         self.w_eikonal_loss = m['w_eikonal_loss']
         self.uncertainty_based = m['uncertainty_weight_loss']
         self.BA = m['BA']
-        if self.BA:
+        if self.BA and not self._refines_cameras:
             raise NotImplementedError("goslam_b200.Mapper: mapping-side camera refinement (mapping.BA: True) is not "
                                       "supported")
         self.BA_cam_lr = m['BA_cam_lr']
@@ -286,8 +356,15 @@ class Mapper(object):
                               f' | Loss of total: {total_loss.detach():.4f}, depth: {depth_loss:.4f}, '
                               f'color: {color_loss:.4f}, sdf: {sdf_loss:.4f}, n_rays: {rays_o.shape}!')
 
-    def _train(self, snapshot, frame_list, n_rays, optimizer):
-        batch = build_ray_batch(snapshot, frame_list, n_rays, (self.fx, self.fy, self.cx, self.cy))
+    def _camera_leaves(self, snapshot, visit_list, optimizer):
+        """the per-entry pose leaves of this call's visit iterations: none (RefiningMapper makes them)"""
+        return None
+
+    def _batch(self, snapshot, frame_list, n_rays, leaves):
+        return build_ray_batch(snapshot, frame_list, n_rays, (self.fx, self.fy, self.cx, self.cy))
+
+    def _train(self, snapshot, frame_list, n_rays, optimizer, leaves=None):
+        batch = self._batch(snapshot, frame_list, n_rays, leaves)
         if len(batch.rays_o) < 100:
             return
         self.optimize_map(rays_o=batch.rays_o, rays_d=batch.rays_d, rays_color=batch.color, rays_depth=batch.depth,
@@ -311,6 +388,7 @@ class Mapper(object):
 
         snapshot = snapshot_frames(self.video, visit_list + unvisit_list, self.decay)
         optimizer = self.optimizer
+        leaves = self._camera_leaves(snapshot, visit_list, optimizer)      # before last_visit moves
 
         bd = self.video.get_bound()
         with self.video.mapping.get_lock():
@@ -339,9 +417,45 @@ class Mapper(object):
         for _ in range(num_joint_iters):
             if len(visit_list) < 1:
                 continue
-            self._train(snapshot, visit_list, self.mapping_pixels // len(visit_list), optimizer)
+            self._train(snapshot, visit_list, self.mapping_pixels // len(visit_list), optimizer, leaves)
 
         self.reload_map += 1
         self.init = False
         del snapshot
         torch.cuda.empty_cache()
+
+
+class RefiningMapper(Mapper):
+    """Mapper with the reference's camera refinement in mapping (cfg['mapping']['BA'], src/mapping.py:173-194, 266-273):
+    once last_visit >= 10 (tested before this call moves it), every entry of the visit list — a frame listed twice
+    gets two — has a quaternion-translation leaf from its snapshot c2w (c2w_to_quadt, one launch); the leaves replace
+    the optimizer's previous camera group (kept while it has more than the two network groups) as one group at
+    BA_cam_lr with the optimizer's other defaults; every visit iteration builds its rays from the current leaves
+    (build_pose_ray_batch), so AdamW moves the map and the cameras together.  The unvisit iterations use the snapshot
+    c2w: the leaves have no gradient there and AdamW skips them.  clip_grad_norm_ covers the network parameters only,
+    and the refined poses are not written back to the video, as in the reference.  With BA false, or before
+    last_visit reaches 10, it is Mapper.
+
+    Documented difference: the AdamW state of a camera group that is replaced is dropped from optimizer.state (the
+    reference keeps it, unread, for the life of the optimizer)."""
+    _refines_cameras = True
+
+    def _camera_leaves(self, snapshot, visit_list, optimizer):
+        if not (self.BA and self.last_visit >= 10):
+            return None
+        dev = snapshot.c2w.device
+        slots = torch.tensor([snapshot.slot[int(f)] for f in visit_list], dtype=torch.int64).pin_memory()
+        quadt = c2w_to_quadt(snapshot.c2w.index_select(0, slots.to(dev, non_blocking=True)))
+        leaves = [q.detach().requires_grad_(True) for q in quadt]          # rows of one buffer, each its own leaf
+        if len(optimizer.param_groups) > 2:
+            for p in optimizer.param_groups.pop()['params']:
+                optimizer.state.pop(p, None)
+        if len(leaves) > 0:
+            optimizer.add_param_group({'params': leaves, 'lr': self.BA_cam_lr})
+        return leaves
+
+    def _batch(self, snapshot, frame_list, n_rays, leaves):
+        if leaves is None:
+            return build_ray_batch(snapshot, frame_list, n_rays, (self.fx, self.fy, self.cx, self.cy))
+        return build_pose_ray_batch(snapshot, frame_list, n_rays, (self.fx, self.fy, self.cx, self.cy),
+                                    torch.stack(leaves))

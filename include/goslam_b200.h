@@ -673,6 +673,26 @@ int goslam_update_op(const goslam_update_weights* weights, const void* net, cons
  *
  * goslam_mapping_all_rays — rays_o, rays_d [H*W,3] of every pixel of one image in raster order under c2w [4,4] (device),
  *   the arithmetic of goslam_mapping_rays.
+ *
+ * Camera refinement (mapping.BA: src/mapping.py:173-194, 266-273; src/nerf_func.py:44-112): one quaternion-translation
+ * leaf quadt = (w, x, y, z, tx, ty, tz) per entry of the visit list, repeated frames included.
+ *
+ * goslam_mapping_c2w_to_quadt — quadt [n,7] (f32) of c2w [n,4,4] (row-major f32): Rt_to_quaternion(c2w, Tquad=False)
+ *   for a batch.  The unit quaternion of the rotation block by Shepperd's four-branch method in double, normalised,
+ *   sign fixed to w >= 0 (quad2rotation is even in q), then the translation.  One launch.
+ *
+ * goslam_mapping_pose_rays — goslam_mapping_rays with each entry's pose taken from quadt [n_entries,7] (entry-indexed,
+ *   not slot-indexed) in place of c2w: R = quad2rotation(q) with the reference's f32 expressions, each operation
+ *   rounded, two_s = 2 / (((r^2 + i^2) + j^2) + k^2), R00 = 1 - two_s (j^2 + k^2), R01 = two_s (i j - k r), ...;
+ *   rays_d and rays_o = (tx, ty, tz) then as goslam_mapping_rays, with the same draws, records and outputs.
+ *
+ * goslam_mapping_pose_rays_backward — the same entry table, draws and quadt, plus d_rays_o, d_rays_d [R,3] (f32,
+ *   R <= max_rays rows in the forward's order); writes (does not accumulate) d_quadt [n_entries,7] (f32).  Per entry,
+ *   in double: G[a][c] = sum_r d_rays_d[r][a] dirs[r][c] (dirs recomputed from the records as the forward computes
+ *   them), g_t = sum_r d_rays_o[r], then with R = I + s A(q), s = 2 / |q|^2 (|q| need not be 1):
+ *     d_q = -s^2 q <G, A> + s <G, dA/dq>,   d_t = g_t.
+ *   One block of 256 threads per entry sums its rows in a fixed order (no atomics): the result does not depend on the
+ *   launch or on the 64-entry chunking, and an entry without rows gets zeros.  Neither pose entry synchronises the host.
  * ---------------------------------------------------------------------------------- */
 size_t goslam_mapping_snapshot_workspace_bytes(int F, int H, int W);
 int goslam_mapping_snapshot(const float* images, const float* mask, const float* disps, float* update_priority, int buffer,
@@ -684,6 +704,16 @@ int goslam_mapping_rays(const void* workspace, size_t workspace_bytes, int F, in
                         float* color, int64_t max_rays, void* stream);
 int goslam_mapping_all_rays(const float* c2w, int H, int W, double fx, double fy, double cx, double cy, float* rays_o,
                             float* rays_d, void* stream);
+int goslam_mapping_c2w_to_quadt(const float* c2w, int n, float* quadt, void* stream);
+int goslam_mapping_pose_rays(const void* workspace, size_t workspace_bytes, int F, int H, int W, const float* quadt,
+                             const int64_t* draws, int64_t n_draws, int n_entries, const int* slots, const int* counts,
+                             const int* draw, double fx, double fy, double cx, double cy, float* rays_o, float* rays_d,
+                             float* depth, float* color, int64_t max_rays, void* stream);
+int goslam_mapping_pose_rays_backward(const void* workspace, size_t workspace_bytes, int F, int H, int W,
+                                      const float* quadt, const int64_t* draws, int64_t n_draws, int n_entries,
+                                      const int* slots, const int* counts, const int* draw, double fx, double fy,
+                                      double cx, double cy, const float* d_rays_o, const float* d_rays_d,
+                                      int64_t max_rays, float* d_quadt, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Feature / context encoder: DroidNet's BasicEncoder forward (src/modules/extractor.py) for norm_fn 'instance'
