@@ -30,13 +30,15 @@ def install(force=True):
 
 def __getattr__(name):
     """goslam_b200.FactorGraph / DepthVideo / Frontend / Backend / MultiviewFilter / MotionFilter /
-    PoseTrajectoryFiller / CorrBlock / AltCorrBlock / BasicEncoder / InstantNeuS / RefiningMapper, imported on first use"""
+    PoseTrajectoryFiller / CorrBlock / AltCorrBlock / BasicEncoder / InstantNeuS / RefiningMapper and the rendering
+    metrics image_metrics / keyframe_views / eval_render / RenderMetrics, imported on first use"""
     import importlib
     where = {"FactorGraph": ".factor_graph", "DepthVideo": ".depth_video", "Frontend": ".frontend", "Backend": ".backend",
              "MultiviewFilter": ".multiview_filter", "MotionFilter": ".motion_filter",
              "PoseTrajectoryFiller": ".trajectory_filler", "CorrBlock": ".modules.corr",
              "AltCorrBlock": ".modules.corr", "BasicEncoder": ".modules.extractor", "InstantNeuS": ".neus",
-             "RefiningMapper": ".mapping"}
+             "RefiningMapper": ".mapping", "image_metrics": ".render_eval", "keyframe_views": ".render_eval",
+             "eval_render": ".render_eval", "RenderMetrics": ".render_eval"}
     if name in where:
         return getattr(importlib.import_module(where[name], __name__), name)
     raise AttributeError("module %r has no attribute %r" % (__name__, name))

@@ -885,6 +885,33 @@ size_t goslam_ape_workspace_bytes(int64_t n);
 int goslam_ape_sim3(const double* est, const double* ref, int64_t n, void* workspace, size_t workspace_bytes,
                     double* out, double* errors, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Rendering quality of K views against their reference images (not a function of the reference project): PSNR, SSIM
+ * and depth L1 per frame.  Device pointers, no allocation, no host synchronisation.
+ *
+ * goslam_render_metrics — color [K, H*W, 3] f32 (Renderer.render_img's 'color' layout), depth [K, H*W] f32 in metres,
+ *   gt_color [K, 3, H, W] f32 (DepthVideo.images' layout; data range 1), gt_depth [K, H, W] f32, mask [K, H, W] u8 or
+ *   NULL.  Per frame k:
+ *   psnr[k]     = -10 log10(MSE), MSE over all H*W*3 values; +inf when MSE = 0.
+ *   ssim[k]     = per channel, the SSIM map at the (H-10) x (W-10) positions where the 11 x 11 window fits (no
+ *                 padding), averaged over the positions and then the three channels.  Window: the separable Gaussian
+ *                 w_i = exp(-(i-5)^2 / 4.5) / sum_j exp(-(j-5)^2 / 4.5), i = 0..10 (sigma 1.5).  With mu, the
+ *                 window means of x (rendered) and y (reference), sigma_x^2 = E[x^2] - mu_x^2, sigma_y^2 likewise,
+ *                 sigma_xy = E[xy] - mu_x mu_y, C1 = 0.01^2, C2 = 0.03^2:
+ *                 SSIM = (2 mu_x mu_y + C1)(2 sigma_xy + C2) / ((mu_x^2 + mu_y^2 + C1)(sigma_x^2 + sigma_y^2 + C2)).
+ *   depth_l1[k] = the mean of |depth - gt_depth| over the pixels where gt_depth is finite and > 0 and the mask, if
+ *                 given, is non-zero; NaN when there are none.  depth_count[k] (i64) = that number of pixels.
+ *   The moments are filtered and every sum is taken in f64, in a fixed order: two calls give the same bits, and a
+ *   frame's results do not depend on the other frames of the call.
+ *   GOSLAM_EINVAL: K < 0, H or W below 11, H*W above 2^31 - 1, or (for K > 0) a NULL pointer other than mask.  K = 0
+ *   returns GOSLAM_OK and touches nothing.  GOSLAM_EWORKSPACE: no workspace or fewer than
+ *   goslam_render_metrics_workspace_bytes(K, H, W) bytes (0 only for an invalid shape).
+ * ---------------------------------------------------------------------------------- */
+size_t goslam_render_metrics_workspace_bytes(int K, int H, int W);
+int goslam_render_metrics(const float* color, const float* depth, const float* gt_color, const float* gt_depth,
+                          const uint8_t* mask, int K, int H, int W, void* workspace, size_t workspace_bytes,
+                          double* psnr, double* ssim, double* depth_l1, int64_t* depth_count, void* stream);
+
 /* Training-only entry points of the reference module are exported for ABI completeness
  * and return GOSLAM_EUNSUPPORTED (inference path is torch.no_grad, src/slam.py:45). */
 int goslam_corr_index_backward(void);
