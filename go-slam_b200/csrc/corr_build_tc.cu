@@ -62,19 +62,25 @@ constexpr int kStoreWarps = 3;                           // producer-warpgroup w
 //   level-0 staging (2 per warpgroup, m64)      4 x 16 KB
 //   level-1 staging (2 per warpgroup, m64)      4 x 4 KB
 //   level-2/3 band pool                         2 x 128 x (pitch2 + 32) B
-//   + 1 KB of alignment slack.  w = 80 (n_xb = 5): 210 KB; w = 128 (n_xb = 8): 218 KB (<= 227 KB).
+//   reverse-edge pairing (partner, work order)  2 KB
+//   + 1 KB of alignment slack.  w = 80 (n_xb = 5): 212 KB; w = 128 (n_xb = 8): 220 KB (<= 227 KB).
 constexpr int kBarBytes = 1024;
 constexpr int kL0HalfBytes = 64 * 2 * 128;        // m64 half of a tile's level 0: 64 source px x 2 tile rows x 128 B
 constexpr int kL1HalfBytes = 64 * 64;             // ... of its level 1: 64 source px x one tile row of 2 tiles (64 B)
 constexpr int kL0WarpBytes = kL0HalfBytes / kGroupWarps, kL1WarpBytes = kL1HalfBytes / kGroupWarps;  // 16 source px
 constexpr int kL3BandBytes = kBM * 32;            // a band's level-3 pieces, 32 B per source pixel
 constexpr int kFixedBytes = 1024 + kBarBytes + (1 + kBStages) * kTileBytes;
+// Reverse-edge pairing (a build with an alias table): per edge of the call its partner if it is a reader
+// (int16, -1 otherwise) and the work order of the edges (full edges first, then readers), for calls of up to
+// kMaxPairEdges edges; larger calls are not paired.
+constexpr int kMaxPairEdges = 512;
+constexpr int kPairBytes = 2 * kMaxPairEdges * 2;
 // the level-2 staging is dense: one piece of pitch2 bytes per source pixel, the box of the level-2 tensor map
 __host__ __device__ constexpr int pitch2_of(int n_xb) { return (n_xb * 16 + 31) / 32 * 32; }
 // one of the two band buffers, level 2 then level 3
 __host__ __device__ constexpr int band_bytes(int n_xb) { return kBM * pitch2_of(n_xb) + kL3BandBytes; }
 __host__ __device__ constexpr int smem_bytes(int n_xb) {
-  return kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + 2 * band_bytes(n_xb);
+  return kFixedBytes + 2 * kBStages * (kL0HalfBytes + kL1HalfBytes) + 2 * band_bytes(n_xb) + kPairBytes;
 }
 static_assert(smem_bytes(kMaxXB) <= 227 * 1024, "corr_build_tc_kernel exceeds the 227 KB of shared memory of a block");
 
@@ -92,7 +98,42 @@ struct TcParams {
   // source pixel's plane (plane = H4*W4 tiles; the padding is unspecified); levels 2, 3 stay row-major.
   int w4_0, h4_0, w4_1, h4_1;
   int pitch2, pitch3;         // bytes per (source pixel, band) of levels 2 / 3 (multiples of 32)
+  // optional per-slot level-0 alias table (CorrPool), one 16-byte row per slot: alias[4s] = 2 * (slot holding s's
+  // level 0) + (1 if that level 0 is stored transposed), words 1-3 zero.  With it the build pairs reverse edges of the call (pair_edges) and writes
+  // the entry of every slot it builds; without it every edge writes its own level 0 and no table is touched.
+  int* alias;
 };
+
+// Edge r of a call is the READER of edge e when (ii[r], jj[r]) == (jj[e], ii[e]), ii[e] != jj[e], both
+// orientations occur exactly once in the call, and e < r.  corr(j,i)[q][p] = <f_j(q), f_i(p)> = corr(i,j)[p][q]
+// and the wgmma sums the same products in the same k order for both, so a reader's level 0 is bit for bit the
+// transpose of its partner's: the reader skips its level-0 stores and the lookup reads the partner's planes.
+// Rig-2 self-edges (ii == jj) read the second camera and are never paired.  Fills part[n] (the partner of a
+// reader, -1 otherwise) and order[] (the full edges, then the readers, each in call order) for n < N; every
+// thread of the block takes part.
+__device__ void pair_edges(const TcParams& p, int16_t* part, int16_t* order) {
+  const int N = p.N;
+  for (int n = threadIdx.x; n < N; n += blockDim.x) {
+    const int64_t a = p.ii[n], b = p.jj[n];
+    int fwd = 0, rev = 0, partner = -1;
+    for (int m = 0; m < N; ++m) {
+      const int64_t c = __ldg(p.ii + m), d = __ldg(p.jj + m);
+      fwd += (c == a && d == b);
+      if (c == b && d == a) { ++rev; partner = m; }
+    }
+    part[n] = (int16_t)((a != b && fwd == 1 && rev == 1 && partner < n) ? partner : -1);
+  }
+  __syncthreads();
+  int n_full = 0;
+  for (int m = 0; m < N; ++m) n_full += part[m] < 0;
+  for (int n = threadIdx.x; n < N; n += blockDim.x) {
+    const bool rd = part[n] >= 0;
+    int rank = 0;
+    for (int m = 0; m < n; ++m) rank += (part[m] >= 0) == rd;
+    order[rd ? n_full + rank : rank] = (int16_t)n;
+  }
+  __syncthreads();
+}
 
 // Build-time switch for profiling builds only (tools/build_variant.py -DGOSLAM_TC_EXPERIMENT=N); the shipped
 // library has it at 0.  1 = no output writes.  2 = stores only: no operand loads and no MMAs (the accumulators
@@ -138,7 +179,7 @@ __device__ __forceinline__ float pool_pair(uint32_t top, uint32_t bot) {
 template <typename F>
 __device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], unsigned char* st0, unsigned char* st1,
                                                     unsigned char* pool2_row0, int p2src, int p2row, int xb,
-                                                    int wrow, int lane, F between_levels) {
+                                                    int wrow, int lane, bool l0, F between_levels) {
   // packed rounded fp16 pairs: W[rh][ty][r4][jx] = x pair (8jx + 2(lane%4), +1) of patch row 4ty + r4
   uint32_t W[2][2][4][2];
 #pragma unroll
@@ -152,10 +193,10 @@ __device__ __forceinline__ void tiled_half_epilogue(const float (&acc)[2][32], u
           const int j = 2 * r4 + jx;
           W[rh][ty][r4][jx] = pack2(acc[ty][4 * j + 2 * rh], acc[ty][4 * j + 2 * rh + 1]);
         }
-  // ---- level 0: 8 x stmatrix.x4 ----
+  // ---- level 0: 8 x stmatrix.x4 (not for a reader edge, whose level 0 its partner holds) ----
   // Matrix row s (source row 8rh + s) takes tile row ty = a ^ (s >> 2): the 8 rows of a matrix then land on
   // 8 different swizzle phases (R & 7 = (2s + ty) & 7), so each matrix is one conflict-free wavefront.
-  {
+  if (l0) {
     const bool lo = (lane & 3) < 2;                // lanes holding tile 2jx (the others: tile 2jx + 1)
     const bool dflip = (lane >> 4) & 1;            // data rows s = lane/4 >= 4
     const int s8 = lane & 7;                       // address: row s8 of matrix lane/8 = (rh, tile parity)
@@ -235,6 +276,8 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
   // level-0 / level-1 staging, two m64 halves per warpgroup, then the two band buffers (levels 2, 3)
   unsigned char* smL0 = smB + kBStages * kTileBytes;
   unsigned char* smL1 = smL0 + 2 * kBStages * kL0HalfBytes;
+  int16_t* part = reinterpret_cast<int16_t*>(smL1 + 2 * kBStages * kL1HalfBytes + 2 * band_bytes(p.n_xb));
+  int16_t* order = part + kMaxPairEdges;
   constexpr bool wr = kExperiment != 1;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -247,6 +290,37 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     fence_barrier_init();
   }
   __syncthreads();
+  const bool paired = p.alias != nullptr && p.ii != nullptr && p.N <= kMaxPairEdges;
+  if (paired) pair_edges(p, part, order);
+  if (p.alias != nullptr && blockIdx.x == 0) {
+    // the level-0 alias entry (one 16-byte row) of every slot this call builds, staged in the level-0 staging
+    // (not yet in use) and written with bulk copies, so that the kernel's global writes all leave through the
+    // async proxy; stream order puts them before any lookup of these slots
+    int4* rows = reinterpret_cast<int4*>(smL0);
+    for (int n0 = 0; n0 < p.N; n0 += kMaxPairEdges) {
+      const int cnt = min(kMaxPairEdges, p.N - n0);
+      for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
+        const int n = n0 + i, s = p.out_slot ? __ldg(p.out_slot + n) : n;
+        const int e = paired ? part[n] : -1;
+        rows[i] = make_int4(e < 0 ? 2 * s : 2 * (p.out_slot ? __ldg(p.out_slot + e) : e) + 1, 0, 0, 0);
+      }
+      fence_async_smem();
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        for (int i = 0; i < cnt; ++i) {
+          const int s = p.out_slot ? __ldg(p.out_slot + n0 + i) : n0 + i;
+          bulk_store(p.alias + 4 * (size_t)s, rows + i, 16);
+        }
+        bulk_commit();
+        bulk_wait_read<0>();                     // the staging is reused below; the writes finish by kernel exit
+      }
+      __syncthreads();
+    }
+  }
+  // work item -> edge: the full edges' items first, then the readers', so that the round-robin deal gives
+  // every CTA the same mix of both (to within one item each)
+  const int per_edge = p.n_mt * p.n_yb;
+  auto edge_of = [&](int item) { const int k = item / per_edge; return paired ? (int)order[k] : k; };
 
   if (warp >= kEpiThreads / 32) {
     // ===================== TMA producer (one thread of the producer warpgroup) =====================
@@ -258,7 +332,7 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
       for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
         const int yb = item % p.n_yb;
         const int mt = (item / p.n_yb) % p.n_mt;
-        const int n = item / (p.n_yb * p.n_mt);
+        const int n = edge_of(item);
         int n1 = n, n2 = n;
         if (p.ii != nullptr) {
           const int fi = (int)p.ii[n], fj = (int)p.jj[n];
@@ -297,7 +371,7 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
       for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it) {
         const int yb = item % p.n_yb;
         const int mt = (item / p.n_yb) % p.n_mt;
-        const int n = item / (p.n_yb * p.n_mt);
+        const int n = edge_of(item);
         const bool out2 = wr && p.num_levels > 2 && 2 * yb < h2, out3 = wr && p.num_levels > 3 && yb < h3;
         unsigned char* s2 = pool2 + (it & 1) * band_bytes(p.n_xb);
         const uint32_t s2_u = smem_u32(s2), s3_u = s2_u + kBM * p2src;
@@ -349,8 +423,9 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
     for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it) {
       const int yb = item % p.n_yb;
       const int mt = (item / p.n_yb) % p.n_mt;
-      const int n = item / (p.n_yb * p.n_mt);
+      const int n = edge_of(item);
       const int n_out = p.out_slot ? __ldg(p.out_slot + n) : n;
+      const bool own0 = !paired || part[n] < 0;   // a reader's level 0 is its partner's, transposed
       mbar_wait(full_a, aph);
       aph ^= 1;
       bool a_held = true;
@@ -410,11 +485,11 @@ corr_build_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_cons
           const bool out0 = wr && s0 < p.hw;         // rows >= hw of the ragged last m-tile: clipped by the maps
           if (lane == 0) bulk_wait_read<3>();
           __syncwarp();
-          tiled_half_epilogue(acc[mh], st0, st1, band + mh * 64 * p2src, p2src, p2row, xb, wq * 16, lane, [&] {
+          tiled_half_epilogue(acc[mh], st0, st1, band + mh * 64 * p2src, p2src, p2row, xb, wq * 16, lane, own0, [&] {
             fence_async_smem();                      // the staged box becomes visible to the TMA engine
             __syncwarp();
             if (lane == 0) {
-              if (out0) tma_store_4d_hint(&mapL0, st0 + wq * kL0WarpBytes, xb * 64, 2 * yb, s0, n_out, stream);
+              if (out0 && own0) tma_store_4d_hint(&mapL0, st0 + wq * kL0WarpBytes, xb * 64, 2 * yb, s0, n_out, stream);
               bulk_commit();
               bulk_wait_read<3>();
             }
@@ -563,7 +638,7 @@ int corr_build_setup(int) {
 
 // launch the tensor-core kernel on the video-level K-major (pre-scaled) feature maps f = [F, hw, 128]
 int launch_tc(const __half* f, int F, const int64_t* ii, const int64_t* jj, int rig, const int* out_slot,
-              __half* const* levels, int num_levels, int N, int h, int w, cudaStream_t st) {
+              int* alias, __half* const* levels, int num_levels, int N, int h, int w, cudaStream_t st) {
   const int hw = h * w;
   // the tensor stores need 16-byte aligned level buffers
   for (int i = 0; i < num_levels; ++i)
@@ -579,7 +654,7 @@ int launch_tc(const __half* f, int F, const int64_t* ii, const int64_t* jj, int 
   p.num_levels = num_levels; p.N = N; p.h = h; p.w = w; p.hw = hw;
   p.n_mt = gs_cdiv(hw, kBM); p.n_yb = gs_cdiv(h, kPY); p.n_xb = gs_cdiv(w, kPX);
   p.n_items = N * p.n_mt * p.n_yb;
-  p.ii = ii; p.jj = jj; p.rig = rig; p.out_slot = out_slot;
+  p.ii = ii; p.jj = jj; p.rig = rig; p.out_slot = out_slot; p.alias = alias;
   p.w4_0 = gs_cdiv(w, 4); p.h4_0 = gs_cdiv(h, 4);
   p.w4_1 = gs_cdiv(w >> 1, 4); p.h4_1 = gs_cdiv(h >> 1, 4);
   p.pitch2 = pitch2_of(p.n_xb); p.pitch3 = 32;
@@ -623,13 +698,64 @@ size_t goslam_corr_level_plane_elems(int level, int layout, int h, int w) {
 int goslam_corr_pool_build(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
                            const int64_t* jj, const int* slots, void* const* levels,
                            int num_levels, int N, int D, int h, int w, void* stream) {
+  return goslam_corr_pool_build_paired(fmaps_kmajor, F, rig, ii, jj, slots, nullptr, levels, num_levels, N, D, h,
+                                       w, stream);
+}
+
+int goslam_corr_pool_build_paired(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
+                                  const int64_t* jj, const int* slots, int* alias, void* const* levels,
+                                  int num_levels, int N, int D, int h, int w, void* stream) {
   if (N < 0 || F <= 0 || rig < 1 || D != kD || h <= 0 || w <= 0 || num_levels < 1 || num_levels > 4)
     return GOSLAM_EINVAL;
   if ((h >> (num_levels - 1)) <= 0 || (w >> (num_levels - 1)) <= 0) return GOSLAM_EINVAL;
   if (w > kMaxXB * kPX) return GOSLAM_EINVAL;
   if (N == 0) return GOSLAM_OK;
-  return launch_tc(reinterpret_cast<const __half*>(fmaps_kmajor), F, ii, jj, rig, slots,
+  return launch_tc(reinterpret_cast<const __half*>(fmaps_kmajor), F, ii, jj, rig, slots, alias,
                    reinterpret_cast<__half* const*>(levels), num_levels, N, h, w, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// Materialize aliased level-0 planes: slot slots[i] gets its own level 0, the transpose of holders[i]'s, and its
+// alias entry is reset to itself.  Element (q, p) of the slot is element (p, q) of the holder; the padding of a
+// plane is written as zeros, as the build leaves it.
+__global__ void __launch_bounds__(256)
+corr_unalias_kernel(__half* __restrict__ l0, int* __restrict__ alias, const int* __restrict__ slots,
+                    const int* __restrict__ holders, int h, int w) {
+  const int hw = h * w, w4 = gs_cdiv(w, 4);
+  const long long plane = (long long)gs_cdiv(h, 4) * w4 * 16;
+  const int s = __ldg(slots + blockIdx.y), t = __ldg(holders + blockIdx.y);
+  __half* dst = l0 + (long long)s * hw * plane;
+  const __half* src = l0 + (long long)t * hw * plane;
+  const long long total = (long long)hw * plane;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int q = (int)(i / plane), off = (int)(i % plane);
+    const int tile = off >> 4, py = (tile / w4) * 4 + ((off >> 2) & 3), px = (tile % w4) * 4 + (off & 3);
+    __half v = __float2half(0.f);
+    if (py < h && px < w) {
+      const int qy = q / w, qx = q % w;
+      const int qoff = ((qy >> 2) * w4 + (qx >> 2)) * 16 + (qy & 3) * 4 + (qx & 3);
+      v = src[(long long)(py * w + px) * plane + qoff];
+    }
+    dst[i] = v;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) alias[4 * (size_t)s] = 2 * s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int goslam_corr_pool_unalias(void* level0, int* alias, const int* slots, const int* holders, int n, int h, int w,
+                             void* stream) {
+  if (n < 0 || h <= 0 || w <= 0) return GOSLAM_EINVAL;
+  if (n == 0) return GOSLAM_OK;
+  corr_unalias_kernel<<<dim3(264, n), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<__half*>(level0), alias,
+                                                                       slots, holders, h, w);
+  GS_CHECK_LAUNCH();
+  return GOSLAM_OK;
 }
 
 }  // extern "C"

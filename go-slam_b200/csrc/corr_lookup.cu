@@ -50,6 +50,7 @@ struct LookupArgs {
   // otherwise row y starts at element (y >> rsh) * pitch + (y & rsh) * wrow   (rsh in {0, 1};
   // reference layout: rsh = 0, pitch = w2)
   int rsh[kMaxLevels], pitch[kMaxLevels], wrow[kMaxLevels];
+  const int* alias;      // optional level-0 alias table, 4 words per slot (goslam_corr_pool_lookup_aliased)
 };
 
 // ---- row fetch: 8 consecutive elements starting at absolute element index e0 ----------
@@ -119,6 +120,23 @@ __device__ __forceinline__ void fetch_row8_tiled_h(const __half* __restrict__ pl
   w[3] = __funnelshift_r(u3, u4, sh);
 }
 
+// Transposed level 0 (a reader edge, goslam_corr_pool_lookup_aliased): tap (y1, x1 + t) of source pixel q is
+// element q (tiled offset qoff) of plane y1 * w2 + x1 + t of the holder slot.  Columns outside [0, w2) read as
+// zero; the taps fill the words fetch_row8_tiled_h fills.
+__device__ __forceinline__ void fetch_row8_transposed_h(const __half* __restrict__ vol, long long plane_base, int y1,
+                                                        int x1, int w2, long long plane, int qoff, uint32_t (&w)[4]) {
+  const unsigned short* row = reinterpret_cast<const unsigned short*>(vol) + plane_base +
+                              (long long)y1 * w2 * plane + qoff;
+  uint32_t t[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int x = x1 + i;
+    t[i] = (x >= 0 && x < w2) ? (uint32_t)__ldg(row + (long long)x * plane) : 0u;
+  }
+#pragma unroll
+  for (int m = 0; m < 4; ++m) w[m] = t[2 * m] | (t[2 * m + 1] << 16);
+}
+
 __device__ __forceinline__ __half2 u2h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
 __device__ __forceinline__ uint32_t h22u(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 
@@ -145,7 +163,7 @@ __device__ __forceinline__ void lookup_pass_h(const __half* __restrict__ vol, lo
                                               long long plane_base, int h2, int w2, int w4, int rsh,
                                               int pitch, int wrow, float x0,
                                               float y0, int row, bool active, __half* stage,
-                                              int stage_ld, int px_in_tile) {
+                                              int stage_ld, int px_in_tile, long long plane, int qoff) {
   constexpr int RD = 2 * R + 1;
   static_assert(RD + 1 == 8, "row-lane mapping assumes radius 3 (8-tap windows)");
   const float fx0 = floorf(x0), fy0 = floorf(y0);
@@ -155,7 +173,8 @@ __device__ __forceinline__ void lookup_pass_h(const __half* __restrict__ vol, lo
 
   uint32_t own[4] = {0, 0, 0, 0};
   if (active && y1 >= 0 && y1 < h2 && x1 > -8 && x1 < w2) {
-    if (w4 > 0) fetch_row8_tiled_h(vol + plane_base, y1, x1, w4, own);
+    if (qoff >= 0) fetch_row8_transposed_h(vol, plane_base, y1, x1, w2, plane, qoff, own);
+    else if (w4 > 0) fetch_row8_tiled_h(vol + plane_base, y1, x1, w4, own);
     else fetch_row8_h(vol, plane_base + (long long)(y1 >> rsh) * pitch + (y1 & rsh) * wrow + x1, total, own);
     mask_cols_h(own, x1, w2);
   }
@@ -273,6 +292,7 @@ corr_lookup_kernel(const LookupArgs a) {
 
   const int n = blockIdx.y;
   const int nv = a.slot ? __ldg(a.slot + n) : n;      // where this edge's volume lives
+  const int al = a.alias ? __ldg(a.alias + 4 * (size_t)nv) : 2 * nv;   // ... and its level 0 (holder slot, transposed)
   const int k0 = blockIdx.x * kTile;
   const int lane8 = threadIdx.x & 7;          // window row
   const int pslot = threadIdx.x >> 3;         // 0..31 pixel slot within a pass
@@ -302,15 +322,20 @@ corr_lookup_kernel(const LookupArgs a) {
     const long long total = (long long)a.cap * a.hw1 * plane;
     const T* vol = reinterpret_cast<const T*>(a.vol[lvl]);
     const float sc = a.inv_scale[lvl];
+    // per edge (blockIdx.y), so no divergence: a transposed level 0 is read as element k of the holder's planes
+    const bool tr = lvl == 0 && (al & 1);
 #pragma unroll
     for (int ps = 0; ps < 2; ++ps) {
       const int k = k0 + ps * 32 + pslot;
-      const long long pbase = ((long long)nv * a.hw1 + k) * plane;
+      const long long pbase = tr ? (long long)(al >> 1) * a.hw1 * plane
+                                 : ((long long)(lvl == 0 ? al >> 1 : nv) * a.hw1 + k) * plane;
       if constexpr (sizeof(T) == 2) {
+        const int qy = k / w2, qx = k - qy * w2;
+        const int qoff = tr ? ((qy >> 2) * a.w4[0] + (qx >> 2)) * 16 + (qy & 3) * 4 + (qx & 3) : -1;
         lookup_pass_h<R>(reinterpret_cast<const __half*>(vol), total, pbase, h2, w2, a.w4[lvl], a.rsh[lvl],
                          a.pitch[lvl], a.wrow[lvl], cx[ps] * sc,
                          cy[ps] * sc, lane8, act[ps], reinterpret_cast<__half*>(stage), LD,
-                         ps * 32 + pslot);
+                         ps * 32 + pslot, plane, qoff);
       } else {
         lookup_pass_f<R>(reinterpret_cast<const float*>(vol), pbase, h2, w2, cx[ps] * sc,
                          cy[ps] * sc, lane8, act[ps], reinterpret_cast<float*>(stage), LD,
@@ -376,10 +401,19 @@ int goslam_corr_pyramid_lookup(const void* const* pyramid, int dtype, int num_le
 int goslam_corr_pool_lookup(const void* const* pyramid, int dtype, int num_levels, const int* slots,
                             int capacity, int layout, const float* coords_hw2, void* out, int N, int h1,
                             int w1, int h2, int w2, int radius, void* stream) {
+  return goslam_corr_pool_lookup_aliased(pyramid, dtype, num_levels, slots, nullptr, capacity, layout, coords_hw2,
+                                         out, N, h1, w1, h2, w2, radius, stream);
+}
+
+int goslam_corr_pool_lookup_aliased(const void* const* pyramid, int dtype, int num_levels, const int* slots,
+                                    const int* alias, int capacity, int layout, const float* coords_hw2,
+                                    void* out, int N, int h1, int w1, int h2, int w2, int radius,
+                                    void* stream) {
   if (N < 0 || h1 <= 0 || w1 <= 0 || num_levels < 1 || num_levels > kMaxLevels || capacity < N)
     return GOSLAM_EINVAL;
   if (layout != GOSLAM_LAYOUT_ROWMAJOR && layout != GOSLAM_LAYOUT_TILED) return GOSLAM_EINVAL;
   if (layout == GOSLAM_LAYOUT_TILED && dtype != GOSLAM_F16) return GOSLAM_EINVAL;
+  if (alias != nullptr && (layout != GOSLAM_LAYOUT_TILED || h1 != h2 || w1 != w2)) return GOSLAM_EINVAL;
   if (N == 0) return GOSLAM_OK;
   LookupArgs a{};
   for (int i = 0; i < num_levels; ++i) {
@@ -397,7 +431,7 @@ int goslam_corr_pool_lookup(const void* const* pyramid, int dtype, int num_level
     }
   }
   a.num_levels = num_levels; a.coords = coords_hw2; a.interleaved = 1; a.out = out;
-  a.N = N; a.hw1 = h1 * w1; a.radius = radius; a.slot = slots; a.cap = capacity;
+  a.N = N; a.hw1 = h1 * w1; a.radius = radius; a.slot = slots; a.cap = capacity; a.alias = alias;
   if (dtype == GOSLAM_F16) return launch_lookup<__half>(a, (cudaStream_t)stream);
   if (dtype == GOSLAM_F32) return launch_lookup<float>(a, (cudaStream_t)stream);
   return GOSLAM_EINVAL;

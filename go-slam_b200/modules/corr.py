@@ -28,7 +28,14 @@ class CorrPool:
     once (FactorGraph.max_factors is the natural capacity); a CorrBlock built `from_video(...,
     pool=pool)` holds only a table of slot ids, so cat() joins two tables and __getitem__ filters
     one.  The build and lookup kernels follow the table on the device
-    (goslam_corr_pool_build / goslam_corr_pool_lookup)."""
+    (goslam_corr_pool_build_paired / goslam_corr_pool_lookup_aliased).
+
+    Reverse edges share level 0: corr(j,i)[q][p] == corr(i,j)[p][q] bit for bit, so when one build call holds
+    both (i, j) and (j, i) once each, the later one (the reader) writes levels 1-3 only and reads level 0 as
+    the transpose of its partner's.  `alias[s]` (int32, device) = 2 * (slot holding slot s's level 0) + (1 if
+    transposed), in word 0 of a 16-byte row; the build writes it for every slot it fills.  Pairs never cross a build call, so they never
+    cross a block; a block that keeps a reader but lets its partner go materializes the reader's level 0 first
+    (`unalias`).  Every reader still owns its level-0 region, so slot bookkeeping is unchanged."""
 
     TILED = 1                                                    # == GOSLAM_LAYOUT_TILED
 
@@ -44,6 +51,10 @@ class CorrPool:
                        for i in range(num_levels)]
         self._free = list(range(self.capacity - 1, -1, -1))     # stack; slot 0 is handed out first
         self._iota = torch.arange(self.capacity, dtype=torch.int32, device=device)
+        # [capacity, 4]: word 0 of a row is the entry, the 16-byte rows let the build write them with bulk copies
+        self.alias = torch.zeros((self.capacity, 4), dtype=torch.int32, device=device)
+        self.alias[:, 0] = self._iota * 2                        # every slot holds its own level 0
+        self.paired = False                                      # set once a paired build has run
 
     def slot_table(self, slots):
         """device int32 table for a list of slot ids (a view of a resident iota when the ids are a
@@ -61,8 +72,16 @@ class CorrPool:
         return n_yb * ((n_xb * 8 + 15) // 16 * 16) if i == 2 else n_yb * 16
 
     def level_rowmajor(self, i, slots=None):
-        """level i as [n, ht, wd, ht>>i, wd>>i] (a gathered, de-tiled copy; tests / debugging)."""
-        lvl = self.levels[i] if slots is None else self.levels[i][slots]
+        """level i as [n, ht, wd, ht>>i, wd>>i] (a gathered, de-tiled copy; tests / debugging); an aliased level 0
+        is read through `alias`, as the lookup reads it."""
+        if i == 0 and self.paired:
+            slots = self._iota.long() if slots is None else torch.as_tensor(slots, device=self.alias.device).long()
+            al = self.alias[slots, 0].long()
+            own = self._detile(0, self.levels[0][al >> 1])
+            return torch.where((al & 1).bool().view(-1, 1, 1, 1, 1), own.permute(0, 3, 4, 1, 2), own).contiguous()
+        return self._detile(i, self.levels[i] if slots is None else self.levels[i][slots])
+
+    def _detile(self, i, lvl):
         hl, wl = self.ht >> i, self.wd >> i
         n = lvl.shape[0]
         if i < 2:
@@ -103,7 +122,24 @@ class CorrPool:
             self.levels[i] = new
         self._free = list(range(capacity - 1, self.capacity - 1, -1)) + self._free
         self._iota = torch.arange(capacity, dtype=torch.int32, device=dev)
+        alias = torch.zeros((capacity, 4), dtype=torch.int32, device=dev)
+        alias[:self.capacity].copy_(self.alias)                  # live aliases carry over
+        alias[self.capacity:, 0] = self._iota[self.capacity:] * 2
+        self.alias = alias
         self.capacity = capacity
+
+    def unalias(self, slots, keep=lambda holder: False):
+        """give each of `slots` whose level 0 is another slot's transpose its own copy, unless `keep(holder)`
+        (one device kernel; reads the slots' alias entries on the host)."""
+        if not self.paired or not slots:
+            return
+        al = self.alias[self.slot_table(list(slots)).long(), 0].tolist()
+        todo = [(s, a >> 1) for s, a in zip(slots, al) if a & 1 and not keep(a >> 1)]
+        if todo:
+            dev = self.alias.device
+            ss = torch.tensor([s for s, _ in todo], dtype=torch.int32, device=dev)
+            hs = torch.tensor([t for _, t in todo], dtype=torch.int32, device=dev)
+            _lib.call("corr_pool_unalias", self.levels[0], self.alias, ss, hs, len(todo), self.ht, self.wd)
 
 
 class CorrBlock:
@@ -157,8 +193,9 @@ class CorrBlock:
         self.pool = pool
         self._slots_host = pool.alloc(N)
         self.slots = pool.slot_table(self._slots_host)
-        _lib.call("corr_pool_build", fmaps_kmajor, int(fmaps_kmajor.shape[0]), int(rig), ii, jj, self.slots,
-                  _ptr_array(pool.levels), self.num_levels, N, 128, self.ht, self.wd)
+        _lib.call("corr_pool_build_paired", fmaps_kmajor, int(fmaps_kmajor.shape[0]), int(rig), ii, jj, self.slots,
+                  pool.alias, _ptr_array(pool.levels), self.num_levels, N, 128, self.ht, self.wd)
+        pool.paired = pool.paired or N > 1
 
     def __call__(self, coords):
         batch, num, ht, wd, _ = coords.shape
@@ -184,8 +221,8 @@ class CorrBlock:
         coords = coords.reshape(N, ht, wd, 2).contiguous().float()
         out = torch.empty((batch, num, self.num_levels * rd * rd, ht, wd), dtype=torch.float16,
                           device=pool.levels[0].device)
-        _lib.call("corr_pool_lookup", _ptr_array(pool.levels), 1, self.num_levels, self.slots, pool.capacity,
-                  pool.TILED, coords, out, N, ht, wd, pool.ht, pool.wd, int(self.radius))
+        _lib.call("corr_pool_lookup_aliased", _ptr_array(pool.levels), 1, self.num_levels, self.slots, pool.alias,
+                  pool.capacity, pool.TILED, coords, out, N, ht, wd, pool.ht, pool.wd, int(self.radius))
         return out
 
     def cat(self, other):
@@ -202,7 +239,9 @@ class CorrBlock:
         if other.pool is None:
             raise RuntimeError("CorrBlock.cat: a pooled block cannot take the edges of a row-major one")
         # blocks in different pools (e.g. two CorrBlock(f1, f2)): both copied into a new private pool, the
-        # copy the reference's torch.cat makes
+        # copy the reference's torch.cat makes; the raw slot copy needs every level 0 materialized first
+        self.pool.unalias(self._slots_host)
+        other.pool.unalias(other._slots_host)
         n = len(self._slots_host) + len(other._slots_host)
         pool = CorrPool(n, self.ht, self.wd, self.num_levels, device=self.pool.levels[0].device)
         for i, lvl in enumerate(pool.levels):
@@ -224,7 +263,12 @@ class CorrBlock:
         kept = set(keep)
         if len(kept) != len(keep):
             raise RuntimeError("CorrBlock[index]: a pooled block cannot hold one slot twice")
-        self.pool.release(s for i, s in enumerate(self._slots_host) if i not in kept)
+        gone = [s for i, s in enumerate(self._slots_host) if i not in kept]
+        if gone:
+            # a kept reader whose partner goes takes a copy of its level 0 before the partner's slot is reused
+            kept_slots = set(self._slots_host[i] for i in keep)
+            self.pool.unalias([self._slots_host[i] for i in keep], keep=lambda holder: holder in kept_slots)
+        self.pool.release(gone)
         self._slots_host = [self._slots_host[i] for i in keep]
         self.slots = self.pool.slot_table(self._slots_host)
         return self

@@ -110,6 +110,29 @@ int goslam_corr_pool_build(const void* fmaps_kmajor, int F, int rig, const int64
 int goslam_corr_pool_lookup(const void* const* pyramid, int dtype, int num_levels, const int* slots,
                             int capacity, int layout, const float* coords_hw2, void* out, int N,
                             int h1, int w1, int h2, int w2, int radius, void* stream);
+/* Reverse-edge pairing.  corr(j,i)[q][p] = corr(i,j)[p][q], bit for bit (same products, same k order), so
+ * of the two orientations of an edge only one needs its level 0 stored.  alias[capacity][4] (int32, device,
+ * owned with the pool; 16-byte rows, so the build writes them with bulk copies) says where each slot's
+ * level 0 is: alias[s][0] = 2 * t + x, slot t holds it, x = 1 if transposed (2 * s: the slot's own).
+ * goslam_corr_pool_build_paired = goslam_corr_pool_build that pairs the edges of the call on the device:
+ * edge r is the READER of edge e when (ii[r], jj[r]) == (jj[e], ii[e]), ii[e] != jj[e], both orientations
+ * occur exactly once in the call and e < r (calls of more than 512 edges are not paired).  A reader writes
+ * levels 1-3 but not level 0; the build sets alias[] of every slot it writes.  alias == NULL: no pairing,
+ * no table (goslam_corr_pool_build).  Pairs never cross calls, so releasing a whole block orphans nothing.
+ * goslam_corr_pool_lookup_aliased = goslam_corr_pool_lookup (tiled layout, h1 == h2, w1 == w2) that reads
+ * level 0 through alias[]: tap (y, x) of source pixel q of a transposed slot is element q of plane y*w + x
+ * of the holder.  alias == NULL: goslam_corr_pool_lookup.
+ * goslam_corr_pool_unalias gives slots[i] (i < n) its own level 0, the transpose of slot holders[i]'s, and
+ * sets alias[slots[i]][0] = 2 * slots[i]: run before a holder's slot is released while its reader lives on. */
+int goslam_corr_pool_build_paired(const void* fmaps_kmajor, int F, int rig, const int64_t* ii,
+                                  const int64_t* jj, const int* slots, int* alias, void* const* levels,
+                                  int num_levels, int N, int D, int h, int w, void* stream);
+int goslam_corr_pool_lookup_aliased(const void* const* pyramid, int dtype, int num_levels, const int* slots,
+                                    const int* alias, int capacity, int layout, const float* coords_hw2,
+                                    void* out, int N, int h1, int w1, int h2, int w2, int radius,
+                                    void* stream);
+int goslam_corr_pool_unalias(void* level0, int* alias, const int* slots, const int* holders, int n, int h,
+                             int w, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * On-the-fly windowed correlation (no volume).

@@ -1,4 +1,7 @@
-"""time the correlation build for several edge counts (L2-resident vs DRAM-streaming outputs).
+"""time the correlation build for several edge counts (L2-resident vs DRAM-streaming outputs), and for the
+benchmark's |i - j| <= 3 window, whose 36 edges are 18 reverse pairs that store level 0 once per pair.
+"written" is what the build stores (a reader edge's level 0 is its partner's, transposed), "algorithmic" what
+the same edges would store unpaired; the rate is over the written bytes.
 usage: time_build.py [h w]   (default 40 80)"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -14,9 +17,22 @@ h, w = (int(sys.argv[1]), int(sys.argv[2])) if len(sys.argv) > 2 else (40, 80)
 g = torch.Generator().manual_seed(0)
 fm = torch.randn(16, 1, 128, h, w, generator=g).half().to(dev)
 km = fmaps_to_kmajor(fm)
-for N in ((36,) if os.environ.get("TOOL_VARIANT") else (2, 36, 72)):
-    ii = torch.arange(N, device=dev) % 16
-    jj = (torch.arange(N, device=dev) * 7 + 3) % 16
+
+
+def readers(ii, jj):
+    """edges whose level 0 the build does not store: the later edge of a reverse pair (CorrPool)"""
+    e = list(zip(ii.tolist(), jj.tolist()))
+    return sum(1 for r, (a, b) in enumerate(e)
+               if a != b and e.count((a, b)) == 1 and e.count((b, a)) == 1 and e.index((b, a)) < r)
+
+
+fwd = [(i, j) for i in range(8) for j in range(8) if 0 < j - i <= 3]
+window = (torch.tensor([i for i, _ in fwd] + [j for _, j in fwd]), torch.tensor([j for _, j in fwd] + [i for i, _ in fwd]))
+cases = [("no pairs", N, torch.arange(N) % 16, (torch.arange(N) * 7 + 3) % 16) for N in
+         ((36,) if os.environ.get("TOOL_VARIANT") else (2, 36, 72))] + [("window", 36) + window]
+for tag, N, ii, jj in cases:
+    n_rd = readers(ii, jj)
+    ii, jj = ii.to(dev), jj.to(dev)
     pool = CorrPool(N, h, w, device=dev)
 
     def run():
@@ -32,8 +48,10 @@ for N in ((36,) if os.environ.get("TOOL_VARIANT") else (2, 36, 72)):
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 20
     lvl = sum((h >> i) * (w >> i) for i in range(4))
-    gb = N * h * w * lvl * 2 / 1e9
-    print(f"{h}x{w} {'build':8s} N={N:3d} {ms*1e3:8.1f} us  {ms*1e3/N:7.2f} us/edge  out={gb*1e3:7.1f} MB (algorithmic)  {gb/ms*1e3:7.1f} GB/s")
+    alg = N * h * w * lvl * 2 / 1e9
+    gb = alg - n_rd * (h * w) ** 2 * 2 / 1e9
+    print(f"{h}x{w} {'build':8s} N={N:3d} {ms*1e3:8.1f} us  {ms*1e3/N:7.2f} us/edge  out={gb*1e3:7.1f} MB written "
+          f"({alg*1e3:.1f} MB algorithmic, {tag}: {n_rd} readers)  {gb/ms*1e3:7.1f} GB/s")
     # the card's write ceiling beside it: a plain device fill of the same byte count
     buf = torch.empty(int(gb * 1e9) // 2, dtype=torch.half, device=dev)
     for _ in range(3):
