@@ -4,9 +4,10 @@ reproduce single-GPU droid_backends.ba."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import numpy as np
-import torch
-import torch.distributed as dist
+from tools import measure  # noqa: E402
+measure.require_cuda("run_sharded_ba.py")
+import torch  # noqa: E402
+import torch.distributed as dist  # noqa: E402
 
 
 def main():
@@ -14,6 +15,8 @@ def main():
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     dist.init_process_group("nccl", device_id=dev)
+    if rank == 0:
+        measure.emit({})
     from goslam_b200 import droid_backends, parallel, synthetic
     num_kf, ht, wd = 16, 40, 80
     sc, g = synthetic.make_scene(num_kf=num_kf, ht=ht, wd=wd, seed=9, rgbd=True, with_fmaps=False)
@@ -33,14 +36,12 @@ def main():
     p2, d2 = D["poses"].clone(), D["disps"].clone()
     be = parallel.CudaBackend(p2, d2, D["intrinsics"][0].contiguous(), D["disps_sens"], t0, t1)
     torch.cuda.synchronize(); dist.barrier()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    parallel.sharded_ba(be, d2, tg, wg, eta_f, D["ii"], D["jj"], iters, 1e-4, 0.1)
-    e1.record(); torch.cuda.synchronize()
+    t_sharded = measure.cuda_time(lambda: parallel.sharded_ba(be, d2, tg, wg, eta_f, D["ii"], D["jj"], iters, 1e-4, 0.1),
+                                  1, warmup=0)["median_ms"]
     rel = lambda a, b: ((a - b).abs().max() / b.abs().max()).item()   # noqa: E731
     ok = rel(p2, p1) < 1e-5 and rel(d2, d1) < 1e-5
     print("rank %d/%d: poses rel %.2e disps rel %.2e  sharded BA %.1f us  %s" %
-          (rank, world, rel(p2, p1), rel(d2, d1), 1e3 * e0.elapsed_time(e1), "OK" if ok else "MISMATCH"), flush=True)
+          (rank, world, rel(p2, p1), rel(d2, d1), 1e3 * t_sharded, "OK" if ok else "MISMATCH"), flush=True)
     # ---- the same through PEER MEMORY (goslam_ba_phase1_peers / goslam_ba_phase2_peers): no collective per iteration
     for (nk, h, w, lm, ep, its) in ((num_kf, ht, wd, 1e-4, 0.1, iters), (40, 30, 40, 1e-5, 1e-2, 2)):
         sc3, g3 = synthetic.make_scene(num_kf=nk, ht=h, wd=w, seed=11, rgbd=True, with_fmaps=False)
@@ -61,10 +62,8 @@ def main():
         sel = parallel.local_edges(E["ii"], lo, hi)
         tl, wl, il, jl = tg3[sel].contiguous(), wg3[sel].contiguous(), E["ii"][sel].contiguous(), E["jj"][sel].contiguous()
         torch.cuda.synchronize(); dist.barrier()
-        e0.record()
-        for _ in range(its):
-            be3.iteration(tl, wl, ef3, il, jl, lm, ep, False, lo, hi)
-        e1.record()
+        t_peer = measure.cuda_time(lambda: [be3.iteration(tl, wl, ef3, il, jl, lm, ep, False, lo, hi) for _ in range(its)],
+                                   1, warmup=0)["median_ms"]
         link.wait_idle()
         torch.cuda.synchronize()
         db = link.disps.tensor
@@ -74,7 +73,7 @@ def main():
         dist.broadcast(ref_p, src=0); dist.broadcast(ref_d, src=0)
         same = torch.equal(ref_p, pb) and torch.equal(ref_d, db)
         print("rank %d/%d: PEER exchange P=%d %dx%d: poses rel %.2e disps rel %.2e  %d iterations %.1f us  replicas identical %s  %s" %
-              (rank, world, nk - 1, h, w, rel(pb, pa), rel(db, da), its, 1e3 * e0.elapsed_time(e1), same,
+              (rank, world, nk - 1, h, w, rel(pb, pa), rel(db, da), its, 1e3 * t_peer, same,
                "OK" if ok3 and same else "MISMATCH"), flush=True)
         ok = ok and ok3 and same
         link.close()

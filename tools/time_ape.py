@@ -6,29 +6,21 @@ card's name and power limit are read in the same run.
     python tools/time_ape.py [--reps 20] [--out result.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
-
-import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tools import measure  # noqa: E402
+measure.require_cuda("time_ape.py")
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
 from goslam_b200 import slam  # noqa: E402
 
 DEV = torch.device("cuda:0")
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        out = "unknown (%s)" % e
-    return torch.cuda.get_device_name(0), out
 
 
 def inputs(n, seed):
@@ -48,27 +40,13 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--out")
     args = ap.parse_args()
-    name, smi = card()
-    print("card: %s | %s" % (name, smi))
     rows = []
     for n in (2000, 6000, 10 ** 6):
         ref, est = inputs(n, n)
-        for _ in range(3):
-            slam.ape(ref, est)
-        ms = []
-        for _ in range(args.reps):
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            slam.ape(ref, est)
-            b.record()
-            b.synchronize()
-            ms.append(a.elapsed_time(b))
-        rows.append({"n": n, "median_ms": float(np.median(ms)), "min_ms": float(np.min(ms)), "max_ms": float(np.max(ms))})
-        print("n = %8d  ape %.3f ms (min %.3f, max %.3f)" % (n, rows[-1]["median_ms"], rows[-1]["min_ms"],
-                                                                rows[-1]["max_ms"]))
-    if args.out:
-        with open(args.out, "w") as f:
-            json.dump({"card": name, "nvidia_smi": smi, "reps": args.reps, "rows": rows}, f, indent=1)
+        t = measure.cuda_time(lambda: slam.ape(ref, est), args.reps)
+        rows.append({"n": n, "median_ms": t["median_ms"], "min_ms": t["min_ms"], "max_ms": t["max_ms"]})
+        print("n = %8d  ape %.3f ms (min %.3f, max %.3f)" % (n, t["median_ms"], t["min_ms"], t["max_ms"]))
+    measure.emit({"reps": args.reps, "rows": rows}, args.out)
 
 
 if __name__ == "__main__":

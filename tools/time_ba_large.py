@@ -1,10 +1,13 @@
 """CUDA-event timing of droid_backends.ba on global-BA-sized systems (config 4: 64 kf, 30x40, ~384 edges,
-P = 63) and of its phases through the split entry points.  usage: python tools/time_ba_large.py [num_kf ht wd]"""
+P = 63) and of its phases through the split entry points: 5 samples of 20 back-to-back calls.
+usage: python tools/time_ba_large.py [num_kf ht wd]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import torch
-from goslam_b200 import droid_backends, parallel, synthetic
+from tools import measure  # noqa: E402
+measure.require_cuda("time_ba_large.py")
+import torch  # noqa: E402
+from goslam_b200 import droid_backends, parallel, synthetic  # noqa: E402
 
 dev = torch.device("cuda:0")
 num_kf, ht, wd = (int(a) for a in sys.argv[1:4]) if len(sys.argv) >= 4 else (64, 30, 40)
@@ -18,16 +21,9 @@ intr = D["intrinsics"][0].contiguous()
 p0, d0 = D["poses"].clone(), D["disps"].clone()
 
 
-def t(fn, n=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record(); torch.cuda.synchronize()
-    return 1e3 * e0.elapsed_time(e1) / n
+def t(fn):
+    r = measure.cuda_time(fn, reps=5, warmup=3, batch=20)
+    return "%9.1f us (%.1f-%.1f)" % (1e3 * r["median_ms"], 1e3 * r["min_ms"], 1e3 * r["max_ms"])
 
 
 def ba(iters, motion_only=False):
@@ -36,17 +32,18 @@ def ba(iters, motion_only=False):
                       1e-5, 1e-2, motion_only)
 
 
+measure.emit({})
 print("edges %d, P %d, 6P %d, %dx%d" % (D["ii"].numel(), num_kf - 1, 6 * (num_kf - 1), ht, wd))
 for it in (1, 2):
-    print("ba iters=%d              %9.1f us" % (it, t(lambda: ba(it))))
-print("ba motion_only iters=2   %9.1f us" % t(lambda: ba(2, True)))
+    print("ba iters=%d              %s" % (it, t(lambda: ba(it))))
+print("ba motion_only iters=2   %s" % t(lambda: ba(2, True)))
 num = D["disps"].shape[0]
 kx = torch.unique(torch.cat([torch.arange(1, num_kf, device=dev), D["ii"]]))
 eta_f = torch.zeros(num, ht, wd, device=dev)
 eta_f[kx] = eta
 be = parallel.CudaBackend(D["poses"], D["disps"], intr, D["disps_sens"], 1, num_kf)
 sysm = be.phase1(tg, wg, eta_f, D["ii"], D["jj"], False)
-print("phase1 (prep+lin+system) %9.1f us" % t(lambda: be.phase1(tg, wg, eta_f, D["ii"], D["jj"], False)))
+print("phase1 (prep+lin+system) %s" % t(lambda: be.phase1(tg, wg, eta_f, D["ii"], D["jj"], False)))
 
 
 def p2():
@@ -54,4 +51,4 @@ def p2():
     be.phase2(sysm, 1e-5, 1e-2, False, 0, num)
 
 
-print("phase2 (solve+backsub)   %9.1f us" % t(p2))
+print("phase2 (solve+backsub)   %s" % t(p2))

@@ -13,16 +13,17 @@ the card's name and power limit are read in the same run.  Thresholds are the go
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 import types
-
-import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+from tools import measure  # noqa: E402
+measure.require_cuda("time_backend.py")
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
 
 from goslam_b200 import droid_backends, graph as graph_ops, synthetic  # noqa: E402
 from goslam_b200.depth_video import DepthVideo  # noqa: E402
@@ -32,14 +33,6 @@ HT8, WD8 = 48, 64
 BETA = 0.75
 DENSE = dict(radius=1, nms=5, thresh=25.0)
 LOOP = dict(radius=1, nms=12, thresh=25.0, window=25)
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        return "unknown (%s)" % e
 
 
 def make_video(n):
@@ -72,23 +65,13 @@ def select(d, n, p, loop):
                                    t_start_loop=t_start_loop, loop=loop)
 
 
-def timed(fn):
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    r = fn()
-    torch.cuda.synchronize()
-    return time.perf_counter() - t, r
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--sizes", type=int, nargs="+", default=[64, 256, 1024])
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("time_backend: needs a CUDA device")
-    res = {"card": card(), "feature_map": [HT8, WD8], "reps": a.reps, "rows": []}
+    res = {"feature_map": [HT8, WD8], "reps": a.reps, "rows": []}
     for n in a.sizes:
         video = make_video(n)
         for mode, p, loop in (("dense", DENSE, False), ("loop", LOOP, True)):
@@ -111,19 +94,15 @@ def main():
             times = {name: [] for name in paths}
             for _ in range(a.reps):
                 for name, fn in paths.items():
-                    times[name].append(timed(fn)[0])
+                    times[name] += measure.host_time(fn, 1, 0)["samples_ms"]
             row = {"n": n, "mode": mode, "edges": 0 if e_new is None else int(e_new[0].numel()),
                    "pairs_old": (n - r0) * n, "pairs_new": int(torch.isfinite(new_distance(video, r0, n, 0, k)).sum()),
                    "index_bytes_old": 2 * 8 * (n - r0) * n}
             for name, ts in times.items():
-                row[name + "_ms"] = round(1e3 * float(np.median(ts)), 4)
+                row[name + "_ms"] = round(float(np.median(ts)), 4)
             res["rows"].append(row)
             print(json.dumps(row), flush=True)
-    print(json.dumps({"card": res["card"]}))
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
+    measure.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -9,18 +9,18 @@ three add up to a little more than the chunk).  Host clock around work that ends
     python tools/time_filler.py [--reps 10] [--out result.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
-import time
 import types
-
-import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+from tools import measure  # noqa: E402
+measure.require_cuda("time_filler.py")
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
 
 from goslam_b200 import lietorch  # noqa: E402
 from goslam_b200.depth_video import DepthVideo  # noqa: E402
@@ -31,15 +31,6 @@ from goslam_b200.trajectory_filler import PoseTrajectoryFiller, fill_interpolate
 
 DEV = torch.device("cuda:0")
 H, W, BUFFER, NUM_KF, KF_STEP, M = 320, 640, 512, 64, 5, 16
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        out = "unknown (%s)" % e
-    return torch.cuda.get_device_name(0), out
 
 
 def seeded(module, seed):
@@ -111,11 +102,8 @@ def reference_fill(video, net, MEAN, STDV, timestamps, images, depths, intrinsic
 
 
 def wall(fn):
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return 1e3 * (time.perf_counter() - t), out
+    """ms of one synchronised call"""
+    return measure.host_time(fn, 1, 0)["median_ms"]
 
 
 def split(filler, video, chunk):
@@ -144,10 +132,11 @@ def split(filler, video, chunk):
             graph.update(N, N + M, motion_only=True)
 
     video.counter.value += M
+    t01 = []
     try:
-        te, _ = wall(enc)
-        ti, (t0, t1) = wall(interp)
-        tu, _ = wall(lambda: updates(t0, t1))
+        te = wall(enc)
+        ti = wall(lambda: t01.extend(interp()))
+        tu = wall(lambda: updates(*t01))
     finally:
         video.counter.value -= M
     return {"encoder": te, "interp_handover": ti, "updates": tu}
@@ -158,7 +147,6 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    name, smi = card()
     video, net, chunk = setup()
     filler = PoseTrajectoryFiller(net, video, device="cuda:0")
     MEAN, STDV = filler.MEAN, filler.STDV
@@ -174,21 +162,17 @@ def main():
     runs = {"dropin": [], "reference_body": []}
     parts = []
     for _ in range(a.reps):                                            # alternate the two so drift hits both
-        runs["dropin"].append(wall(ours)[0])
-        runs["reference_body"].append(wall(ref)[0])
+        runs["dropin"].append(wall(ours))
+        runs["reference_body"].append(wall(ref))
         parts.append(split(filler, video, chunk))
-    p_ours, p_ref = wall(ours)[1].data, wall(ref)[1].data
+    p_ours, p_ref = ours().data, ref().data
     med = {k: float(np.median(v)) for k, v in runs.items()}
-    res = {"card": name, "nvidia_smi": smi, "shape": [H, W, H // 8, W // 8], "chunk": M, "keyframes": NUM_KF,
+    res = {"shape": [H, W, H // 8, W // 8], "chunk": M, "keyframes": NUM_KF,
            "ms_per_chunk": med, "dropin_split_ms": {k: float(np.median([p[k] for p in parts])) for k in parts[0]},
            "max_pose_diff": float((p_ours - p_ref).abs().max()), "reps": a.reps}
     print("per chunk: drop-in %.2f ms, reference body %.2f ms; split %s; |dpose| %.2e" % (
         med["dropin"], med["reference_body"], res["dropin_split_ms"], res["max_pose_diff"]), flush=True)
-    print(json.dumps(res))
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
+    measure.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -1,11 +1,15 @@
-"""pooled 4-level lookup time per shape (36 edges): python tools/time_lookup.py"""
+"""pooled 4-level lookup time per shape (36 edges), CUDA events around 20 back-to-back lookups, 5 samples:
+python tools/time_lookup.py"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import torch
-from goslam_b200.modules import CorrBlock
-from goslam_b200.modules.corr import CorrPool, fmaps_to_kmajor
+from tools import measure  # noqa: E402
+measure.require_cuda("time_lookup.py")
+import torch  # noqa: E402
+from goslam_b200.modules import CorrBlock  # noqa: E402
+from goslam_b200.modules.corr import CorrPool, fmaps_to_kmajor  # noqa: E402
 dev = torch.device("cuda:0")
+measure.emit({})
 for (h, w, rig) in ((40, 80, 1), (40, 60, 1), (40, 60, 2), (48, 64, 1), (60, 80, 1), (30, 40, 1)):
     g = torch.Generator().manual_seed(0)
     fm = torch.randn(8, rig, 128, h, w, generator=g).half().to(dev)
@@ -21,12 +25,6 @@ for (h, w, rig) in ((40, 80, 1), (40, 60, 1), (40, 60, 2), (48, 64, 1), (60, 80,
             coords = torch.stack([torch.rand(N, h, w, generator=g) * w, torch.rand(N, h, w, generator=g) * h], dim=-1)[None].to(dev)
         else:
             coords = (torch.stack([gx, gy], dim=-1).float()[None, None].expand(1, N, h, w, 2) + off).contiguous().to(dev)
-        for _ in range(3):
-            blk(coords)
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(20):
-            blk(coords)
-        e1.record(); torch.cuda.synchronize()
-        print("%dx%d rig %d %-13s lookup %7.1f us" % (h, w, rig, name, 1e3 * e0.elapsed_time(e1) / 20), flush=True)
+        t = measure.cuda_time(lambda: blk(coords), reps=5, batch=20)
+        print("%dx%d rig %d %-13s lookup %7.1f us (%.1f-%.1f)" % (h, w, rig, name, 1e3 * t["median_ms"], 1e3 * t["min_ms"],
+                                                                  1e3 * t["max_ms"]), flush=True)

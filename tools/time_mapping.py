@@ -1,11 +1,14 @@
-"""kernel-level breakdown of one mapping iteration (forward under grad + loss + backward + AdamW) with torch.profiler.
+"""kernel-level breakdown of one mapping iteration (forward under grad + loss + backward + AdamW): device us per
+iteration by kernel name, from one profiler pass (measure.kernel_times) over 3 iterations.
 usage: time_mapping.py [log2_rays]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import torch
-import bench
-from goslam_b200 import synthetic
+from tools import measure  # noqa: E402
+measure.require_cuda("time_mapping.py")
+import torch  # noqa: E402
+import bench  # noqa: E402
+from goslam_b200 import synthetic  # noqa: E402
 
 dev = torch.device("cuda:0")
 R = 1 << (int(sys.argv[1]) if len(sys.argv) > 1 else 16)
@@ -32,10 +35,8 @@ def step():
 
 for _ in range(3):
     step()
-torch.cuda.synchronize()
-from torch.profiler import profile, ProfilerActivity
-with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
-    for _ in range(3):
-        step()
-    torch.cuda.synchronize()
-print(prof.key_averages().table(sort_by="cuda_time_total", row_limit=28, max_name_column_width=70))
+us = measure.kernel_times(step, steps=3)
+measure.emit({})
+for name, t in sorted(us.items(), key=lambda kv: -kv[1])[:28]:
+    print("%9.1f us  %5.1f launches  %s" % (t, us.launches[name], name[:70]))
+print("%9.1f us  total kernel time per iteration" % sum(us.values()))

@@ -9,11 +9,12 @@ on a trained_like net, at the mesher's resolutions.  CUDA events per stage, medi
 usage: python tools/time_mesh.py [res ...]        (default 256 512 1024)"""
 import ctypes
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tools import measure  # noqa: E402
+measure.require_cuda("time_mesh.py")
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
@@ -22,12 +23,6 @@ from goslam_b200 import _lib, neus, synthetic  # noqa: E402
 dev = torch.device("cuda:0")
 BOUND = [[-2.0, 1.5], [-1.2, 1.8], [-1.0, 2.2]]
 RT_BOUND = [[-1.7, 1.3], [-1.0, 1.6], [-0.8, 2.0]]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True).stdout.strip()
-    return q or torch.cuda.get_device_name(0)
 
 
 def make_net():
@@ -46,12 +41,9 @@ def make_net():
 
 
 def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    e1.synchronize()
-    return out, e0.elapsed_time(e1)
+    """fn's result and the ms of that one call"""
+    out = []
+    return out, measure.cuda_time(lambda: out.append(fn()), 1, warmup=0)["median_ms"]
 
 
 def one_pass(net, res):
@@ -61,7 +53,7 @@ def one_pass(net, res):
     b = net.bound.cpu().tolist()
     bmin, bmax = [x[0] for x in b], [x[1] for x in b]
     ms = {}
-    u, ms["field"] = timed(lambda: net._sdf_grid(bmin, bmax, res))
+    (u,), ms["field"] = timed(lambda: net._sdf_grid(bmin, bmax, res))
     ws = torch.empty(lib.goslam_mc_workspace_bytes(res, res, res), dtype=torch.uint8, device=dev)
     counts = torch.empty(2, dtype=torch.int64, device=dev)
     _, ms["count"] = timed(lambda: _lib.check(lib.goslam_mc_count(_lib.ptr(u), res, res, res, 0.0, _lib.ptr(ws), ws.numel(),
@@ -74,9 +66,9 @@ def one_pass(net, res):
                                                                  _lib.ptr(verts), nv, _lib.ptr(faces), nf, st), "mc_emit"))
     del ws, u
     rt = np.array(net.realtime_bound.cpu().numpy(), np.float32)
-    (cv, cf), ms["cull"] = timed(lambda: neus.cull_mesh(verts, faces, (rt[:, 0] - 0.01).tolist(), (rt[:, 1] + 0.01).tolist()))
+    ((cv, cf),), ms["cull"] = timed(lambda: neus.cull_mesh(verts, faces, (rt[:, 0] - 0.01).tolist(), (rt[:, 1] + 0.01).tolist()))
     flat = sum(b, [])
-    rgb, ms["colour"] = timed(lambda: net._vertex_colors(cv, flat))
+    (rgb,), ms["colour"] = timed(lambda: net._vertex_colors(cv, flat))
     host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (cv, cf, rgb)]
 
     def copy():
@@ -92,13 +84,13 @@ def marcher_rate(net):
     with torch.no_grad():
         for _ in range(2):
             net(ro, rd, zv, ds)
-        times = [timed(lambda: net(ro, rd, zv, ds))[1] for _ in range(5)]
-    return zv.numel() / (np.median(times) * 1e-3)
+        t = measure.cuda_time(lambda: net(ro, rd, zv, ds), 5, warmup=0)
+    return zv.numel() / (t["median_ms"] * 1e-3)
 
 
 def main():
     resolutions = [int(a) for a in sys.argv[1:]] or [256, 512, 1024]
-    print("card: %s" % card())
+    measure.emit({})
     net = make_net()
     rate = marcher_rate(net)
     print("marcher: %.3g samples/s (2^16 rays x 72 samples)" % rate)

@@ -11,17 +11,17 @@ same run.
     python tools/time_render_eval.py [--reps 20] [--out result.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 import types
 
-import numpy as np
-import torch
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+from tools import measure  # noqa: E402
+measure.require_cuda("time_render_eval.py")
+
+import torch  # noqa: E402
 
 from goslam_b200 import lietorch, render_eval  # noqa: E402
 
@@ -29,28 +29,9 @@ DEV = torch.device("cuda:0")
 BYTES_PER_PIXEL = 32
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:  # noqa: BLE001
-        out = "unknown (%s)" % e
-    return torch.cuda.get_device_name(0), out
-
-
 def timed(fn, reps, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ms.append(a.elapsed_time(b))
-    return float(np.median(ms)), float(np.min(ms)), float(np.max(ms))
+    t = measure.cuda_time(fn, reps, warmup)
+    return t["median_ms"], t["min_ms"], t["max_ms"]
 
 
 def metrics_inputs(K, H, W, seed):
@@ -68,8 +49,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--out")
     args = ap.parse_args()
-    name, smi = card()
-    print("card: %s | %s" % (name, smi))
+    measure.emit({})
     rows = []
     for K, H, W in ((100, 320, 640), (100, 480, 640)):
         inp = metrics_inputs(K, H, W, 1)
@@ -96,9 +76,7 @@ def main():
     rows.append({"what": "eval_render", "K": n, "H": H, "W": W, "median_ms_per_frame": med / n,
                  "min_ms_per_frame": lo / n, "max_ms_per_frame": hi / n})
     print("eval_render %d views %dx%d: %.2f ms per frame (min %.2f, max %.2f)" % (n, H, W, med / n, lo / n, hi / n))
-    if args.out:
-        with open(args.out, "w") as f:
-            json.dump({"card": name, "nvidia_smi": smi, "reps": args.reps, "rows": rows}, f, indent=1)
+    measure.emit({"reps": args.reps, "rows": rows}, args.out)
 
 
 if __name__ == "__main__":

@@ -1,11 +1,14 @@
 """goslam_b200.droid_net.UpdateModule at the config-2 update size (36 edges, 40x80) against the reference forward in
-torch / cuDNN under autocast; per-kernel times: ncu launch list of tools/profile_update_op.py."""
-import os, sys, time
+torch / cuDNN under autocast.  GPU: CUDA events around 20 back-to-back calls, 5 samples; wall: host clock around the
+same 20 calls and a device synchronise.  Per-kernel times: tools/measure.py's kernel_times, as tools/profile_step.py
+uses it."""
+import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import torch
-from goslam_b200.droid_net import UpdateModule, _nhwc_view
-from goslam_b200.modules.gru import conv2d_nhwc, to_nchw, to_nhwc, to_nhwc_padded
+from tools import measure  # noqa: E402
+measure.require_cuda("time_update_op.py")
+import torch  # noqa: E402
+from goslam_b200.droid_net import UpdateModule  # noqa: E402
 
 dev = torch.device("cuda:0")
 B, h, w = 36, 40, 80
@@ -20,22 +23,16 @@ ii = (torch.arange(B) // 5).to(dev)
 jj = ((torch.arange(B) + 1) % 8).to(dev)
 
 
-def t(fn, n=20, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0 = time.perf_counter()
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record(); torch.cuda.synchronize()
-    return 1e3 * e0.elapsed_time(e1) / n, 1e6 * (time.perf_counter() - t0) / n
+def t(name, fn, n=20):
+    gpu = measure.cuda_time(fn, reps=5, batch=n)
+    wall = measure.host_time(lambda: [fn() for _ in range(n)], reps=5, warmup=0)
+    print("%-38s GPU %8.1f us (%.1f-%.1f)   wall %8.1f us (%.1f-%.1f)" % (
+        name, 1e3 * gpu["median_ms"], 1e3 * gpu["min_ms"], 1e3 * gpu["max_ms"],
+        1e3 * wall["median_ms"] / n, 1e3 * wall["min_ms"] / n, 1e3 * wall["max_ms"] / n))
 
 
-for name, fn in [("whole forward (one library call)", lambda: m(net, inp, corr, flow, ii, jj))]:
-    gpu_us, wall_us = t(fn)
-    print("%-38s GPU %8.1f us   wall %8.1f us" % (name, gpu_us, wall_us))
+measure.emit({})
+t("whole forward (one library call)", lambda: m(net, inp, corr, flow, ii, jj))
 
 
 def torch_reference_forward():
@@ -58,5 +55,4 @@ def torch_reference_forward():
         return n2, delta, weight, eta, upmask
 
 
-gpu_us, wall_us = t(torch_reference_forward)
-print("%-38s GPU %8.1f us   wall %8.1f us" % ("torch/cuDNN autocast reference forward", gpu_us, wall_us))
+t("torch/cuDNN autocast reference forward", torch_reference_forward)
